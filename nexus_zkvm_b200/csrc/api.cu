@@ -62,7 +62,6 @@ void nb200_ctx_destroy(nb200_ctx* ctx) {
   cudaSetDevice(ctx->device);
   comm_release(ctx);
   fft_drop_tables(ctx);
-  fft_fused_release(ctx);
   if (ctx->tw.d_tw) cudaFree(ctx->tw.d_tw);
   if (ctx->tw.d_itw) cudaFree(ctx->tw.d_itw);
   if (ctx->tw.d_tw2) cudaFree(ctx->tw.d_tw2);

@@ -39,7 +39,6 @@ struct NcclApi {
   ncclResult_t (*AllGather)(const void*, void*, size_t, ncclDataType_t, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*Send)(const void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*Recv)(void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
-  ncclResult_t (*Broadcast)(const void*, void*, size_t, ncclDataType_t, int, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*AllReduce)(const void*, void*, size_t, ncclDataType_t, ncclRedOp_t, ncclComm_t, cudaStream_t) = nullptr;
   ncclResult_t (*GroupStart)() = nullptr;
   ncclResult_t (*GroupEnd)() = nullptr;
@@ -58,7 +57,7 @@ static NcclApi& nccl() {
   if (!a.h) a.h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
   if (!a.h) return a;
 #define NB_SYM(f) a.f = (decltype(a.f))dlsym(a.h, "nccl" #f); if (!a.f) return a;
-  NB_SYM(GetUniqueId) NB_SYM(CommInitRank) NB_SYM(CommDestroy) NB_SYM(AllGather) NB_SYM(Send) NB_SYM(Recv) NB_SYM(Broadcast) NB_SYM(AllReduce) NB_SYM(GroupStart) NB_SYM(GroupEnd) NB_SYM(GetErrorString)
+  NB_SYM(GetUniqueId) NB_SYM(CommInitRank) NB_SYM(CommDestroy) NB_SYM(AllGather) NB_SYM(Send) NB_SYM(Recv) NB_SYM(AllReduce) NB_SYM(GroupStart) NB_SYM(GroupEnd) NB_SYM(GetErrorString)
 #undef NB_SYM
   a.ok = true;
   return a;
@@ -295,42 +294,6 @@ nb200_status exchange_cols_to_rows_chunk(nb200_ctx* ctx, cudaStream_t st, const 
   return NB200_OK;
 }
 
-// columns -> rows: `src` = this rank's `count` columns (its shard_range of `total`) of LEN words each; `dst_rows` = all `total` columns restricted to
-// this rank's LEN / world rows.  One strided D2D pack per peer, grouped ncclSend / ncclRecv; a peer's block lands in place (its columns are adjacent).
-nb200_status exchange_cols_to_rows(nb200_ctx* ctx, const u32* src, size_t total, size_t LEN, u32* dst_rows) {
-  Comm* c = (Comm*)ctx->comm;
-  const int world = c ? c->world : 1, rank = c ? c->rank : 0;
-  const size_t S = LEN / world;
-  size_t first = 0, count = 0;
-  shard_range(total, world, rank, &first, &count);
-  if (count) NB_CUDA(ctx, cudaMemcpy2DAsync(dst_rows + first * S, S * 4, src + (size_t)rank * S, LEN * 4, S * 4, count, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (world == 1) return NB200_OK;
-  u32* pack = nullptr;
-  if (count) NB_CUDA(ctx, dmalloc(ctx, (void**)&pack, (size_t)(world - 1) * count * S * 4));
-  nb200_status st = NB200_OK;
-  size_t slot = 0;
-  for (int q = 0; q < world && st == NB200_OK; ++q) {
-    if (q == rank || !count) continue;
-    if (cudaMemcpy2DAsync(pack + slot * count * S, S * 4, src + (size_t)q * S, LEN * 4, S * 4, count, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "exchange: pack");
-    ++slot;
-  }
-  if (st == NB200_OK) {
-    ncclResult_t r = nccl().GroupStart();
-    slot = 0;
-    for (int q = 0; q < world && r == ncclSuccess; ++q) {
-      if (q == rank) continue;
-      size_t qf = 0, qc = 0;
-      shard_range(total, world, q, &qf, &qc);
-      if (count) { r = nccl().Send(pack + slot * count * S, count * S, ncclUint32, q, c->comm, ctx->stream); ++slot; }
-      if (r == ncclSuccess && qc) r = nccl().Recv(dst_rows + qf * S, qc * S, ncclUint32, q, c->comm, ctx->stream);
-    }
-    ncclResult_t r2 = nccl().GroupEnd();
-    if (r != ncclSuccess || r2 != ncclSuccess) st = set_err(ctx, NB200_ERR_CUDA, std::string("exchange cols->rows: ") + nccl().GetErrorString(r != ncclSuccess ? r : r2));
-  }
-  dfree(ctx, pack);
-  return st;
-}
-
 // rows -> columns (the inverse): `src_rows` = all `total` columns x this rank's S rows; `dst` = this rank's columns, LEN words each.
 nb200_status exchange_rows_to_cols(nb200_ctx* ctx, const u32* src_rows, size_t total, size_t LEN, u32* dst) {
   Comm* c = (Comm*)ctx->comm;
@@ -369,12 +332,6 @@ nb200_status comm_all_gather_dev(nb200_ctx* ctx, const u32* mine, size_t words, 
   Comm* c = (Comm*)ctx->comm;
   if (!c) { if (mine != out) NB_CUDA(ctx, cudaMemcpyAsync(out, mine, words * 4, cudaMemcpyDeviceToDevice, ctx->stream)); return NB200_OK; }
   NB_NCCL(ctx, nccl().AllGather(mine, out, words, ncclUint32, c->comm, ctx->stream));
-  return NB200_OK;
-}
-nb200_status comm_broadcast_dev(nb200_ctx* ctx, u32* buf, size_t words, int root, cudaStream_t st) {
-  Comm* c = (Comm*)ctx->comm;
-  if (!c) return NB200_OK;
-  NB_NCCL(ctx, nccl().Broadcast(buf, buf, words, ncclUint32, root, c->comm, st ? st : ctx->stream));
   return NB200_OK;
 }
 // element-wise sum of u32 words over the ranks (used where exactly one rank contributes a non-zero word: gathers of owned values)

@@ -40,9 +40,6 @@ struct nb200_ctx {
   void* h_pinned = nullptr;
   size_t h_pinned_bytes = 0;
   void* fft_tables = nullptr;          // per-ctx circle-twiddle tables (fft.cu)
-  // column-chunk pipeline of the commit transforms (fft_fused.cu): side streams + events, created on first use
-  cudaStream_t chunk_stream[2] = {nullptr, nullptr};
-  cudaEvent_t chunk_ev[3] = {nullptr, nullptr, nullptr};
   void* comm = nullptr;                // NCCL communicator state (comm.cu), nullptr = single GPU
   size_t total_mem = 0;                // device memory (bytes), read once at ctx creation
   size_t live_bytes = 0;               // bytes held by nb200_cols batches of this ctx (the dominant allocations): the library's own accounting —
@@ -126,17 +123,14 @@ struct RowScatter { int world = 1; u32 log_slice = 0; size_t col0 = 0; u32* lde_
 nb200_status commit_transforms(nb200_ctx* ctx, const u32* evals, u32* coeffs, u32* lde, u32* half_ext, size_t n_cols, u32 log_size, u32 log_blowup,
                                const RowScatter* scatter = nullptr, bool* scattered = nullptr);
 bool commit_transforms_can_scatter(u32 n, u32 bl, u32 log_slice, int world);
-void fft_fused_release(nb200_ctx* ctx);
 // ---- multi-GPU plumbing (comm.cu): NCCL over the ranks that prove one trace together; all no-ops / local copies without a communicator
 void comm_release(nb200_ctx* ctx);
 int comm_rank(const nb200_ctx* ctx);
 int comm_world(const nb200_ctx* ctx);
 int comm_log_world(const nb200_ctx* ctx);
 void comm_shard_range(size_t total, int world, int rank, size_t* first, size_t* count);
-nb200_status exchange_cols_to_rows(nb200_ctx* ctx, const u32* src, size_t total, size_t LEN, u32* dst_rows);
 nb200_status exchange_rows_to_cols(nb200_ctx* ctx, const u32* src_rows, size_t total, size_t LEN, u32* dst);
 nb200_status comm_all_gather_dev(nb200_ctx* ctx, const u32* mine, size_t words, u32* out);
-nb200_status comm_broadcast_dev(nb200_ctx* ctx, u32* buf, size_t words, int root, cudaStream_t st = nullptr);
 // symmetric peer heap (CUDA IPC over NVLink): see comm.cu
 struct PeerBuf { u32* d = nullptr; int seg = -1; size_t off = 0; };
 nb200_status peer_alloc(nb200_ctx* ctx, const void* owner, size_t words, PeerBuf* out);

@@ -403,22 +403,11 @@ nb200_status expand_reorder(nb200_ctx* ctx, const void* src, u32 elem_bytes, u32
 }
 
 // ---- circle-twiddle tables (layer 0 of each transform size), owned by the ctx (freed in nb200_ctx_destroy) ----
-struct CircleTables { std::map<u32, std::pair<u32*, u32*>> by_log, prod_by_log; };
-// doubled product of the circle twiddle h with line layer 1's twiddle h >> 1 (negated for odd h): the radix-4 pairing of layers (1, 0)
-__global__ void circle_product_kernel(const u32* __restrict__ tw, u32 tw_len, u32 n, u32* __restrict__ out) {
-  u32 h = blockIdx.x * blockDim.x + threadIdx.x;
-  if (h >= (1u << (n - 1))) return;
-  u32 c = circle_tw(tw, tw_len, n, h);
-  u32 l1 = (n >= 2) ? line_tw(tw, tw_len, n, 1, h >> 1) : 1u;
-  u32 p = m31_mul(c, l1);
-  if (h & 1u) p = m31_neg(p);
-  out[h] = p << 1;
-}
+struct CircleTables { std::map<u32, std::pair<u32*, u32*>> by_log; };
 void fft_drop_tables(nb200_ctx* ctx) {
   CircleTables* ct = (CircleTables*)ctx->fft_tables;
   if (!ct) return;
   for (auto& kv : ct->by_log) { cudaFree(kv.second.first); cudaFree(kv.second.second); }
-  for (auto& kv : ct->prod_by_log) { cudaFree(kv.second.first); cudaFree(kv.second.second); }
   delete ct;
   ctx->fft_tables = nullptr;
 }
@@ -442,26 +431,6 @@ nb200_status fft_circle_tables(nb200_ctx* ctx, u32 n, const u32** fwd, const u32
   return NB200_OK;
 }
 
-nb200_status fft_circle_product_tables(nb200_ctx* ctx, u32 n, const u32** fwd, const u32** inv) {
-  if (!ctx->fft_tables) ctx->fft_tables = new CircleTables();
-  CircleTables& ct = *(CircleTables*)ctx->fft_tables;
-  auto it = ct.prod_by_log.find(n);
-  if (it == ct.prod_by_log.end()) {
-    u32 *f = nullptr, *g = nullptr;
-    size_t len = (size_t)1 << (n - 1);
-    NB_CUDA(ctx, cudaMalloc(&f, len * 4));
-    if (cudaMalloc(&g, len * 4) != cudaSuccess) { cudaFree(f); cudaGetLastError(); return set_err(ctx, NB200_ERR_OOM, "circle product tables"); }
-    u32 thr = 256, blk = (u32)((len + thr - 1) / thr);
-    circle_product_kernel<<<blk, thr, 0, ctx->stream>>>(ctx->tw.d_tw, 1u << ctx->tw.half_log, n, f);
-    NB_LAUNCH_CHECK(ctx);
-    circle_product_kernel<<<blk, thr, 0, ctx->stream>>>(ctx->tw.d_itw, 1u << ctx->tw.half_log, n, g);
-    NB_LAUNCH_CHECK(ctx);
-    it = ct.prod_by_log.emplace(n, std::make_pair(f, g)).first;
-  }
-  *fwd = it->second.first; *inv = it->second.second;
-  return NB200_OK;
-}
-
 // ---- pass planning ----
 struct PassPlan { u32 lo, T, W; };
 static void plan_passes(u32 n, std::vector<PassPlan>& out) {
@@ -476,7 +445,6 @@ static void plan_passes(u32 n, std::vector<PassPlan>& out) {
   // the 12-layer contiguous kernel (4 columns per CTA, 3 CTAs/SM) is the most efficient one: prefer it when the strided passes can
   // absorb the extra layer (a 9-layer strided pass applies its top layer while staging, see FUSE_TOP): 2^21 = 12 + 9
   if (LA == 13 && n - 12 <= 9 * npass) LA = 12;
-  if (const char* e = getenv("NB200_FFT_LA")) { u32 v = (u32)atoi(e); if (v >= 9 && v <= 13 && n - v <= 9 * npass && n > v) LA = v; }  // tuning knob
   out.push_back(PassPlan{0, LA, 0});
   u32 rest = n - LA, lo = LA;
   for (u32 k = 0; k < npass; ++k) {
@@ -490,8 +458,7 @@ static void plan_passes(u32 n, std::vector<PassPlan>& out) {
 template <bool INV, int T, int W, int CB, int NZ>
 static nb200_status launch_tile(nb200_ctx* ctx, const FftPass& p) {
   constexpr int threads = 1 << (T - 4);
-  static const size_t pad = getenv("NB200_FFT_PAD_SMEM") ? (size_t)atoi(getenv("NB200_FFT_PAD_SMEM")) * 1024 : 0;   // occupancy experiments
-  const size_t smem = ((size_t)CB << (T + 2)) + pad;
+  constexpr size_t smem = (size_t)CB << (T + 2);
   static bool attr_set[NB_MAX_DEVICES] = {false};   // cudaFuncSetAttribute is per device
   if (!attr_set[ctx->device % NB_MAX_DEVICES]) {
     NB_CUDA(ctx, cudaFuncSetAttribute(fft_tile_kernel<INV, T, W, CB, NZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

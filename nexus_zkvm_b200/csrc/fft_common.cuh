@@ -172,7 +172,5 @@ __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_gr
 
 // circle (layer 0) twiddle tables of a transform size, cached per ctx (fft.cu)
 nb200_status fft_circle_tables(nb200_ctx* ctx, u32 n, const u32** fwd, const u32** inv);
-// the product tables of the circle layer with line layer 1 (radix16p), same indexing as the circle tables
-nb200_status fft_circle_product_tables(nb200_ctx* ctx, u32 n, const u32** fwd, const u32** inv);
 
 }  // namespace nb

@@ -12,9 +12,7 @@
 //   C  fft_tile_async_kernel<FWD>   layers LA-1..0 of each forward transform, contiguous tiles       read 8 B   write 8 B
 //
 // per trace element — 40 B against the 44 B of four independent passes, one launch and one global->shared staging less,
-// and none of B's forward inputs is ever read from memory.  By default each kernel is launched once over the whole batch.  Cutting the
-// batch into column chunks whose intermediates (A's output, B's LDE output) stay in L2 until the next kernel consumes them, with chunks
-// alternating between two streams, is opt-in (NB200_FFT_CHUNK_MIB): whole-batch launches avoid the chunks' tail waves.
+// and none of B's forward inputs is ever read from memory.
 //
 // Staging uses cp.async (LDGSTS.128) with one commit group per column: the first radix-16 round of column c starts as soon
 // as ITS tile has landed while the tiles of the later columns are still in flight, instead of every column waiting for the
@@ -22,7 +20,6 @@
 // Butterfly network, twiddle addressing and the shared-memory swizzle are those of fft.cu, so results are bit-identical
 // to the per-pass kernels: tests/test_gpu_bench_size_parity.py, tests/test_gpu_commit_parity.py.
 #include "fft_common.cuh"
-#include <cstdlib>
 #include <type_traits>
 
 namespace nb {
@@ -93,11 +90,12 @@ __device__ __forceinline__ void stage_out(const TileGeo<T, W>& geo, const u32* s
 // One radix-16 round (<= 4 butterfly layers) over the CB column tiles of a CTA: column c is read at sm_src + c*2^T and written at
 // sm_dst + c*2^T (equal pointers = in place).  RI = position of the round inside the pass (0 = lowest layers), as in fft.cu.
 // SCALE: multiply the outputs by sc2/2 (the 2^-n of interpolate).  WAITC: this is the first round after an asynchronous stage-in.
-// PROD: full 4-layer rounds run as two radix-4 steps with product twiddles (fft_common.cuh radix16p; ptw2 / cptw2 = product bank / circle product table).
+// PROD: full 4-layer rounds run as two radix-4 steps with product twiddles (fft_common.cuh radix16p; ptw2 = product bank).
 template <bool INV, int T, int W, int CB, int RI, bool SCALE, bool WAITC, int NZ, bool PROD = false>
 __device__ __forceinline__ void tile_round(const u32* __restrict__ tw2, const u32* __restrict__ ctw2, const u32 tw_len, const u32 tn, const u32 lo,
                                            const u32 tile_hi, const u32* sm_src, u32* sm_dst, const u32 ncb, const u32 sc2,
-                                           const u32* __restrict__ ptw2 = nullptr, const u32* __restrict__ cptw2 = nullptr) {
+                                           const u32* __restrict__ ptw2 = nullptr) {
+  static_assert(!PROD || W > 0, "product twiddles of the circle layer (W == 0) have no table");
   constexpr int L = T - W, NFULL = L / 4, REM = L % 4;
   constexpr int b = RI < NFULL ? W + 4 * RI : T - 4;
   constexpr int jlo = RI < NFULL ? 0 : 4 - REM;
@@ -135,7 +133,7 @@ __device__ __forceinline__ void tile_round(const u32* __restrict__ tw2, const u3
   if (USEP) {
     {
       const u32 hbase = (tile_hi << (L - (b - W) - 1)) | (tau_hi << 3);
-      const u32* __restrict__ src = (W == 0 && b == 0) ? (cptw2 + hbase) : (ptw2 + (tw_len - (1u << (tn - (lo + b - W)))) + hbase);
+      const u32* __restrict__ src = ptw2 + (tw_len - (1u << (tn - (lo + b - W)))) + hbase;
       uint4 a = __ldg(reinterpret_cast<const uint4*>(src)), c4 = __ldg(reinterpret_cast<const uint4*>(src) + 1);
       pt[0] = a.x; pt[1] = a.y; pt[2] = a.z; pt[3] = a.w; pt[4] = c4.x; pt[5] = c4.y; pt[6] = c4.z; pt[7] = c4.w;
     }
@@ -202,8 +200,8 @@ __device__ __forceinline__ void tile_round(const u32* __restrict__ tw2, const u3
 // ================================================================================================================
 // A / C: one pass over a contiguous-or-strided tile with asynchronous staging (same work as fft.cu's fft_tile_kernel)
 // ================================================================================================================
-template <bool INV, int T, int W, int CB, int MINB, bool PROD>
-__global__ void __launch_bounds__(1 << (T - 4), MINB) fft_tile_async_kernel(const FftPass p, const u32* __restrict__ ptw2, const u32* __restrict__ cptw2) {
+template <bool INV, int T, int W, int CB, int MINB>
+__global__ void __launch_bounds__(1 << (T - 4), MINB) fft_tile_async_kernel(const FftPass p) {
   extern __shared__ __align__(16) u32 sm[];
   constexpr int L = T - W;
   constexpr int NROUNDS = L / 4 + ((L % 4) ? 1 : 0);
@@ -220,7 +218,7 @@ __global__ void __launch_bounds__(1 << (T - 4), MINB) fft_tile_async_kernel(cons
   static_for<0, NROUNDS>([&](auto rr) {   // (the 2^-n scaling of interpolate is applied by fft_mid_kernel)
     constexpr int RR = decltype(rr)::value;
     constexpr int RI = INV ? RR : NROUNDS - 1 - RR;
-    tile_round<INV, T, W, CB, RI, false, RR == 0, 0, PROD>(p.tw2, p.ctw2, p.tw_len, p.tn, lo, tile_hi, sm, sm, ncb, 0u, ptw2, cptw2);
+    tile_round<INV, T, W, CB, RI, false, RR == 0, 0>(p.tw2, p.ctw2, p.tw_len, p.tn, lo, tile_hi, sm, sm, ncb, 0u);
     __syncthreads();
   });
   if (W == 0 && p.shard_log) {
@@ -269,7 +267,7 @@ __global__ void __launch_bounds__(1 << (T - 4), MINB) fft_mid_kernel(const FftMi
   // ---- inverse layers lo..n-1, scaled: S0 = coefficients
   static_for<0, NROUNDS>([&](auto rr) {
     constexpr int RR = decltype(rr)::value;
-    tile_round<true, T, W, CB, RR, RR == NROUNDS - 1, RR == 0, 0, PROD>(p.itw2, nullptr, p.tw_len, p.n, lo, tile_hi, S0, S0, ncb, p.sc2, p.iptw2, nullptr);
+    tile_round<true, T, W, CB, RR, RR == NROUNDS - 1, RR == 0, 0, PROD>(p.itw2, nullptr, p.tw_len, p.n, lo, tile_hi, S0, S0, ncb, p.sc2, p.iptw2);
     __syncthreads();
   });
   stage_out<T, W, CB>(geo, S0, p.coeffs, p.coeff_stride, col0, ncb);
@@ -281,7 +279,7 @@ __global__ void __launch_bounds__(1 << (T - 4), MINB) fft_mid_kernel(const FftMi
     static_for<0, NROUNDS>([&](auto rr) {
       constexpr int RR = decltype(rr)::value;
       constexpr int RI = NROUNDS - 1 - RR;
-      tile_round<false, T, W, CB, RI, false, false, 0, PROD>(p.tw2, nullptr, p.tw_len, ftn, lo, fhi, RR == 0 ? S0 : S1, S1, ncb, 0u, p.ptw2, nullptr);
+      tile_round<false, T, W, CB, RI, false, false, 0, PROD>(p.tw2, nullptr, p.tw_len, ftn, lo, fhi, RR == 0 ? S0 : S1, S1, ncb, 0u, p.ptw2);
       __syncthreads();
     });
     stage_out<T, W, CB>(geo, S1, p.fdst[f], p.fstride[f], col0, ncb);
@@ -301,8 +299,8 @@ static nb200_status set_smem(nb200_ctx* ctx, K kernel, size_t smem, bool* flags)
   return NB200_OK;
 }
 
-template <bool INV, int T, int CB, int MINB, bool PROD = false>
-static nb200_status launch_contig(nb200_ctx* ctx, cudaStream_t st, const u32* src, size_t src_stride, u32* dst, size_t dst_stride, size_t n_cols, u32 n, u32 tn,
+template <bool INV, int T, int CB, int MINB>
+static nb200_status launch_contig(nb200_ctx* ctx, const u32* src, size_t src_stride, u32* dst, size_t dst_stride, size_t n_cols, u32 n, u32 tn,
                                   const RowScatter* sc = nullptr, int which = 0) {
   FftPass p;
   p.shard_log = 0; p.shard_col0 = 0;
@@ -322,22 +320,20 @@ static nb200_status launch_contig(nb200_ctx* ctx, cudaStream_t st, const u32* sr
   p.n_cols = (u32)n_cols; p.n = n; p.lo = 0; p.T = T; p.W = 0; p.cb = CB; p.scale = 0; p.apply_scale = 0; p.tn = tn; p.ztop = n;
   constexpr size_t smem = (size_t)CB << (T + 2);
   static bool flags[NB_MAX_DEVICES] = {false};
-  const u32 *pf = nullptr, *pi = nullptr;
-  if (PROD) NB_TRY(fft_circle_product_tables(ctx, tn, &pf, &pi));
-  NB_TRY(set_smem(ctx, fft_tile_async_kernel<INV, T, 0, CB, MINB, PROD>, smem, flags));
+  NB_TRY(set_smem(ctx, fft_tile_async_kernel<INV, T, 0, CB, MINB>, smem, flags));
   dim3 grid(1u << (n - T), (u32)((n_cols + CB - 1) / CB));
-  fft_tile_async_kernel<INV, T, 0, CB, MINB, PROD><<<grid, 1 << (T - 4), smem, st>>>(p, INV ? ctx->tw.d_iptw2 : ctx->tw.d_ptw2, INV ? pi : pf);
+  fft_tile_async_kernel<INV, T, 0, CB, MINB><<<grid, 1 << (T - 4), smem, ctx->stream>>>(p);
   NB_LAUNCH_CHECK(ctx);
   return NB200_OK;
 }
 
 template <int T, int W, int CB, int MINB, bool PROD = false>
-static nb200_status launch_mid(nb200_ctx* ctx, cudaStream_t st, const FftMid& p) {
+static nb200_status launch_mid(nb200_ctx* ctx, const FftMid& p) {
   constexpr size_t smem = (size_t)2 * CB << (T + 2);
   static bool flags[NB_MAX_DEVICES] = {false};
   NB_TRY(set_smem(ctx, fft_mid_kernel<T, W, CB, MINB, PROD>, smem, flags));
   dim3 grid(1u << (p.n - T), (u32)((p.n_cols + CB - 1) / CB));
-  fft_mid_kernel<T, W, CB, MINB, PROD><<<grid, 1 << (T - 4), smem, st>>>(p);
+  fft_mid_kernel<T, W, CB, MINB, PROD><<<grid, 1 << (T - 4), smem, ctx->stream>>>(p);
   NB_LAUNCH_CHECK(ctx);
   return NB200_OK;
 }
@@ -350,20 +346,10 @@ static bool fused_plan(u32 n, FusedPlan* pl) {
   return true;
 }
 
-static int env_int(const char* name, int dflt) { const char* e = getenv(name); return (e && e[0]) ? atoi(e) : dflt; }
-
 bool fft_fused_supported(u32 n, u32 log_blowup, const void* a, const void* b, const void* c) {
-  static const int mode = env_int("NB200_FFT_FUSED", 1);
   FusedPlan pl;
-  if (!mode || log_blowup < 1 || log_blowup > 2 || !fused_plan(n, &pl)) return false;
+  if (log_blowup < 1 || log_blowup > 2 || !fused_plan(n, &pl)) return false;
   return (((uintptr_t)a | (uintptr_t)b | (uintptr_t)c) & 15u) == 0;
-}
-
-static nb200_status chunk_streams(nb200_ctx* ctx) {
-  if (ctx->chunk_stream[0]) return NB200_OK;
-  for (int i = 0; i < 2; ++i) NB_CUDA(ctx, cudaStreamCreateWithFlags(&ctx->chunk_stream[i], cudaStreamNonBlocking));
-  for (int i = 0; i < 3; ++i) NB_CUDA(ctx, cudaEventCreateWithFlags(&ctx->chunk_ev[i], cudaEventDisableTiming));
-  return NB200_OK;
 }
 
 // evals (n_cols x 2^n, read only) -> coeffs (n_cols x 2^n) and lde (n_cols x 2^(n+bl)); optionally half_ext (n_cols x 2^(n+bl)):
@@ -376,82 +362,41 @@ nb200_status fft_commit_transforms(nb200_ctx* ctx, const u32* evals, u32* coeffs
   NB_ARG(ctx, ctx->tw.d_tw && ctx->tw.half_log + 1 >= (half_ext ? m + 1 : m), "commit transforms: twiddles not prepared for this size");
   NB_ARG(ctx, !half_ext || bl == 1, "commit transforms: the half-coset extension is produced for blow-up 2 only");
   const size_t len = (size_t)1 << n, mlen = (size_t)1 << m;
-  // column chunks: intermediates of a chunk (A's output 4 B, B's forward outputs 8 (+8) B per element) should stay in L2
-  static const int chunk_mib = env_int("NB200_FFT_CHUNK_MIB", 0);   // 0 = whole-batch launches (default); chunking is opt-in
-  static const int two_streams = env_int("NB200_FFT_STREAMS", 2);
-  size_t per_col = len * 4 * (1 + (1u << bl) + (half_ext ? 2 : 0));
-  size_t chunk = chunk_mib > 0 ? std::max<size_t>(4, (((size_t)chunk_mib << 20) / per_col) & ~(size_t)3) : n_cols;
-  if (chunk > n_cols) chunk = n_cols;
-  const bool multi = two_streams >= 2 && n_cols > chunk;
-  if (multi) {
-    NB_TRY(chunk_streams(ctx));
-    NB_CUDA(ctx, cudaEventRecord(ctx->chunk_ev[2], ctx->stream));
-    for (int i = 0; i < 2; ++i) NB_CUDA(ctx, cudaStreamWaitEvent(ctx->chunk_stream[i], ctx->chunk_ev[2], 0));
+  // A
+  if (pl.LA == 12) NB_TRY((launch_contig<true, 12, 4, 3>(ctx, evals, len, coeffs, len, n_cols, n, n)));
+  else NB_TRY((launch_contig<true, 13, 2, 2>(ctx, evals, len, coeffs, len, n_cols, n, n)));
+  // B
+  FftMid p;
+  p.src = coeffs; p.src_stride = len; p.coeffs = coeffs; p.coeff_stride = len;
+  p.itw2 = ctx->tw.d_itw2; p.tw2 = ctx->tw.d_tw2; p.tw_len = 1u << ctx->tw.half_log;
+  p.iptw2 = ctx->tw.d_iptw2; p.ptw2 = ctx->tw.d_ptw2;
+  p.n_cols = (u32)n_cols; p.n = n; p.lo = pl.LA; p.sc2 = m31_inv((u32)(1u << n) % P31) << 1;
+  p.nfwd = 0;
+  for (u32 r = 0; r < (1u << bl); ++r) {
+    p.fdst[p.nfwd] = lde + ((size_t)r << n); p.fstride[p.nfwd] = mlen; p.ftn[p.nfwd] = m; p.fhi[p.nfwd] = r; ++p.nfwd;
   }
-  const u32 sc = m31_inv((u32)(1u << n) % P31);
-  size_t k = 0;
-  for (size_t c0 = 0; c0 < n_cols; c0 += chunk, ++k) {
-    const size_t nc = std::min(chunk, n_cols - c0);
-    cudaStream_t st = multi ? ctx->chunk_stream[k & 1] : ctx->stream;
-    const u32* ev = evals + c0 * len;
-    u32* co = coeffs + c0 * len;
-    // A
-    static const int var_a = env_int("NB200_FFT_VAR_A", 0), var_b = env_int("NB200_FFT_VAR_B", 3), var_c = env_int("NB200_FFT_VAR_C", 0);   // tile-shape variants (profiles/README.md)
-    if (pl.LA == 12) {
-      if (var_a == 1) NB_TRY((launch_contig<true, 12, 3, 4>(ctx, st, ev, len, co, len, nc, n, n)));
-      else if (var_a == 2) NB_TRY((launch_contig<true, 12, 2, 4>(ctx, st, ev, len, co, len, nc, n, n)));
-      else if (var_a == 3) NB_TRY((launch_contig<true, 12, 4, 3, true>(ctx, st, ev, len, co, len, nc, n, n)));
-      else NB_TRY((launch_contig<true, 12, 4, 3>(ctx, st, ev, len, co, len, nc, n, n)));
-    } else NB_TRY((launch_contig<true, 13, 2, 2>(ctx, st, ev, len, co, len, nc, n, n)));
-    // B
-    FftMid p;
-    p.src = co; p.src_stride = len; p.coeffs = co; p.coeff_stride = len;
-    p.itw2 = ctx->tw.d_itw2; p.tw2 = ctx->tw.d_tw2; p.tw_len = 1u << ctx->tw.half_log;
-    p.iptw2 = ctx->tw.d_iptw2; p.ptw2 = ctx->tw.d_ptw2;
-    p.n_cols = (u32)nc; p.n = n; p.lo = pl.LA; p.sc2 = sc << 1;
-    p.nfwd = 0;
-    for (u32 r = 0; r < (1u << bl); ++r) {
-      p.fdst[p.nfwd] = lde + c0 * mlen + ((size_t)r << n); p.fstride[p.nfwd] = mlen; p.ftn[p.nfwd] = m; p.fhi[p.nfwd] = r; ++p.nfwd;
-    }
-    if (half_ext) {
-      for (u32 r = 0; r < 2; ++r) {
-        p.fdst[p.nfwd] = half_ext + c0 * mlen + ((size_t)r << n); p.fstride[p.nfwd] = mlen; p.ftn[p.nfwd] = m + 1; p.fhi[p.nfwd] = r; ++p.nfwd;
-      }
-    }
-    switch (pl.Lm) {
-      case 4: NB_TRY((launch_mid<12, 8, 2, 3>(ctx, st, p))); break;
-      case 5: NB_TRY((launch_mid<12, 7, 2, 3>(ctx, st, p))); break;
-      case 6: NB_TRY((launch_mid<12, 6, 2, 3>(ctx, st, p))); break;
-      case 7: NB_TRY((launch_mid<12, 5, 2, 3>(ctx, st, p))); break;
-      case 8:
-        if (var_b == 1) NB_TRY((launch_mid<12, 4, 1, 4>(ctx, st, p)));
-        else if (var_b == 3) NB_TRY((launch_mid<12, 4, 2, 3, true>(ctx, st, p)));
-        else NB_TRY((launch_mid<12, 4, 2, 3>(ctx, st, p)));
-        break;
-      case 9: NB_TRY((launch_mid<13, 4, 1, 2>(ctx, st, p))); break;
-      default: return set_err(ctx, NB200_ERR_STATE, "commit transforms: plan");
-    }
-    // C: the contiguous low layers of every forward transform (each 2^n-word block is independent below layer n: run them as
-    // one launch over the 2^m-word columns)
-    RowScatter sc_chunk;
-    if (scatter) { sc_chunk = *scatter; sc_chunk.col0 += c0; }
-    const RowScatter* scp = scatter ? &sc_chunk : nullptr;
-    auto fwd_low = [&](u32* buf, u32 tn, int which) -> nb200_status {
-      if (pl.LA != 12) return launch_contig<false, 13, 2, 2>(ctx, st, buf, mlen, buf, mlen, nc, m, tn, scp, which);
-      if (var_c == 1) return launch_contig<false, 12, 3, 4>(ctx, st, buf, mlen, buf, mlen, nc, m, tn, scp, which);
-      if (var_c == 2) return launch_contig<false, 12, 2, 4>(ctx, st, buf, mlen, buf, mlen, nc, m, tn, scp, which);
-      if (var_c == 3) return launch_contig<false, 12, 4, 3, true>(ctx, st, buf, mlen, buf, mlen, nc, m, tn, scp, which);
-      return launch_contig<false, 12, 4, 3>(ctx, st, buf, mlen, buf, mlen, nc, m, tn, scp, which);
-    };
-    NB_TRY(fwd_low(lde + c0 * mlen, m, 0));
-    if (half_ext) NB_TRY(fwd_low(half_ext + c0 * mlen, m + 1, 1));
-  }
-  if (multi) {
-    for (int i = 0; i < 2; ++i) {
-      NB_CUDA(ctx, cudaEventRecord(ctx->chunk_ev[i], ctx->chunk_stream[i]));
-      NB_CUDA(ctx, cudaStreamWaitEvent(ctx->stream, ctx->chunk_ev[i], 0));
+  if (half_ext) {
+    for (u32 r = 0; r < 2; ++r) {
+      p.fdst[p.nfwd] = half_ext + ((size_t)r << n); p.fstride[p.nfwd] = mlen; p.ftn[p.nfwd] = m + 1; p.fhi[p.nfwd] = r; ++p.nfwd;
     }
   }
+  switch (pl.Lm) {
+    case 4: NB_TRY((launch_mid<12, 8, 2, 3>(ctx, p))); break;
+    case 5: NB_TRY((launch_mid<12, 7, 2, 3>(ctx, p))); break;
+    case 6: NB_TRY((launch_mid<12, 6, 2, 3>(ctx, p))); break;
+    case 7: NB_TRY((launch_mid<12, 5, 2, 3>(ctx, p))); break;
+    case 8: NB_TRY((launch_mid<12, 4, 2, 3, true>(ctx, p))); break;
+    case 9: NB_TRY((launch_mid<13, 4, 1, 2>(ctx, p))); break;
+    default: return set_err(ctx, NB200_ERR_STATE, "commit transforms: plan");
+  }
+  // C: the contiguous low layers of every forward transform (each 2^n-word block is independent below layer n: run them as
+  // one launch over the 2^m-word columns)
+  auto fwd_low = [&](u32* buf, u32 tn, int which) -> nb200_status {
+    if (pl.LA == 12) return launch_contig<false, 12, 4, 3>(ctx, buf, mlen, buf, mlen, n_cols, m, tn, scatter, which);
+    return launch_contig<false, 13, 2, 2>(ctx, buf, mlen, buf, mlen, n_cols, m, tn, scatter, which);
+  };
+  NB_TRY(fwd_low(lde, m, 0));
+  if (half_ext) NB_TRY(fwd_low(half_ext, m + 1, 1));
   return NB200_OK;
 }
 
@@ -477,13 +422,7 @@ nb200_status commit_transforms(nb200_ctx* ctx, const u32* evals, u32* coeffs, u3
 // can the last LDE pass store straight into row-slice buffers of 2^log_slice rows?  (the same answer on every rank: it depends on sizes only)
 bool commit_transforms_can_scatter(u32 n, u32 bl, u32 log_slice, int world) {
   FusedPlan pl;
-  static const int fused = env_int("NB200_FFT_FUSED", 1);
-  return fused && bl == 1 && fused_plan(n, &pl) && world <= NB_MAX_SHARD_RANKS && log_slice >= pl.LA;
-}
-
-void fft_fused_release(nb200_ctx* ctx) {
-  for (int i = 0; i < 2; ++i) if (ctx->chunk_stream[i]) { cudaStreamDestroy(ctx->chunk_stream[i]); ctx->chunk_stream[i] = nullptr; }
-  for (int i = 0; i < 3; ++i) if (ctx->chunk_ev[i]) { cudaEventDestroy(ctx->chunk_ev[i]); ctx->chunk_ev[i] = nullptr; }
+  return bl == 1 && fused_plan(n, &pl) && world <= NB_MAX_SHARD_RANKS && log_slice >= pl.LA;
 }
 
 }  // namespace nb

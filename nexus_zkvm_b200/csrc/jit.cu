@@ -20,15 +20,6 @@
 
 namespace nb {
 
-// threads per CTA the constraint kernels are compiled for (their __launch_bounds__): 1024 -> <= 64 registers per thread; NB200_JIT_BOUND=512 lets
-// the compiler use up to 128 (fewer spills of the chunk state, half the warps per SM) — a tuning knob, part of the generated source and so of its cache key
-static u32 jit_bound() {
-  static u32 v = 0;
-  if (!v) { v = JIT_BLOCK; if (const char* e = getenv("NB200_JIT_BOUND")) { int x = atoi(e); if (x == 256 || x == 512 || x == 1024) v = (u32)x; } }
-  return v;
-}
-
-
 namespace {
 struct Nvrtc {
   void* h = nullptr;
@@ -221,8 +212,7 @@ std::string gen_source(const AirComponent& c) {
     else s << "__ldg(ccols[" << m << "] + offrow(row, " << c.masks[m].off << ", EL))";
     return s.str();
   };
-  size_t CH = 250;
-  if (const char* e = getenv("NB200_JIT_CHUNK")) { long v = atol(e); if (v >= 16 && v <= 100000) CH = (size_t)v; }
+  const size_t CH = 250;
   size_t n_chunks = (c.prog.size() + CH - 1) / CH;
   const ChunkLive live = chunk_liveness(c.prog, CH, nb, ne);
   u32 k = 0;
@@ -249,7 +239,7 @@ std::string gen_source(const AirComponent& c) {
   // The CTAs re-converge (__syncthreads) after every chunk: the warps of a CTA then execute the same few tens of KB of straight-line
   // code at a time and the instruction cache serves them from one fetch.  Without the barriers the warps drift apart over the ~0.7 MB
   // program and the kernel becomes instruction-fetch bound.
-  o << "extern \"C\" __global__ void __launch_bounds__(" << jit_bound() << ", 1) nbjit(const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff,\n"
+  o << "extern \"C\" __global__ void __launch_bounds__(" << JIT_BLOCK << ", 1) nbjit(const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff,\n"
     << "    const u32* __restrict__ dinv, u32* __restrict__ a0, u32* __restrict__ a1, u32* __restrict__ a2, u32* __restrict__ a3, u32 EL, u32 row0) {\n"
     << "  const u32 row = row0 + blockIdx.x * blockDim.x + threadIdx.x;   // row0: a rank of a multi-GPU proof evaluates its slice of the domain's rows\n  St s;\n"
     << "  for (int i = 0; i < " << nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n  s.rr = Q{0u, 0u, 0u, 0u};\n";
@@ -346,14 +336,6 @@ std::string gen_logup_source(const AirComponent& c) {
 
 std::string jit_source(const AirComponent& c) { return gen_source(c); }
 std::string jit_logup_source(const AirComponent& c) { return gen_logup_source(c); }
-
-// threads per CTA at launch: the code is compiled for up to JIT_BLOCK threads at <= 64 registers; 512 runs as two CTAs per SM, which sit in
-// different phases of the program and share the pipes.  On H100, 256 / 512 / 1024 give the same whole-proof time within noise (profiles/README.md)
-static u32 jit_block() {
-  static u32 b = 0;
-  if (!b) { b = 512; if (const char* e = getenv("NB200_JIT_BLOCK")) { int v = atoi(e); if (v == 256 || v == 512 || v == 1024) b = (u32)v; } }
-  return b < jit_bound() ? b : jit_bound();
-}
 
 bool jit_enabled() {
   const char* e = getenv("NB200_JIT");
@@ -479,7 +461,7 @@ nb200_status jit_launch_logup(nb200_ctx* ctx, const JitKernel& jk, const u32* co
   if (rows < JIT_BLOCK) return set_err(ctx, NB200_ERR_STATE, "jit: domain too small");
   NB_TRY(jit_set_cols(ctx, jk, d_cols));
   void* args[] = {(void*)&d_cols, (void*)&d_params, (void*)&d_out, (void*)&log_size};
-  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / jit_block())), dim3(jit_block()), args, 0, ctx->stream);
+  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args, 0, ctx->stream);
   ctx->launches += 1;
   if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
   return NB200_OK;
@@ -493,7 +475,7 @@ nb200_status jit_launch_constraints(nb200_ctx* ctx, const JitKernel& jk, const u
   u32 el = dom_log;
   u32* a0 = acc[0]; u32* a1 = acc[1]; u32* a2 = acc[2]; u32* a3 = acc[3];
   void* args[] = {(void*)&d_cols, (void*)&d_params, (void*)&d_coeff, (void*)&d_dinv, (void*)&a0, (void*)&a1, (void*)&a2, (void*)&a3, (void*)&el, (void*)&row0};
-  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / jit_block())), dim3(jit_block()), args, 0, ctx->stream);
+  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args, 0, ctx->stream);
   ctx->launches += 1;
   if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
   return NB200_OK;

@@ -8,6 +8,9 @@
 namespace nb {
 
 static const u32 JIT_BLOCK = 1024;       // the generated kernels are compiled for up to this many threads per CTA (<= 64 registers)
+// threads per CTA at launch: two CTAs per SM, which sit in different phases of the program and share the pipes.  On H100, 256 / 512 / 1024
+// gave the same whole-proof time within noise (profiles/README.md)
+static const u32 JIT_LAUNCH_BLOCK = 512;
 static const u32 JIT_MIN_INSTR = 64;      // shorter programs stay on the bytecode interpreter
 static const u32 JIT_COEFF_WORDS = 12;   // words per constraint in the coefficient table the generated kernel reads
 

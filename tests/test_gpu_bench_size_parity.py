@@ -87,7 +87,7 @@ def _oracle_tree(evals_by_batch, blow):
 def test_commit_evals_at_bench_size(ctx, n_cols):
     """(b) nb200_commit_evals (the call bench.py's `value` times) on 2^20-row trees: 27 columns = the reference's tree 0; 68 and 80
     columns = slices of trees 1 / 2 (347 / 1012 columns; the oracle hashes 64+ real columns per tree in seconds, not 1012) —
-    68 is not a multiple of the 16-column Blake2s block nor of the L2 column chunk, 80 is."""
+    68 is not a multiple of the 16-column Blake2s block, 80 is."""
     rng = np.random.default_rng(3000 + n_cols)
     ev = _cols(rng, n_cols, 20)
     batch = ctx.upload(ev)

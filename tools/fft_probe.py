@@ -1,5 +1,4 @@
-"""Event-timed probe of the commit transforms (iFFT + LDE) for one batch; knobs come from the environment
-(NB200_FFT_FUSED, NB200_FFT_CHUNK_MIB, NB200_FFT_STREAMS) because the library reads them once per process.
+"""Event-timed probe of the commit transforms (fused iFFT + LDE) for one batch, beside the per-transform passes.
     python tools/fft_probe.py [log_rows] [n_cols] [reps]"""
 import ctypes as C
 import json
@@ -44,7 +43,5 @@ with torch.cuda.stream(stream):
         torch.cuda.synchronize()
         tl.append((a.elapsed_time(b), b.elapsed_time(c)))
     elems = n_cols << log_rows
-    print(json.dumps({"log_rows": log_rows, "n_cols": n_cols, "fused": os.environ.get("NB200_FFT_FUSED", "1"),
-                      "chunk_mib": os.environ.get("NB200_FFT_CHUNK_MIB", "48"), "streams": os.environ.get("NB200_FFT_STREAMS", "2"),
-                      "ms": round(t, 3), "GBps_12B": round(12.0 * elems / (t * 1e-3) / 1e9, 1), "all_ms": [round(x, 3) for x in times],
+    print(json.dumps({"log_rows": log_rows, "n_cols": n_cols, "ms": round(t, 3), "GBps_12B": round(12.0 * elems / (t * 1e-3) / 1e9, 1), "all_ms": [round(x, 3) for x in times],
                       "legacy_ifft_ms": round(min(x[0] for x in tl), 3), "legacy_lde_ms": round(min(x[1] for x in tl), 3)}))
