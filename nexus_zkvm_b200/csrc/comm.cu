@@ -21,11 +21,6 @@
 #include <cstring>
 #include <algorithm>
 
-extern "C" nb200_status nb200_cols_alloc(nb200_ctx*, size_t, uint32_t, nb200_cols**);
-extern "C" void nb200_cols_free(nb200_ctx*, nb200_cols*);
-extern "C" void nb200_tree_free(nb200_ctx*, nb200_tree*);
-extern "C" nb200_status nb200_hash_node(int merkle_hash, const uint8_t* left, const uint8_t* right, const uint32_t* values, size_t n_values, uint8_t out[32]);
-
 extern "C" nb200_status nb200_comm_all_gather(nb200_ctx* ctx, const uint8_t* mine, size_t bytes, uint8_t* out);
 
 namespace nb {
@@ -349,6 +344,18 @@ nb200_status comm_all_reduce_sum_host(nb200_ctx* ctx, u32* host, size_t words) {
   return st;
 }
 
+nb200_status hash_top_layers(nb200_ctx* ctx, u32 k, const std::vector<TopCol>& top, std::vector<std::vector<uint8_t>>& layers) {
+  for (u32 l = k; l-- > 0;) {
+    layers[l].resize((size_t)32 << l);
+    for (size_t i = 0; i < ((size_t)1 << l); ++i) {
+      std::vector<u32> vals;
+      for (auto& tc : top) if (tc.log == l) vals.push_back(tc.vals[i]);
+      NB_TRY(nb200_hash_node(ctx->merkle_hash, &layers[l + 1][64 * i], &layers[l + 1][64 * i + 32], vals.data(), vals.size(), &layers[l][32 * i]));
+    }
+  }
+  return NB200_OK;
+}
+
 }  // namespace nb
 using namespace nb;
 
@@ -427,94 +434,73 @@ nb200_status nb200_commit_sharded(nb200_ctx* ctx, const nb200_cols* shard_evals,
   for (size_t b = 0; b < n_replicated; ++b) NB_ARG(ctx, replicated[b] && replicated[b]->log_size < n, "commit_sharded: replicated batches must be smaller than the sharded columns");
   NB_TRY(twiddles_prepare(ctx, std::max<u32>(m, 1)));
   const size_t len = (size_t)1 << n, mlen = (size_t)1 << m, S = mlen >> k;   // S = rows per rank
-  nb200_cols *co = nullptr, *lde = nullptr, *rows = nullptr;
-  u32* pack = nullptr;
-  std::vector<nb200_cols*> small_lde;
-  nb200_tree* sub = nullptr;
-  auto fail = [&](nb200_status st) {
-    if (co) nb200_cols_free(ctx, co); if (lde) nb200_cols_free(ctx, lde); if (rows) nb200_cols_free(ctx, rows);
-    for (auto* s : small_lde) nb200_cols_free(ctx, s);
-    if (sub) nb200_tree_free(ctx, sub);
-    dfree(ctx, pack);
-    return st;
-  };
-#define NB_TRYS(expr) do { nb200_status _s = (expr); if (_s != NB200_OK) return fail(_s); } while (0)
-#define NB_CUDAS(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) return fail(set_err(ctx, NB200_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(_e))); } while (0)
-#define NB_NCCLS(call) do { ncclResult_t _r = (call); if (_r != ncclSuccess) return fail(set_err(ctx, NB200_ERR_CUDA, std::string(#call) + ": " + nccl().GetErrorString(_r))); } while (0)
-  // 1. column-sharded transforms
-  NB_TRYS(nb200_cols_alloc(ctx, count, n, &co));
-  NB_TRYS(nb200_cols_alloc(ctx, count, m, &lde));
-  if (count) NB_TRYS(commit_transforms(ctx, shard_evals->d, co->d, lde->d, nullptr, count, n, log_blowup));
-  // 2. exchange: my columns' rows of peer q -> q; every peer's columns' rows of mine <- that peer
-  NB_TRYS(nb200_cols_alloc(ctx, total_cols, m - k, &rows));
-  if (world > 1 && count) NB_CUDAS(dmalloc(ctx, (void**)&pack, (size_t)(world - 1) * count * S * 4));
-  if (count) NB_CUDAS(cudaMemcpy2DAsync(rows->d + first * S, S * 4, lde->d + (size_t)rank * S, mlen * 4, S * 4, count, cudaMemcpyDeviceToDevice, ctx->stream));
-  if (world > 1) {
-    size_t slot = 0;
-    for (int q = 0; q < world; ++q) {
-      if (q == rank || !count) continue;
-      NB_CUDAS(cudaMemcpy2DAsync(pack + slot * count * S, S * 4, lde->d + (size_t)q * S, mlen * 4, S * 4, count, cudaMemcpyDeviceToDevice, ctx->stream));
-      ++slot;
+  ColsPtr co, rows;
+  NB_TRY(alloc(ctx, co, count, n));
+  {
+    ColsPtr lde;
+    DevBuf pack;
+    // 1. column-sharded transforms
+    NB_TRY(alloc(ctx, lde, count, m));
+    if (count) NB_TRY(commit_transforms(ctx, shard_evals->d, co->d, lde->d, nullptr, count, n, log_blowup));
+    // 2. exchange: my columns' rows of peer q -> q; every peer's columns' rows of mine <- that peer
+    NB_TRY(alloc(ctx, rows, total_cols, m - k));
+    if (world > 1 && count) NB_TRY(alloc(ctx, pack, (size_t)(world - 1) * count * S));
+    if (count) NB_CUDA(ctx, cudaMemcpy2DAsync(rows->d + first * S, S * 4, lde->d + (size_t)rank * S, mlen * 4, S * 4, count, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (world > 1) {
+      size_t slot = 0;
+      for (int q = 0; q < world; ++q) {
+        if (q == rank || !count) continue;
+        NB_CUDA(ctx, cudaMemcpy2DAsync(pack.p + slot * count * S, S * 4, lde->d + (size_t)q * S, mlen * 4, S * 4, count, cudaMemcpyDeviceToDevice, ctx->stream));
+        ++slot;
+      }
+      NB_NCCL(ctx, nccl().GroupStart());
+      slot = 0;
+      for (int q = 0; q < world; ++q) {
+        if (q == rank) continue;
+        size_t qf = 0, qc = 0;
+        shard_range(total_cols, world, q, &qf, &qc);
+        if (count) { NB_NCCL(ctx, nccl().Send(pack.p + slot * count * S, count * S, ncclUint32, q, c->comm, ctx->stream)); ++slot; }
+        if (qc) NB_NCCL(ctx, nccl().Recv(rows->d + qf * S, qc * S, ncclUint32, q, c->comm, ctx->stream));
+      }
+      NB_NCCL(ctx, nccl().GroupEnd());
     }
-    NB_NCCLS(nccl().GroupStart());
-    slot = 0;
-    for (int q = 0; q < world; ++q) {
-      if (q == rank) continue;
-      size_t qf = 0, qc = 0;
-      shard_range(total_cols, world, q, &qf, &qc);
-      if (count) { NB_NCCLS(nccl().Send(pack + slot * count * S, count * S, ncclUint32, q, c->comm, ctx->stream)); ++slot; }
-      if (qc) NB_NCCLS(nccl().Recv(rows->d + qf * S, qc * S, ncclUint32, q, c->comm, ctx->stream));
-    }
-    NB_NCCLS(nccl().GroupEnd());
   }
-  nb200_cols_free(ctx, lde); lde = nullptr;
-  dfree(ctx, pack); pack = nullptr;
   // 3. row-sharded sub-tree (+ the replicated smaller columns: each rank takes its slice; columns with fewer than `world` LDE rows
   //    live above the cap layer and are hashed on the host below)
   std::vector<ColRef> refs;
-  for (size_t g = 0; g < total_cols; ++g) refs.push_back(ColRef{rows->d + g * S, m - k});
-  struct TopCol { u32 log; std::vector<u32> vals; };
+  for (size_t g = 0; g < total_cols; ++g) refs.push_back(ColRef{rows->col(g), m - k});
   std::vector<TopCol> top;
+  std::vector<ColsPtr> small_lde;
   for (size_t b = 0; b < n_replicated; ++b) {
     const nb200_cols* ev = replicated[b];
     const u32 sl = ev->log_size + log_blowup;
-    nb200_cols *sco = nullptr, *sld = nullptr;
-    NB_TRYS(nb200_cols_alloc(ctx, ev->n_cols, ev->log_size, &sco));
-    small_lde.push_back(sco);
-    NB_TRYS(nb200_cols_alloc(ctx, ev->n_cols, sl, &sld));
-    small_lde.push_back(sld);
-    NB_TRYS(commit_transforms(ctx, ev->d, sco->d, sld->d, nullptr, ev->n_cols, ev->log_size, log_blowup));
+    ColsPtr sco, sld;
+    NB_TRY(alloc(ctx, sco, ev->n_cols, ev->log_size));
+    NB_TRY(alloc(ctx, sld, ev->n_cols, sl));
+    NB_TRY(commit_transforms(ctx, ev->d, sco->d, sld->d, nullptr, ev->n_cols, ev->log_size, log_blowup));
     for (size_t g = 0; g < ev->n_cols; ++g) {
       if (sl >= k) refs.push_back(ColRef{sld->col(g) + ((size_t)rank << (sl - k)), sl - k});
       else {
         TopCol t; t.log = sl; t.vals.resize((size_t)1 << sl);
-        NB_CUDAS(cudaMemcpyAsync(t.vals.data(), sld->col(g), t.vals.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        NB_CUDA(ctx, cudaMemcpyAsync(t.vals.data(), sld->col(g), t.vals.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
         top.push_back(std::move(t));
       }
     }
+    small_lde.push_back(std::move(sco));
+    small_lde.push_back(std::move(sld));
   }
-  NB_TRYS(merkle_commit(ctx, refs, &sub));
-  NB_CUDAS(cudaStreamSynchronize(ctx->stream));
+  nb200_tree* sub_raw = nullptr;
+  NB_TRY(merkle_commit(ctx, refs, &sub_raw));
+  TreePtr sub(sub_raw);
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   // caps exchange + top k levels on the host (identical on every rank)
-  std::vector<uint8_t> caps((size_t)32 * world);
-  NB_TRYS(nb200_comm_all_gather(ctx, sub->root, 32, caps.data()));
-  if (caps_out) memcpy(caps_out, caps.data(), caps.size());
-  std::vector<uint8_t> level = caps;
-  for (u32 l = k; l-- > 0;) {
-    std::vector<uint8_t> up((size_t)32 << l);
-    for (size_t i = 0; i < ((size_t)1 << l); ++i) {
-      std::vector<u32> vals;
-      for (auto& t : top) if (t.log == l) vals.push_back(t.vals[i]);
-      NB_TRYS(nb200_hash_node(ctx->merkle_hash, &level[64 * i], &level[64 * i + 32], vals.data(), vals.size(), &up[32 * i]));
-    }
-    level.swap(up);
-  }
-  memcpy(root, level.data(), 32);
-  for (auto* s : small_lde) nb200_cols_free(ctx, s);
-  *coeffs_out = co; *rows_out = rows; *subtree_out = sub;
-#undef NB_TRYS
-#undef NB_CUDAS
-#undef NB_NCCLS
+  std::vector<std::vector<uint8_t>> layers(k + 1);
+  layers[k].resize((size_t)32 * world);
+  NB_TRY(nb200_comm_all_gather(ctx, sub->root, 32, layers[k].data()));
+  if (caps_out) memcpy(caps_out, layers[k].data(), layers[k].size());
+  NB_TRY(hash_top_layers(ctx, k, top, layers));
+  memcpy(root, layers[0].data(), 32);
+  *coeffs_out = co.release(); *rows_out = rows.release(); *subtree_out = sub.release();
   return NB200_OK;
 }
 

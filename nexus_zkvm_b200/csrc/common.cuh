@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>
+#include <memory>
 #include <string>
 #include <vector>
 #include "../../include/nb200.h"
@@ -109,6 +110,36 @@ void trace_mark(nb200_ctx* ctx, const char* stage);
 inline cudaError_t dmalloc(nb200_ctx* ctx, void** p, size_t bytes) { return cudaMallocAsync(p, bytes ? bytes : 16, ctx->stream); }
 inline void dfree(nb200_ctx* ctx, void* p) { if (p) cudaFreeAsync(p, ctx->stream); }
 
+// Owning handles: an error return frees what a function still holds, in the stream order of its other frees.
+// Batches and trees carry their ctx, so the deleters need none.
+struct ColsDeleter { void operator()(nb200_cols* c) const { nb200_cols_free(c->ctx, c); } };
+struct TreeDeleter { void operator()(nb200_tree* t) const { nb200_tree_free(t->ctx, t); } };
+using ColsPtr = std::unique_ptr<nb200_cols, ColsDeleter>;
+using TreePtr = std::unique_ptr<nb200_tree, TreeDeleter>;
+// one dmalloc buffer of u32 words, freed on ctx->stream
+struct DevBuf {
+  nb200_ctx* ctx = nullptr;
+  u32* p = nullptr;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : ctx(o.ctx), p(o.p) { o.p = nullptr; }
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { dfree(ctx, p); }
+};
+// fill an empty handle; on failure it stays empty
+inline nb200_status alloc(nb200_ctx* ctx, ColsPtr& out, size_t n_cols, u32 log_size) {
+  nb200_cols* c = nullptr;
+  NB_TRY(nb200_cols_alloc(ctx, n_cols, log_size, &c));
+  out.reset(c);
+  return NB200_OK;
+}
+inline nb200_status alloc(nb200_ctx* ctx, DevBuf& out, size_t words) {
+  u32* p = nullptr;
+  NB_CUDA(ctx, dmalloc(ctx, (void**)&p, words * 4));
+  out.ctx = ctx; out.p = p;
+  return NB200_OK;
+}
+
 // ---- internal launchers (implemented in the .cu files) ----
 nb200_status twiddles_prepare(nb200_ctx* ctx, u32 max_domain_log);
 // Circle iFFT in place over a batch (evaluations -> coefficients)
@@ -159,5 +190,9 @@ nb200_status merkle_commit(nb200_ctx* ctx, const std::vector<ColRef>& cols, nb20
 nb200_status merkle_tree_alloc(nb200_ctx* ctx, u32 max_log, nb200_tree** out);
 nb200_status merkle_leaf_absorb(nb200_ctx* ctx, nb200_tree* tree, const u32* d_cols, size_t stride, size_t n_cols, size_t cols_before, size_t total_cols, bool final);
 long leaf_sink_batch(const size_t* n_cols, const u32* log_sizes, size_t n_batches);  // set for the one batch that holds all the largest columns of a tree
+// The top log2(world) = k levels of a row-sharded tree (comm.cu), hashed on the host, identically on every rank: layers[k] holds the world
+// sub-tree roots (the caps) on entry; layers[k-1] .. layers[0] are filled, mixing in the columns of 2^l < world LDE values at layer l.
+struct TopCol { u32 log; std::vector<u32> vals; };
+nb200_status hash_top_layers(nb200_ctx* ctx, u32 k, const std::vector<TopCol>& top, std::vector<std::vector<uint8_t>>& layers);
 
 }  // namespace nb

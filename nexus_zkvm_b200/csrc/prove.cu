@@ -26,12 +26,12 @@ struct nb200_air {
 namespace nb {
 
 struct SchemeTree {
-  std::vector<nb200_cols*> coeffs, ldes;  // owned batches, commitment order
-  std::vector<nb200_cols*> half_ext;      // per batch or empty: the polynomials on the first half of CanonicCoset(lde log + 1).circle_domain(),
+  std::vector<ColsPtr> coeffs, ldes;      // batches, commitment order
+  std::vector<ColsPtr> half_ext;          // per batch or empty: the polynomials on the first half of CanonicCoset(lde log + 1).circle_domain(),
                                           // precomputed at commit time when the scheme was told the AIR's degree bound (see component_quotients)
   struct ColLoc { u32 batch, idx, log; };
   std::vector<ColLoc> cols;               // global column index -> (batch, index in batch, polynomial log size)
-  nb200_tree* merkle = nullptr;
+  TreePtr merkle;
   const u32* coeff_ptr(size_t g) const { return coeffs[cols[g].batch]->col(cols[g].idx); }
   const u32* lde_ptr(size_t g) const { return ldes[cols[g].batch]->col(cols[g].idx); }
   // ---- one proof over N GPUs (nb200_scheme_commit_sharded): the tree's FIRST `big_total` columns (2^big_log rows each: the main component's)
@@ -39,14 +39,19 @@ struct SchemeTree {
   // the smaller columns that follow are replicated in coeffs / ldes / half_ext as usual.  cols[g].batch == BIG marks a sharded column.
   static constexpr u32 BIG = 0xffffffffu;
   bool sharded = false;
+  int rank = 0;
   size_t big_total = 0, own_first = 0, own_count = 0;
   u32 big_log = 0;                              // polynomial log size n; LDE log m = n + blow-up; rows per rank S = 2^m / world
-  nb200_cols* big_coeffs = nullptr;             // own_count x 2^n
-  nb200_cols* big_rows = nullptr;               // big_total x S: LDE rows [rank * S, (rank + 1) * S)
-  nb200_cols* big_rows_hx = nullptr;            // big_total x S: the same rows of the half-coset extension D2 (or nullptr)
-  nb200_cols* big_eval_rows = nullptr;          // big_total x 2^n / world: trace-domain rows (kept for the interaction trace of trees 0 / 1)
-  std::map<size_t, nb200_cols*> full_lde, full_hx;   // columns read at a row offset: full LDE / D2 copies on every rank
+  ColsPtr big_coeffs;                           // own_count x 2^n
+  ColsPtr big_rows;                             // big_total x S: LDE rows [rank * S, (rank + 1) * S)
+  ColsPtr big_rows_hx;                          // big_total x S: the same rows of the half-coset extension D2 (or empty)
+  ColsPtr big_eval_rows;                        // big_total x 2^n / world: trace-domain rows (kept for the interaction trace of trees 0 / 1)
+  std::map<size_t, ColsPtr> full_lde, full_hx;  // columns read at a row offset: full LDE / D2 copies on every rank
   std::vector<std::vector<uint8_t>> top_layers; // host copies of the Merkle layers 0..k (layer k = the world caps); `merkle` is this rank's sub-tree
+  // sharded column idx on the LDE domain / on D2, indexed by the GLOBAL row: only this rank's rows [row0(), row0() + S) may be read
+  size_t row0() const { return (size_t)rank << big_rows->log_size; }
+  const u32* lde_rows(size_t idx) const { return big_rows->col(idx) - row0(); }
+  const u32* hx_rows(size_t idx) const { return big_rows_hx->col(idx) - row0(); }
 };
 
 }  // namespace nb
@@ -58,31 +63,37 @@ struct nb200_scheme {
   uint32_t hint_log_expand = 0;  // nb200_scheme_set_constraint_log_degree: 0 = unknown
 };
 
-extern "C" nb200_status nb200_cols_alloc(nb200_ctx*, size_t, uint32_t, nb200_cols**);
-extern "C" void nb200_cols_free(nb200_ctx*, nb200_cols*);
-extern "C" void nb200_tree_free(nb200_ctx*, nb200_tree*);
-extern "C" nb200_status nb200_hash_node(int merkle_hash, const uint8_t* left, const uint8_t* right, const uint32_t* values, size_t n_values, uint8_t out[32]);
-namespace nb { nb200_status gather_hash(nb200_ctx* ctx, const std::vector<const uint8_t*>& addrs, uint8_t* host_out); }
-
 namespace nb {
 
-// RAII for temporary batches / trees
-struct ColsGuard {
-  nb200_ctx* ctx; nb200_cols* c = nullptr;
-  explicit ColsGuard(nb200_ctx* x) : ctx(x) {}
-  ~ColsGuard() { if (c) nb200_cols_free(ctx, c); }
-  nb200_cols* release() { nb200_cols* r = c; c = nullptr; return r; }
-};
+nb200_status gather_hash(nb200_ctx* ctx, const std::vector<const uint8_t*>& addrs, uint8_t* host_out);
 
-static void free_tree(nb200_ctx* ctx, SchemeTree& t) {
-  for (nb200_cols* c : {t.big_coeffs, t.big_rows, t.big_rows_hx, t.big_eval_rows}) if (c) nb200_cols_free(ctx, c);
-  for (auto& kv : t.full_lde) nb200_cols_free(ctx, kv.second);
-  for (auto& kv : t.full_hx) nb200_cols_free(ctx, kv.second);
-  for (auto* c : t.coeffs) nb200_cols_free(ctx, c);
-  for (auto* c : t.ldes) nb200_cols_free(ctx, c);
-  for (auto* c : t.half_ext) if (c) nb200_cols_free(ctx, c);
-  if (t.merkle) nb200_tree_free(ctx, t.merkle);
-  t = SchemeTree();
+// the parameter table (QM31 values, 16 bytes each) in device memory, for the constraint and LogUp kernels
+static nb200_status upload_params(nb200_ctx* ctx, const void* params, size_t n_params, DevBuf& out) {
+  NB_TRY(alloc(ctx, out, std::max<size_t>(n_params, 1) * 4));
+  if (n_params) NB_CUDA(ctx, cudaMemcpyAsync(out.p, params, n_params * 16, cudaMemcpyHostToDevice, ctx->stream));
+  return NB200_OK;
+}
+
+// The component's specialised kernel (constraints, or the LogUp program when `logup`), compiled on first use; nullptr = none.
+// `interp_fallback`: the caller can run the bytecode interpreter, so programs shorter than JIT_MIN_INSTR are not compiled and a failed
+// compile is only logged (NB200_TRACE).  The sharded row kernels have no interpreter: they try every program and reject a nullptr.
+static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp_idx, bool logup, bool interp_fallback) {
+  std::vector<JitKernel>& v = logup ? air_h->jit_logup : air_h->jit;
+  if (v.size() != air_h->prog.comps.size()) v.resize(air_h->prog.comps.size());
+  JitKernel& jk = v[comp_idx];
+  if (!jk.tried) {
+    jk.tried = true;
+    const AirComponent& c = air_h->prog.comps[comp_idx];
+    const bool worth_it = logup ? (c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0) : c.prog.size() >= JIT_MIN_INSTR;
+    if ((worth_it || !interp_fallback) && jit_enabled()) {
+      nb200_status st = logup ? jit_compile_logup(ctx, c, &jk) : jit_compile_constraints(ctx, c, &jk);
+      if (interp_fallback) {
+        if (st != NB200_OK && ctx->trace) fprintf(stderr, "[nb200] jit unavailable for %s: %s\n", logup ? "logup program" : "component", ctx->err.c_str());
+        trace_mark(ctx, logup ? "jit: compile logup (one-time)" : "jit: compile (one-time)");
+      }
+    }
+  }
+  return jk.kernel ? &jk : nullptr;
 }
 
 static nb200_status finish_tree(nb200_ctx* ctx, SchemeTree& t, HostChannel& ch, nb200_tree* pre_leaf = nullptr) {
@@ -93,7 +104,9 @@ static nb200_status finish_tree(nb200_ctx* ctx, SchemeTree& t, HostChannel& ch, 
       refs.push_back(ColRef{t.ldes[b]->col(c), t.ldes[b]->log_size});
       t.cols.push_back(SchemeTree::ColLoc{(u32)b, (u32)c, t.coeffs[b]->log_size});
     }
-  NB_TRY(merkle_commit(ctx, refs, &t.merkle, pre_leaf));
+  nb200_tree* tree = nullptr;
+  NB_TRY(merkle_commit(ctx, refs, &tree, pre_leaf));
+  t.merkle.reset(tree);
   ch.mix_root(t.merkle->root);
   return NB200_OK;
 }
@@ -106,29 +119,25 @@ nb200_status scheme_commit_evals(nb200_scheme* s, const nb200_cols* const* evals
   if (max_log >= 1) NB_TRY(twiddles_prepare(ctx, max_log));
   trace_mark(ctx, nullptr);
   SchemeTree t;
-#define NB_TRYT(expr) do { nb200_status _s = (expr); if (_s != NB200_OK) { free_tree(ctx, t); return _s; } } while (0)
   for (size_t b = 0; b < n; ++b) {
-    nb200_cols *co = nullptr, *lde = nullptr;
-    NB_TRYT(nb200_cols_alloc(ctx, evals[b]->n_cols, evals[b]->log_size, &co));
-    t.coeffs.push_back(co);
-    NB_TRYT(nb200_cols_alloc(ctx, evals[b]->n_cols, evals[b]->log_size + s->log_blowup, &lde));
-    t.ldes.push_back(lde);
+    ColsPtr co, lde, hx;
+    NB_TRY(alloc(ctx, co, evals[b]->n_cols, evals[b]->log_size));
+    NB_TRY(alloc(ctx, lde, evals[b]->n_cols, evals[b]->log_size + s->log_blowup));
     // when the AIR's degree bound says the quotient step will need these polynomials on the half coset D2 (component_quotients, Q_HALF),
     // the fused pipeline emits them from the coefficient tiles it already holds in shared memory (if the memory is there)
-    nb200_cols* hx = nullptr;
     const u32 lde_log = lde->log_size;
     if (s->hint_log_expand == s->log_blowup + 1 && lde_log > 8) {
       const size_t need = (co->n_cols << lde_log) * 4;
       if (ctx->live_bytes + need + ((size_t)40 << 30) < ctx->total_mem && twiddles_prepare(ctx, lde_log + 1) == NB200_OK)
-        if (nb200_cols_alloc(ctx, co->n_cols, lde_log, &hx) != NB200_OK) hx = nullptr;
+        alloc(ctx, hx, co->n_cols, lde_log);   // without it the quotient step extends the columns itself
     }
-    t.half_ext.push_back(hx);
-    NB_TRYT(commit_transforms(ctx, evals[b]->d, co->d, lde->d, hx ? hx->d : nullptr, co->n_cols, co->log_size, s->log_blowup));
+    NB_TRY(commit_transforms(ctx, evals[b]->d, co->d, lde->d, hx ? hx->d : nullptr, co->n_cols, co->log_size, s->log_blowup));
+    t.coeffs.push_back(std::move(co));
+    t.ldes.push_back(std::move(lde));
+    t.half_ext.push_back(std::move(hx));
   }
-#undef NB_TRYT
   trace_mark(ctx, "commit: ifft+lde");
-  nb200_status st = finish_tree(ctx, t, ch);
-  if (st != NB200_OK) { free_tree(ctx, t); return st; }
+  NB_TRY(finish_tree(ctx, t, ch));
   trace_mark(ctx, "commit: merkle");
   if (root) memcpy(root, t.merkle->root, 32);
   s->trees.push_back(std::move(t));
@@ -137,54 +146,49 @@ nb200_status scheme_commit_evals(nb200_scheme* s, const nb200_cols* const* evals
 
 // The same, from HOST columns (the reference hands over host `Vec<BaseColumn>`s, trace_builder.rs:156-164): upload,
 // finalize_columns on the device when `coset_order`, transforms — pipelined chunk by chunk — then Merkle + mix_root.
+// On failure nothing is handed to the caller (every evals_out[b] is nullptr) and nothing stays allocated.
 nb200_status scheme_commit_host(nb200_scheme* s, const void* const* host, const u32* elem_bytes, const size_t* n_cols, const u32* log_sizes, size_t n, int coset_order,
                                 HostChannel& ch, uint8_t root[32], nb200_cols** evals_out) {
   nb200_ctx* ctx = s->ctx;
+  for (size_t b = 0; b < n; ++b) evals_out[b] = nullptr;
   u32 max_log = 0;
   for (size_t b = 0; b < n; ++b) max_log = std::max(max_log, log_sizes[b] + s->log_blowup);
   if (max_log >= 1) NB_TRY(twiddles_prepare(ctx, max_log));
   trace_mark(ctx, nullptr);
   SchemeTree t;
-  for (size_t b = 0; b < n; ++b) evals_out[b] = nullptr;
+  std::vector<ColsPtr> evals(n);
   // leaf hashes are continued chunk by chunk under the PCIe copy when one batch holds all the largest columns
   LeafSink sink;
+  TreePtr pre_leaf;
   const long leaf_batch = leaf_sink_batch(n_cols, log_sizes, n);
-  // on any failure: nothing is handed to the caller, nothing stays allocated
-  auto fail = [&](nb200_status st) {
-    for (size_t b = 0; b < n; ++b) if (evals_out[b]) { nb200_cols_free(ctx, evals_out[b]); evals_out[b] = nullptr; }
-    if (sink.tree) nb200_tree_free(ctx, sink.tree);
-    free_tree(ctx, t);
-    return st;
-  };
-#define NB_TRYC(expr) do { nb200_status _s = (expr); if (_s != NB200_OK) return fail(_s); } while (0)
-  if (leaf_batch >= 0) NB_TRYC(merkle_tree_alloc(ctx, max_log, &sink.tree));
+  if (leaf_batch >= 0) {
+    NB_TRY(merkle_tree_alloc(ctx, max_log, &sink.tree));
+    pre_leaf.reset(sink.tree);
+  }
   for (size_t b = 0; b < n; ++b) {
-    nb200_cols *co = nullptr, *lde = nullptr, *hx = nullptr;
-    NB_TRYC(nb200_cols_alloc(ctx, n_cols[b], log_sizes[b], &evals_out[b]));
-    NB_TRYC(nb200_cols_alloc(ctx, n_cols[b], log_sizes[b], &co));
-    t.coeffs.push_back(co);
-    NB_TRYC(nb200_cols_alloc(ctx, n_cols[b], log_sizes[b] + s->log_blowup, &lde));
-    t.ldes.push_back(lde);
+    ColsPtr co, lde, hx;
+    NB_TRY(alloc(ctx, evals[b], n_cols[b], log_sizes[b]));
+    NB_TRY(alloc(ctx, co, n_cols[b], log_sizes[b]));
+    NB_TRY(alloc(ctx, lde, n_cols[b], log_sizes[b] + s->log_blowup));
     // The copy from the host is PCIe-bound and leaves the SMs mostly idle: if the AIR's degree bound is known to need the half-coset
     // evaluations of these polynomials later (component_quotients, Q_HALF), compute them now, chunk by chunk, in that shadow.
     const u32 lde_log = log_sizes[b] + s->log_blowup;
     if (s->hint_log_expand == s->log_blowup + 1 && lde_log > 8) {
-      NB_TRYC(twiddles_prepare(ctx, lde_log + 1));
-      NB_TRYC(nb200_cols_alloc(ctx, n_cols[b], lde_log, &hx));
+      NB_TRY(twiddles_prepare(ctx, lde_log + 1));
+      NB_TRY(alloc(ctx, hx, n_cols[b], lde_log));
     }
-    t.half_ext.push_back(hx);
-    NB_TRYC(upload_transform_pipelined(ctx, host[b], n_cols[b], log_sizes[b], coset_order, s->log_blowup, evals_out[b]->d, co->d, lde->d, hx ? hx->d : nullptr,
-                                       (long)b == leaf_batch ? &sink : nullptr, elem_bytes ? elem_bytes[b] : 4u));
+    NB_TRY(upload_transform_pipelined(ctx, host[b], n_cols[b], log_sizes[b], coset_order, s->log_blowup, evals[b]->d, co->d, lde->d, hx ? hx->d : nullptr,
+                                      (long)b == leaf_batch ? &sink : nullptr, elem_bytes ? elem_bytes[b] : 4u));
+    t.coeffs.push_back(std::move(co));
+    t.ldes.push_back(std::move(lde));
+    t.half_ext.push_back(std::move(hx));
   }
-#undef NB_TRYC
   trace_mark(ctx, "commit(host): h2d+ifft+lde");
-  nb200_tree* pre = sink.tree;
-  sink.tree = nullptr;                     // consumed by merkle_commit (also on failure)
-  nb200_status st = finish_tree(ctx, t, ch, pre);
-  if (st != NB200_OK) return fail(st);
+  NB_TRY(finish_tree(ctx, t, ch, pre_leaf.release()));   // merkle_commit consumes the leaf layer, also when it fails
   trace_mark(ctx, "commit: merkle");
   if (root) memcpy(root, t.merkle->root, 32);
   s->trees.push_back(std::move(t));
+  for (size_t b = 0; b < n; ++b) evals_out[b] = evals[b].release();
   return NB200_OK;
 }
 
@@ -196,9 +200,9 @@ nb200_status scheme_commit_host(nb200_scheme* s, const void* const* host, const 
 // replicated; everything small (extension components, composition tree, FRI) is computed redundantly on every rank.
 // ======================================================================================================================================
 // a column the constraints read at a row offset: every rank needs all of it — the all-gather of its row slices (contiguous row ranges in rank order)
-static nb200_status replicate_from_rows(nb200_ctx* ctx, const nb200_cols* rows, size_t g, u32 log_len, nb200_cols** out) {
-  NB_TRY(nb200_cols_alloc(ctx, 1, log_len, out));
-  return comm_all_gather_dev(ctx, rows->col(g), (size_t)1 << rows->log_size, (*out)->d);
+static nb200_status replicate_from_rows(nb200_ctx* ctx, const nb200_cols* rows, size_t g, u32 log_len, ColsPtr& out) {
+  NB_TRY(alloc(ctx, out, 1, log_len));
+  return comm_all_gather_dev(ctx, rows->col(g), (size_t)1 << rows->log_size, out->d);
 }
 
 nb200_status scheme_commit_sharded(nb200_scheme* s, const nb200_cols* big_shard, size_t total_big, u32 n, const nb200_cols* const* small, size_t n_small,
@@ -216,111 +220,120 @@ nb200_status scheme_commit_sharded(nb200_scheme* s, const nb200_cols* big_shard,
   NB_TRY(twiddles_prepare(ctx, want_hx ? m + 1 : m));
   trace_mark(ctx, nullptr);
   SchemeTree t;
-  t.sharded = true; t.big_total = total_big; t.own_first = first; t.own_count = count; t.big_log = n;
-  nb200_cols *lde_full = nullptr, *hx_full = nullptr;
-  auto fail = [&](nb200_status st) { if (lde_full) nb200_cols_free(ctx, lde_full); if (hx_full) nb200_cols_free(ctx, hx_full); free_tree(ctx, t); return st; };
-#define NB_TRYS(expr) do { nb200_status _s = (expr); if (_s != NB200_OK) return fail(_s); } while (0)
+  t.sharded = true; t.rank = rank; t.big_total = total_big; t.own_first = first; t.own_count = count; t.big_log = n;
   // 1-3. column-sharded transforms of this rank's columns, pipelined with the exchange: the columns are transformed in `nch` chunks on ctx->stream;
   // as soon as a chunk is done its row slices (LDE, D2, trace rows) travel to their owners on the communicator's side stream while the next
   // chunk is being transformed.  Every rank uses the same chunk count, so the grouped send / recv pairs of chunk j match.
-  NB_TRYS(nb200_cols_alloc(ctx, count, n, &t.big_coeffs));
-  NB_TRYS(nb200_cols_alloc(ctx, count, m, &lde_full));
-  if (want_hx) NB_TRYS(nb200_cols_alloc(ctx, count, m, &hx_full));
-  // the row-slice buffers: in the symmetric peer heap when CUDA IPC links the ranks (the owners of the columns then write their rows straight into
-  // them over NVLink with the copy engines), else ordinary allocations filled by grouped ncclSend / ncclRecv
-  PeerBuf pb_rows, pb_hx, pb_ev;
-  NB_TRYS(peer_alloc(ctx, s, total_big << (m - k), &pb_rows));
-  const bool peer = pb_rows.d != nullptr;
-  if (peer) {
-    NB_TRYS(nb200_cols_from_device(ctx, pb_rows.d, total_big, m - k, &t.big_rows));
-    if (want_hx) { NB_TRYS(peer_alloc(ctx, s, total_big << (m - k), &pb_hx)); NB_ARG(ctx, pb_hx.d, "peer heap"); NB_TRYS(nb200_cols_from_device(ctx, pb_hx.d, total_big, m - k, &t.big_rows_hx)); }
-    if (keep_eval_rows) { NB_TRYS(peer_alloc(ctx, s, total_big << (n - k), &pb_ev)); NB_ARG(ctx, pb_ev.d, "peer heap"); NB_TRYS(nb200_cols_from_device(ctx, pb_ev.d, total_big, n - k, &t.big_eval_rows)); }
-    NB_TRYS(comm_barrier_stream(ctx));     // every rank has reached this commit: nobody still reads what these buffers held in the previous proof
-  } else {
-    NB_TRYS(nb200_cols_alloc(ctx, total_big, m - k, &t.big_rows));
-    if (want_hx) NB_TRYS(nb200_cols_alloc(ctx, total_big, m - k, &t.big_rows_hx));
-    if (keep_eval_rows) NB_TRYS(nb200_cols_alloc(ctx, total_big, n - k, &t.big_eval_rows));
-  }
-  static const int xchg_chunks = [] { const char* e = getenv("NB200_XCHG_CHUNKS"); int v = e ? atoi(e) : 4; return v < 1 ? 1 : (v > 64 ? 64 : v); }();
-  // with the peer heap and a fused-pipeline size the LAST PASS of the transforms stores every finished tile into its owner's row-slice buffer (NVLink
-  // peer stores from the kernel: compute and exchange are one launch); otherwise the columns are transformed in chunks and re-sharded by copies /
-  // NCCL on the side stream while the next chunk is transformed
-  const bool scatter_ok = peer && commit_transforms_can_scatter(n, bl, m - k, world);
-  RowScatter sc;
-  if (scatter_ok) {
-    sc.world = world; sc.log_slice = m - k; sc.col0 = first;
-    for (int q = 0; q < world; ++q) { sc.lde_rows[q] = peer_ptr(ctx, pb_rows, q); sc.hx_rows[q] = want_hx ? peer_ptr(ctx, pb_hx, q) : nullptr; }
-  }
-  const int nch = (!scatter_ok && world > 1 && total_big / world >= 64) ? xchg_chunks : 1;
-  u32* pack = nullptr;
+  NB_TRY(alloc(ctx, t.big_coeffs, count, n));
   {
-    size_t maxc = 0;
-    for (int r = 0; r < world; ++r) { size_t f, c; comm_shard_range(total_big, world, r, &f, &c); maxc = std::max(maxc, c); }
-    const size_t chunk_cols = (maxc + nch - 1) / nch + 1;
-    if (world > 1 && !peer) NB_CUDA(ctx, dmalloc(ctx, (void**)&pack, (size_t)(world - 1) * chunk_cols * ((size_t)4 << (m - k))));
-  }
-  cudaStream_t xs = comm_side_stream(ctx);
-  auto fail2 = [&](nb200_status st) { comm_join(ctx); cudaStreamSynchronize(ctx->stream); dfree(ctx, pack); return fail(st); };
-#define NB_TRYX(expr) do { nb200_status _s = (expr); if (_s != NB200_OK) return fail2(_s); } while (0)
-  for (int j = 0; j < nch; ++j) {
-    const size_t c0 = count * j / nch, c1 = count * (j + 1) / nch;
-    bool scattered = false;
-    if (c1 > c0) {
-      RowScatter scj = sc;
-      scj.col0 = first + c0;
-      NB_TRYX(commit_transforms(ctx, big_shard->d + (c0 << n), t.big_coeffs->d + (c0 << n), lde_full->d + (c0 << m), hx_full ? hx_full->d + (c0 << m) : nullptr, c1 - c0, n, bl,
-                                scatter_ok ? &scj : nullptr, &scattered));
-      if (scatter_ok && !scattered) return fail2(set_err(ctx, NB200_ERR_STATE, "commit_sharded: the fused pipeline refused the row scatter"));
-    }
-    NB_TRYX(comm_fork(ctx));
+    ColsPtr lde_full, hx_full;
+    NB_TRY(alloc(ctx, lde_full, count, m));
+    if (want_hx) NB_TRY(alloc(ctx, hx_full, count, m));
+    // the row-slice buffers: in the symmetric peer heap when CUDA IPC links the ranks (the owners of the columns then write their rows straight into
+    // them over NVLink with the copy engines), else ordinary allocations filled by grouped ncclSend / ncclRecv
+    PeerBuf pb_rows, pb_hx, pb_ev;
+    NB_TRY(peer_alloc(ctx, s, total_big << (m - k), &pb_rows));
+    const bool peer = pb_rows.d != nullptr;
     if (peer) {
-      if (!scatter_ok) {
-        NB_TRYX(peer_cols_to_rows_chunk(ctx, xs, lde_full->d, total_big, (size_t)1 << m, pb_rows, j, nch));
-        if (want_hx) NB_TRYX(peer_cols_to_rows_chunk(ctx, xs, hx_full->d, total_big, (size_t)1 << m, pb_hx, j, nch));
+      nb200_cols* c = nullptr;
+      NB_TRY(nb200_cols_from_device(ctx, pb_rows.d, total_big, m - k, &c));
+      t.big_rows.reset(c);
+      if (want_hx) {
+        NB_TRY(peer_alloc(ctx, s, total_big << (m - k), &pb_hx));
+        NB_ARG(ctx, pb_hx.d, "peer heap");
+        NB_TRY(nb200_cols_from_device(ctx, pb_hx.d, total_big, m - k, &c));
+        t.big_rows_hx.reset(c);
       }
-      if (keep_eval_rows && count) NB_TRYX(peer_cols_to_rows_chunk(ctx, xs, big_shard->d, total_big, (size_t)1 << n, pb_ev, j, nch));
+      if (keep_eval_rows) {
+        NB_TRY(peer_alloc(ctx, s, total_big << (n - k), &pb_ev));
+        NB_ARG(ctx, pb_ev.d, "peer heap");
+        NB_TRY(nb200_cols_from_device(ctx, pb_ev.d, total_big, n - k, &c));
+        t.big_eval_rows.reset(c);
+      }
+      NB_TRY(comm_barrier_stream(ctx));     // every rank has reached this commit: nobody still reads what these buffers held in the previous proof
     } else {
-      NB_TRYX(exchange_cols_to_rows_chunk(ctx, xs, lde_full->d, total_big, (size_t)1 << m, t.big_rows->d, pack, j, nch));
-      if (want_hx) NB_TRYX(exchange_cols_to_rows_chunk(ctx, xs, hx_full->d, total_big, (size_t)1 << m, t.big_rows_hx->d, pack, j, nch));
-      if (keep_eval_rows) NB_TRYX(exchange_cols_to_rows_chunk(ctx, xs, count ? big_shard->d : nullptr, total_big, (size_t)1 << n, t.big_eval_rows->d, pack, j, nch));
+      NB_TRY(alloc(ctx, t.big_rows, total_big, m - k));
+      if (want_hx) NB_TRY(alloc(ctx, t.big_rows_hx, total_big, m - k));
+      if (keep_eval_rows) NB_TRY(alloc(ctx, t.big_eval_rows, total_big, n - k));
     }
+    static const int xchg_chunks = [] { const char* e = getenv("NB200_XCHG_CHUNKS"); int v = e ? atoi(e) : 4; return v < 1 ? 1 : (v > 64 ? 64 : v); }();
+    // with the peer heap and a fused-pipeline size the LAST PASS of the transforms stores every finished tile into its owner's row-slice buffer (NVLink
+    // peer stores from the kernel: compute and exchange are one launch); otherwise the columns are transformed in chunks and re-sharded by copies /
+    // NCCL on the side stream while the next chunk is transformed
+    const bool scatter_ok = peer && commit_transforms_can_scatter(n, bl, m - k, world);
+    RowScatter sc;
+    if (scatter_ok) {
+      sc.world = world; sc.log_slice = m - k; sc.col0 = first;
+      for (int q = 0; q < world; ++q) { sc.lde_rows[q] = peer_ptr(ctx, pb_rows, q); sc.hx_rows[q] = want_hx ? peer_ptr(ctx, pb_hx, q) : nullptr; }
+    }
+    const int nch = (!scatter_ok && world > 1 && total_big / world >= 64) ? xchg_chunks : 1;
+    DevBuf pack;
+    {
+      size_t maxc = 0;
+      for (int r = 0; r < world; ++r) { size_t f, c; comm_shard_range(total_big, world, r, &f, &c); maxc = std::max(maxc, c); }
+      const size_t chunk_cols = (maxc + nch - 1) / nch + 1;
+      if (world > 1 && !peer) NB_TRY(alloc(ctx, pack, (size_t)(world - 1) * chunk_cols << (m - k)));
+    }
+    cudaStream_t xs = comm_side_stream(ctx);
+    // Until the exchange is joined and the stream drained, the side stream may still read pack, lde_full and hx_full. On an error return this
+    // guard, destroyed before them, joins it and drains the stream so that their memory is not freed under a running copy.
+    struct JoinOnError {
+      nb200_ctx* ctx; bool armed = true;
+      ~JoinOnError() { if (armed) { comm_join(ctx); cudaStreamSynchronize(ctx->stream); } }
+    } join{ctx};
+    for (int j = 0; j < nch; ++j) {
+      const size_t c0 = count * j / nch, c1 = count * (j + 1) / nch;
+      bool scattered = false;
+      if (c1 > c0) {
+        RowScatter scj = sc;
+        scj.col0 = first + c0;
+        NB_TRY(commit_transforms(ctx, big_shard->d + (c0 << n), t.big_coeffs->d + (c0 << n), lde_full->d + (c0 << m), hx_full ? hx_full->d + (c0 << m) : nullptr, c1 - c0, n, bl,
+                                 scatter_ok ? &scj : nullptr, &scattered));
+        if (scatter_ok && !scattered) return set_err(ctx, NB200_ERR_STATE, "commit_sharded: the fused pipeline refused the row scatter");
+      }
+      NB_TRY(comm_fork(ctx));
+      if (peer) {
+        if (!scatter_ok) {
+          NB_TRY(peer_cols_to_rows_chunk(ctx, xs, lde_full->d, total_big, (size_t)1 << m, pb_rows, j, nch));
+          if (want_hx) NB_TRY(peer_cols_to_rows_chunk(ctx, xs, hx_full->d, total_big, (size_t)1 << m, pb_hx, j, nch));
+        }
+        if (keep_eval_rows && count) NB_TRY(peer_cols_to_rows_chunk(ctx, xs, big_shard->d, total_big, (size_t)1 << n, pb_ev, j, nch));
+      } else {
+        NB_TRY(exchange_cols_to_rows_chunk(ctx, xs, lde_full->d, total_big, (size_t)1 << m, t.big_rows->d, pack.p, j, nch));
+        if (want_hx) NB_TRY(exchange_cols_to_rows_chunk(ctx, xs, hx_full->d, total_big, (size_t)1 << m, t.big_rows_hx->d, pack.p, j, nch));
+        if (keep_eval_rows) NB_TRY(exchange_cols_to_rows_chunk(ctx, xs, count ? big_shard->d : nullptr, total_big, (size_t)1 << n, t.big_eval_rows->d, pack.p, j, nch));
+      }
+    }
+    trace_mark(ctx, "sharded commit: ifft+lde (own columns; exchange overlapped)");
+    NB_TRY(comm_join(ctx));
+    if (peer) NB_TRY(comm_barrier_stream(ctx));   // my copies are done AND (the barrier completing) so are everybody's into my buffers
+    // columns that constraints read at a row offset: full copies everywhere
+    for (size_t i = 0; i < n_replicate; ++i) {
+      const size_t g = replicate[i];
+      NB_ARG(ctx, g < total_big, "commit_sharded: replicate index out of range");
+      if (t.full_lde.count(g)) continue;
+      NB_TRY(replicate_from_rows(ctx, t.big_rows.get(), g, m, t.full_lde[g]));
+      if (want_hx) NB_TRY(replicate_from_rows(ctx, t.big_rows_hx.get(), g, m, t.full_hx[g]));
+    }
+    NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    join.armed = false;
   }
-  trace_mark(ctx, "sharded commit: ifft+lde (own columns; exchange overlapped)");
-  NB_TRYX(comm_join(ctx));
-  if (peer) NB_TRYX(comm_barrier_stream(ctx));   // my copies are done AND (the barrier completing) so are everybody's into my buffers
-  // columns that constraints read at a row offset: full copies everywhere
-  for (size_t i = 0; i < n_replicate; ++i) {
-    const size_t g = replicate[i];
-    if (g >= total_big) return fail2(set_err(ctx, NB200_ERR_ARG, "commit_sharded: replicate index out of range"));
-    if (t.full_lde.count(g)) continue;
-    nb200_cols* f = nullptr;
-    NB_TRYX(replicate_from_rows(ctx, t.big_rows, g, m, &f));
-    t.full_lde[g] = f;
-    if (want_hx) { nb200_cols* h = nullptr; NB_TRYX(replicate_from_rows(ctx, t.big_rows_hx, g, m, &h)); t.full_hx[g] = h; }
-  }
-#undef NB_TRYX
-  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  dfree(ctx, pack);
-  nb200_cols_free(ctx, lde_full); lde_full = nullptr;
-  if (hx_full) { nb200_cols_free(ctx, hx_full); hx_full = nullptr; }
   trace_mark(ctx, "sharded commit: exchange tail + replicated columns");
   // 4. the smaller batches: computed in full by every rank
   for (size_t b = 0; b < n_small; ++b) {
-    nb200_cols *co = nullptr, *lde = nullptr, *hx = nullptr;
-    NB_TRYS(nb200_cols_alloc(ctx, small[b]->n_cols, small[b]->log_size, &co));
-    t.coeffs.push_back(co);
-    NB_TRYS(nb200_cols_alloc(ctx, small[b]->n_cols, small[b]->log_size + bl, &lde));
-    t.ldes.push_back(lde);
-    if (want_hx && lde->log_size > 8) NB_TRYS(nb200_cols_alloc(ctx, small[b]->n_cols, lde->log_size, &hx));
-    t.half_ext.push_back(hx);
-    NB_TRYS(commit_transforms(ctx, small[b]->d, co->d, lde->d, hx ? hx->d : nullptr, co->n_cols, co->log_size, bl));
+    ColsPtr co, lde, hx;
+    NB_TRY(alloc(ctx, co, small[b]->n_cols, small[b]->log_size));
+    NB_TRY(alloc(ctx, lde, small[b]->n_cols, small[b]->log_size + bl));
+    if (want_hx && lde->log_size > 8) NB_TRY(alloc(ctx, hx, small[b]->n_cols, lde->log_size));
+    NB_TRY(commit_transforms(ctx, small[b]->d, co->d, lde->d, hx ? hx->d : nullptr, co->n_cols, co->log_size, bl));
+    t.coeffs.push_back(std::move(co));
+    t.ldes.push_back(std::move(lde));
+    t.half_ext.push_back(std::move(hx));
   }
   // 5. row-sharded sub-tree, caps, top levels
-  const size_t S = (size_t)1 << (m - k);
   std::vector<ColRef> refs;
   t.cols.clear();
-  for (size_t g = 0; g < total_big; ++g) { refs.push_back(ColRef{t.big_rows->d + g * S, m - k}); t.cols.push_back(SchemeTree::ColLoc{SchemeTree::BIG, (u32)g, n}); }
-  struct TopCol { u32 log; std::vector<u32> vals; };
+  for (size_t g = 0; g < total_big; ++g) { refs.push_back(ColRef{t.big_rows->col(g), m - k}); t.cols.push_back(SchemeTree::ColLoc{SchemeTree::BIG, (u32)g, n}); }
   std::vector<TopCol> top;
   for (size_t b = 0; b < t.ldes.size(); ++b)
     for (size_t c2 = 0; c2 < t.ldes[b]->n_cols; ++c2) {
@@ -333,32 +346,22 @@ nb200_status scheme_commit_sharded(nb200_scheme* s, const nb200_cols* big_shard,
         top.push_back(std::move(tc));
       }
     }
-  NB_TRYS(merkle_commit(ctx, refs, &t.merkle));
+  nb200_tree* sub = nullptr;
+  NB_TRY(merkle_commit(ctx, refs, &sub));
+  t.merkle.reset(sub);
   NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   t.top_layers.assign(k + 1, {});
   t.top_layers[k].resize((size_t)32 << k);
   {
-    std::vector<u32> mine(8), all((size_t)8 * world);
-    memcpy(mine.data(), t.merkle->root, 32);
-    u32* d = nullptr;
-    NB_CUDA(ctx, dmalloc(ctx, (void**)&d, (size_t)32 * (world + 1)));
-    NB_CUDA(ctx, cudaMemcpyAsync(d, mine.data(), 32, cudaMemcpyHostToDevice, ctx->stream));
-    nb200_status st = comm_all_gather_dev(ctx, d, 8, d + 8);
-    if (st == NB200_OK && cudaMemcpyAsync(t.top_layers[k].data(), d + 8, (size_t)32 * world, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "caps d2h");
-    if (st == NB200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "caps sync");
-    dfree(ctx, d);
-    if (st != NB200_OK) return fail(st);
+    DevBuf d;
+    NB_TRY(alloc(ctx, d, (size_t)8 * (world + 1)));
+    NB_CUDA(ctx, cudaMemcpyAsync(d.p, t.merkle->root, 32, cudaMemcpyHostToDevice, ctx->stream));
+    NB_TRY(comm_all_gather_dev(ctx, d.p, 8, d.p + 8));
+    NB_CUDA(ctx, cudaMemcpyAsync(t.top_layers[k].data(), d.p + 8, (size_t)32 * world, cudaMemcpyDeviceToHost, ctx->stream));
+    NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   }
-  for (u32 l = k; l-- > 0;) {
-    t.top_layers[l].resize((size_t)32 << l);
-    for (size_t i = 0; i < ((size_t)1 << l); ++i) {
-      std::vector<u32> vals;
-      for (auto& tc : top) if (tc.log == l) vals.push_back(tc.vals[i]);
-      NB_TRYS(nb200_hash_node(ctx->merkle_hash, &t.top_layers[l + 1][64 * i], &t.top_layers[l + 1][64 * i + 32], vals.data(), vals.size(), &t.top_layers[l][32 * i]));
-    }
-  }
+  NB_TRY(hash_top_layers(ctx, k, top, t.top_layers));
   memcpy(t.merkle->root, t.top_layers[0].data(), 32);   // from here on `merkle->root` is the root of the WHOLE tree (the sub-tree's own root is top_layers[k][rank])
-#undef NB_TRYS
   trace_mark(ctx, "sharded commit: merkle + caps");
   ch.mix_root(t.merkle->root);
   if (root) memcpy(root, t.merkle->root, 32);
@@ -373,11 +376,10 @@ static nb200_status merkle_decommit_sharded(nb200_ctx* ctx, const SchemeTree& t,
   const u32 k = (u32)comm_log_world(ctx);
   const int rank = comm_rank(ctx);
   const u32 m = t.big_log + blow;
-  const size_t S = (size_t)1 << (m - k);
-  struct CRef { const u32* d; u32 log; bool big; };   // big: d = row-slice base of this rank; else a full replicated column
+  struct CRef { const u32* d; u32 log; bool big; };   // d is indexed by the global row; big: only this rank's rows, else a full replicated column
   std::vector<CRef> cols;
   for (size_t g = 0; g < t.cols.size(); ++g) {
-    if (t.cols[g].batch == SchemeTree::BIG) cols.push_back(CRef{t.big_rows->d + (size_t)t.cols[g].idx * S, m, true});
+    if (t.cols[g].batch == SchemeTree::BIG) cols.push_back(CRef{t.lde_rows(t.cols[g].idx), m, true});
     else cols.push_back(CRef{t.ldes[t.cols[g].batch]->col(t.cols[g].idx), t.ldes[t.cols[g].batch]->log_size, false});
   }
   std::stable_sort(cols.begin(), cols.end(), [](const CRef& a, const CRef& b) { return a.log > b.log; });
@@ -417,7 +419,7 @@ static nb200_status merkle_decommit_sharded(nb200_ctx* ctx, const SchemeTree& t,
       for (size_t c = firstc; c < ci; ++c) {
         const size_t slot = vals.size();
         vals.push_back(0u); val_is_query.push_back(queried ? 1 : 0);
-        if (cols[c].big) { if ((node >> (m - k)) == (u64)rank) { val_addrs.push_back(cols[c].d + (node & (S - 1))); val_slot.push_back(slot); } }
+        if (cols[c].big) { if ((node >> (m - k)) == (u64)rank) { val_addrs.push_back(cols[c].d + node); val_slot.push_back(slot); } }
         else if (rank == 0) { val_addrs.push_back(cols[c].d + node); val_slot.push_back(slot); }
       }
       layer_total.push_back(node);
@@ -570,7 +572,6 @@ nb200_status component_quotients(nb200_scheme* s, nb200_air* air_h, size_t comp_
   nb200_ctx* ctx = s->ctx;
   const AirProgram& air = air_h->prog;
   NB_ARG(ctx, comp_idx < air.comps.size(), "constraint quotients: component index");
-  if (air_h->jit.size() != air.comps.size()) air_h->jit.resize(air.comps.size());
   const AirComponent& c = air.comps[comp_idx];
   const u32 elog = c.eval_log(), lde_log = c.log_size + s->log_blowup;
   if (mode == Q_HALF) NB_ARG(ctx, elog == lde_log + 1 && accum && accum_hi && accum->n_cols == 4 && accum_hi->n_cols == 4 && accum->log_size == lde_log && accum_hi->log_size == lde_log,
@@ -579,59 +580,42 @@ nb200_status component_quotients(nb200_scheme* s, nb200_air* air_h, size_t comp_
   NB_ARG(ctx, coeff.size() == c.n_constraints, "constraint quotients: one coefficient per constraint");
   NB_TRY(twiddles_prepare(ctx, elog));
   const bool reuse_lde = (mode == Q_FULL && elog == lde_log);
-  std::map<std::pair<u32, u32>, nb200_cols*> ext;
-  auto free_ext = [&]() { for (auto& kv : ext) nb200_cols_free(ctx, kv.second); ext.clear(); };
+  std::map<std::pair<u32, u32>, ColsPtr> ext;
   std::vector<const u32*> mask_cols(c.masks.size()), mask_lde(c.masks.size());
-  nb200_status st = NB200_OK;
-  for (size_t m = 0; m < c.masks.size() && st == NB200_OK; ++m) {
+  for (size_t m = 0; m < c.masks.size(); ++m) {
     const AirMask& mk = c.masks[m];
-    if (mk.tree >= s->trees.size() || mk.col >= s->trees[mk.tree].cols.size()) { st = set_err(ctx, NB200_ERR_ARG, "prove: AIR references a column that was not committed"); break; }
-    const SchemeTree::ColLoc& loc = s->trees[mk.tree].cols[mk.col];
-    if (loc.log != c.log_size) { st = set_err(ctx, NB200_ERR_ARG, "prove: column size differs from its component's log_size"); break; }
-    mask_lde[m] = s->trees[mk.tree].ldes[loc.batch]->col(loc.idx);
+    NB_ARG(ctx, mk.tree < s->trees.size() && mk.col < s->trees[mk.tree].cols.size(), "prove: AIR references a column that was not committed");
+    const SchemeTree& tr = s->trees[mk.tree];
+    const SchemeTree::ColLoc& loc = tr.cols[mk.col];
+    NB_ARG(ctx, loc.log == c.log_size, "prove: column size differs from its component's log_size");
+    mask_lde[m] = tr.ldes[loc.batch]->col(loc.idx);
     if (reuse_lde) { mask_cols[m] = mask_lde[m]; continue; }
-    auto key = std::make_pair(mk.tree, loc.batch);
-    if (mode == Q_HALF && loc.batch < s->trees[mk.tree].half_ext.size() && s->trees[mk.tree].half_ext[loc.batch]) {
-      mask_cols[m] = s->trees[mk.tree].half_ext[loc.batch]->col(loc.idx);   // precomputed at commit time
+    if (mode == Q_HALF && loc.batch < tr.half_ext.size() && tr.half_ext[loc.batch]) {
+      mask_cols[m] = tr.half_ext[loc.batch]->col(loc.idx);   // precomputed at commit time
       continue;
     }
-    if (!ext.count(key)) {
-      const nb200_cols* co = s->trees[mk.tree].coeffs[loc.batch];
-      nb200_cols* e = nullptr;
-      st = nb200_cols_alloc(ctx, co->n_cols, mode == Q_HALF ? lde_log : elog, &e);
-      if (st != NB200_OK) break;
-      ext[key] = e;
-      if (mode == Q_HALF) st = fft_evaluate(ctx, co->d, co->log_size, e->d, lde_log, co->n_cols, elog);   // first half of canonic(elog)
-      else st = fft_evaluate(ctx, co->d, co->log_size, e->d, elog, co->n_cols);
+    ColsPtr& e = ext[std::make_pair(mk.tree, loc.batch)];
+    if (!e) {
+      const nb200_cols* co = tr.coeffs[loc.batch].get();
+      NB_TRY(alloc(ctx, e, co->n_cols, mode == Q_HALF ? lde_log : elog));
+      if (mode == Q_HALF) NB_TRY(fft_evaluate(ctx, co->d, co->log_size, e->d, lde_log, co->n_cols, elog));   // first half of canonic(elog)
+      else NB_TRY(fft_evaluate(ctx, co->d, co->log_size, e->d, elog, co->n_cols));
     }
-    if (st == NB200_OK) mask_cols[m] = ext[key]->col(loc.idx);
+    mask_cols[m] = e->col(loc.idx);
   }
-  if (st == NB200_OK) {
-    JitKernel& jk = air_h->jit[comp_idx];
-    trace_mark(ctx, "constraints: extend columns");
-    if (!jk.tried) {
-      jk.tried = true;
-      if (c.prog.size() >= JIT_MIN_INSTR && jit_enabled()) {
-        trace_mark(ctx, "jit: load nvrtc (one-time)");
-        nb200_status js = jit_compile_constraints(ctx, c, &jk);
-        if (js != NB200_OK && ctx->trace) fprintf(stderr, "[nb200] jit unavailable for component: %s\n", ctx->err.c_str());
-        trace_mark(ctx, "jit: compile (one-time)");
-      }
-    }
-    const JitKernel* jp = jk.kernel ? &jk : nullptr;
-    if (mode == Q_HALF) {
-      u32* lo[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
-      u32* hi[4] = {accum_hi->col(0), accum_hi->col(1), accum_hi->col(2), accum_hi->col(3)};
-      st = constraint_eval(ctx, c, mask_lde, d_params, coeff, lo, jp, lde_log, lde_log);                        // D1: the committed LDE
-      if (st == NB200_OK) st = constraint_eval(ctx, c, mask_cols, d_params, coeff, hi, jp, lde_log, elog);     // D2: first half of canonic(elog)
-    } else {
-      u32* accp[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
-      st = constraint_eval(ctx, c, mask_cols, d_params, coeff, accp, jp, elog, elog);
-    }
-    trace_mark(ctx, "constraints: row kernel");
+  trace_mark(ctx, "constraints: extend columns");
+  const JitKernel* jp = ensure_jit(ctx, air_h, comp_idx, false, true);
+  if (mode == Q_HALF) {
+    u32* lo[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
+    u32* hi[4] = {accum_hi->col(0), accum_hi->col(1), accum_hi->col(2), accum_hi->col(3)};
+    NB_TRY(constraint_eval(ctx, c, mask_lde, d_params, coeff, lo, jp, lde_log, lde_log));                        // D1: the committed LDE
+    NB_TRY(constraint_eval(ctx, c, mask_cols, d_params, coeff, hi, jp, lde_log, elog));     // D2: first half of canonic(elog)
+  } else {
+    u32* accp[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
+    NB_TRY(constraint_eval(ctx, c, mask_cols, d_params, coeff, accp, jp, elog, elog));
   }
-  free_ext();
-  return st;
+  trace_mark(ctx, "constraints: row kernel");
+  return NB200_OK;
 }
 
 static bool component_is_sharded(const nb200_scheme* s, const AirComponent& c) {
@@ -658,20 +642,19 @@ static nb200_status component_quotients_sharded(nb200_scheme* s, nb200_air* air_
     const SchemeTree& tr = s->trees[mk.tree];
     const SchemeTree::ColLoc& loc = tr.cols[mk.col];
     NB_ARG(ctx, tr.sharded && loc.batch == SchemeTree::BIG && loc.log == c.log_size && tr.big_rows_hx, "sharded constraint quotients: the component may only read sharded columns of its own size");
-    if (mk.off == 0) { m_lde[m] = tr.big_rows->d + (size_t)loc.idx * S - row0; m_hx[m] = tr.big_rows_hx->d + (size_t)loc.idx * S - row0; }   // indexed by the GLOBAL row
+    if (mk.off == 0) { m_lde[m] = tr.lde_rows(loc.idx); m_hx[m] = tr.hx_rows(loc.idx); }
     else {
       auto f = tr.full_lde.find(loc.idx); auto h = tr.full_hx.find(loc.idx);
       NB_ARG(ctx, f != tr.full_lde.end() && h != tr.full_hx.end(), "sharded constraint quotients: a column read at a row offset was not listed for replication at commit time");
       m_lde[m] = f->second->d; m_hx[m] = h->second->d;
     }
   }
-  JitKernel& jk = air_h->jit[comp_idx];
-  if (!jk.tried) { jk.tried = true; if (jit_enabled()) jit_compile_constraints(ctx, c, &jk); }
-  NB_ARG(ctx, jk.kernel != nullptr, "sharded constraint quotients need the specialised kernel");
+  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, false, false);
+  NB_ARG(ctx, jk != nullptr, "sharded constraint quotients need the specialised kernel");
   u32* lo[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
   u32* hi[4] = {accum_hi->col(0), accum_hi->col(1), accum_hi->col(2), accum_hi->col(3)};
-  NB_TRY(constraint_eval(ctx, c, m_lde, d_params, coeff, lo, &jk, lde_log, lde_log, row0, S));
-  NB_TRY(constraint_eval(ctx, c, m_hx, d_params, coeff, hi, &jk, lde_log, elog, row0, S));
+  NB_TRY(constraint_eval(ctx, c, m_lde, d_params, coeff, lo, jk, lde_log, lde_log, row0, S));
+  NB_TRY(constraint_eval(ctx, c, m_hx, d_params, coeff, hi, jk, lde_log, elog, row0, S));
   for (int q = 0; q < 4; ++q) { NB_TRY(comm_all_gather_dev(ctx, lo[q] + row0, S, lo[q])); NB_TRY(comm_all_gather_dev(ctx, hi[q] + row0, S, hi[q])); }
   trace_mark(ctx, "constraints: row kernel (sharded) + all-gather");
   return NB200_OK;
@@ -682,10 +665,10 @@ static nb200_status half_to_coeffs(nb200_ctx* ctx, nb200_cols* lo, nb200_cols* h
   const u32 h = elog - 1;
   const size_t hl = (size_t)1 << h;
   NB_TRY(fft_interpolate(ctx, lo->d, lo->d, 4, h));                 // lo = coefficients of q mod pi^(elog-2)
-  ColsGuard t(ctx);
-  NB_TRY(nb200_cols_alloc(ctx, 4, h, &t.c));
-  NB_TRY(fft_evaluate(ctx, lo->d, h, t.c->d, h, 4, elog));          // lo evaluated on D2
-  NB_TRY(sub_scale_top_twiddle(ctx, hi->d, t.c->d, 4 * hl, elog));  // (q|D2 - lo|D2) / t
+  ColsPtr t;
+  NB_TRY(alloc(ctx, t, 4, h));
+  NB_TRY(fft_evaluate(ctx, lo->d, h, t->d, h, 4, elog));            // lo evaluated on D2
+  NB_TRY(sub_scale_top_twiddle(ctx, hi->d, t->d, 4 * hl, elog));    // (q|D2 - lo|D2) / t
   NB_TRY(fft_interpolate(ctx, hi->d, hi->d, 4, h, elog));           // hi coefficients
   // the composition's coefficient columns are 2^comp_log apart; this accumulator's polynomial may be smaller (a machine whose largest
   // evaluation domain belongs to another component): found by the prover2-shaped machine, tests/test_gpu_prove_parity.py
@@ -720,127 +703,121 @@ nb200_status accumulate_quotients(nb200_ctx* ctx, u32 lg, const std::vector<Samp
     qm31 bc = qm31_pow(q_coeff, hb[b].cols.size());
     memcpy(B.coeff, bc.c, 16);
   }
-  ColsGuard dom(ctx);
-  NB_TRY(nb200_cols_alloc(ctx, 2, lg, &dom.c));
-  NB_TRY(domain_points(ctx, lg, dom.c->col(0), dom.c->col(1)));
-  return quotients_launch(ctx, qb.data(), qb.size(), qe.data(), qe.size(), dom.c->col(0), dom.c->col(1), lg, out, row0, n_rows);
+  ColsPtr dom;
+  NB_TRY(alloc(ctx, dom, 2, lg));
+  NB_TRY(domain_points(ctx, lg, dom->col(0), dom->col(1)));
+  return quotients_launch(ctx, qb.data(), qb.size(), qe.data(), qe.size(), dom->col(0), dom->col(1), lg, out, row0, n_rows);
 }
 
-// stwo::prover::prove
-nb200_status prove_impl(nb200_scheme* s, nb200_air* air_h, const std::vector<qm31>& params, HostChannel& ch, std::vector<uint8_t>& proof_bytes) {
+// ---- stwo::prover::prove, one function per stage; prove_impl runs them in order ----
+
+static nb200_status zeroed(nb200_ctx* ctx, u32 lg, ColsPtr& out) {
+  NB_TRY(alloc(ctx, out, 4, lg));
+  NB_CUDA(ctx, cudaMemsetAsync(out->d, 0, ((size_t)16) << lg, ctx->stream));
+  return NB200_OK;
+}
+
+// composition polynomial: every component's constraint quotients, combined by the powers of random_coeff, committed as tree 3
+static nb200_status commit_composition(nb200_scheme* s, nb200_air* air_h, const std::vector<qm31>& params, qm31 random_coeff, size_t n_total, HostChannel& ch) {
   nb200_ctx* ctx = s->ctx;
   const AirProgram& air = air_h->prog;
-  if (air_h->jit.size() != air.comps.size()) air_h->jit.resize(air.comps.size());
-  NB_ARG(ctx, s->trees.size() == 3, "prove: the preprocessed, main and interaction trees must be committed first");
-  NB_ARG(ctx, params.size() == air.n_params, "prove: parameter table size");
   const u32 blow = s->log_blowup;
-
-  trace_mark(ctx, nullptr);
-  // ---------------- composition polynomial ----------------
-  qm31 random_coeff = ch.draw_felt();
-  size_t n_total = 0; u32 comp_log = 0;
-  for (auto& c : air.comps) { n_total += c.n_constraints; comp_log = std::max(comp_log, c.eval_log()); }
+  u32 comp_log = 0;
+  for (auto& c : air.comps) comp_log = std::max(comp_log, c.eval_log());
   NB_TRY(twiddles_prepare(ctx, comp_log + blow));
   std::vector<qm31> powers(n_total);
   { qm31 a = qm31_one(); for (size_t i = 0; i < n_total; ++i) { powers[i] = a; a = qm31_mul(a, random_coeff); } }
-  u32* d_params = nullptr;
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_params, std::max<size_t>(params.size(), 1) * 16));
-  if (!params.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_params, params.data(), params.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
+  DevBuf d_params;
+  NB_TRY(upload_params(ctx, params.data(), params.size(), d_params));
 
   // accumulators per (evaluation log, mode): Q_FULL -> {evals on canonic(elog), -}; Q_HALF -> {q on D1, q on D2}
-  struct Acc { nb200_cols* a = nullptr; nb200_cols* b = nullptr; };
+  struct Acc { ColsPtr a, b; };
   std::map<std::pair<u32, int>, Acc> acc;
-  auto free_acc = [&]() { for (auto& kv : acc) { if (kv.second.a) nb200_cols_free(ctx, kv.second.a); if (kv.second.b) nb200_cols_free(ctx, kv.second.b); } acc.clear(); };
-  auto zeroed = [&](u32 lg, nb200_cols** out) -> nb200_status {
-    NB_TRY(nb200_cols_alloc(ctx, 4, lg, out));
-    NB_CUDA(ctx, cudaMemsetAsync((*out)->d, 0, ((size_t)16) << lg, ctx->stream));
-    return NB200_OK;
-  };
   size_t g0 = 0;
   for (const AirComponent& c : air.comps) {
     const u32 elog = c.eval_log();
     const QuotMode mode = quotient_mode(s, c);
-    nb200_status st = NB200_OK;
-    auto key = std::make_pair(elog, (int)mode);
-    if (!acc.count(key)) {
-      Acc a;
-      st = zeroed(mode == Q_HALF ? elog - 1 : elog, &a.a);
-      if (st == NB200_OK && mode == Q_HALF) st = zeroed(elog - 1, &a.b);
-      acc[key] = a;
+    Acc& a = acc[std::make_pair(elog, (int)mode)];
+    if (!a.a) {
+      NB_TRY(zeroed(ctx, mode == Q_HALF ? elog - 1 : elog, a.a));
+      if (mode == Q_HALF) NB_TRY(zeroed(ctx, elog - 1, a.b));
     }
-    if (st == NB200_OK) {
-      std::vector<qm31> coeff(c.n_constraints);
-      for (u32 k = 0; k < c.n_constraints; ++k) coeff[k] = powers[n_total - 1 - (g0 + k)];
-      if (component_is_sharded(s, c)) st = component_quotients_sharded(s, air_h, &c - &air.comps[0], d_params, coeff, acc[key].a, acc[key].b);
-      else st = component_quotients(s, air_h, &c - &air.comps[0], d_params, coeff, mode, acc[key].a, acc[key].b);
-    }
+    std::vector<qm31> coeff(c.n_constraints);
+    for (u32 k = 0; k < c.n_constraints; ++k) coeff[k] = powers[n_total - 1 - (g0 + k)];
+    const size_t comp_idx = &c - &air.comps[0];
+    if (component_is_sharded(s, c)) NB_TRY(component_quotients_sharded(s, air_h, comp_idx, d_params.p, coeff, a.a.get(), a.b.get()));
+    else NB_TRY(component_quotients(s, air_h, comp_idx, d_params.p, coeff, mode, a.a.get(), a.b.get()));
     g0 += c.n_constraints;
-    if (st != NB200_OK) { free_acc(); dfree(ctx, d_params); return st; }
   }
   // DomainEvaluationAccumulator::finalize.  Upstream folds the per-size accumulators upwards (evaluate the running polynomial on the next
   // size, add, interpolate); interpolation is linear, so the result is the sum of the zero-extended coefficient vectors — computed here.
-  nb200_cols* cur = nullptr;  // coefficients of the composition (4 columns of 2^comp_log)
-  {
-    nb200_status st = zeroed(comp_log, &cur);
-    for (auto& kv : acc) {
-      if (st != NB200_OK) break;
-      const u32 elog = kv.first.first;
-      if (kv.first.second == Q_HALF) st = half_to_coeffs(ctx, kv.second.a, kv.second.b, elog, cur->d, (size_t)1 << comp_log);
-      else {
-        st = fft_interpolate(ctx, kv.second.a->d, kv.second.a->d, 4, elog);
-        if (st == NB200_OK) st = add_cols_strided(ctx, cur->d, (size_t)1 << comp_log, kv.second.a->d, (size_t)1 << elog, (size_t)1 << elog, 4);
-      }
+  ColsPtr cur;  // coefficients of the composition (4 columns of 2^comp_log)
+  NB_TRY(zeroed(ctx, comp_log, cur));
+  for (auto& kv : acc) {
+    const u32 elog = kv.first.first;
+    nb200_cols* a = kv.second.a.get();
+    if (kv.first.second == Q_HALF) NB_TRY(half_to_coeffs(ctx, a, kv.second.b.get(), elog, cur->d, (size_t)1 << comp_log));
+    else {
+      NB_TRY(fft_interpolate(ctx, a->d, a->d, 4, elog));
+      NB_TRY(add_cols_strided(ctx, cur->d, (size_t)1 << comp_log, a->d, (size_t)1 << elog, (size_t)1 << elog, 4));
     }
-    free_acc();
-    if (st != NB200_OK) { if (cur) nb200_cols_free(ctx, cur); dfree(ctx, d_params); return st; }
   }
-  NB_ARG(ctx, n_total > 0, "prove: no constraints");
+  acc.clear();   // before tree 3 is allocated
   // tree 3: the composition's 4 coordinate polynomials
-  {
-    SchemeTree t;
-    t.coeffs.push_back(cur);
-    nb200_cols* lde = nullptr;
-    NB_TRY(nb200_cols_alloc(ctx, 4, comp_log + blow, &lde));
-    t.ldes.push_back(lde);
-    NB_TRY(fft_evaluate(ctx, cur->d, comp_log, lde->d, comp_log + blow, 4));
-    NB_TRY(finish_tree(ctx, t, ch));
-    s->trees.push_back(std::move(t));
-  }
-
+  SchemeTree t;
+  ColsPtr lde;
+  NB_TRY(alloc(ctx, lde, 4, comp_log + blow));
+  NB_TRY(fft_evaluate(ctx, cur->d, comp_log, lde->d, comp_log + blow, 4));
+  t.coeffs.push_back(std::move(cur));
+  t.ldes.push_back(std::move(lde));
+  NB_TRY(finish_tree(ctx, t, ch));
+  s->trees.push_back(std::move(t));
   trace_mark(ctx, "composition: coefficients + commit");
-  // ---------------- OODS sampling ----------------
-  qpoint oods;
+  return NB200_OK;
+}
+
+// the out-of-domain point, the points each committed column is sampled at and the values there (tree / column / offset order)
+struct OodsSamples {
+  qpoint point;
+  std::vector<std::vector<std::vector<int32_t>>> offs;   // per tree / column: offsets in declaration order (Components::mask_points)
+  std::vector<std::vector<std::vector<qpoint>>> points;
+  std::vector<std::vector<std::vector<qm31>>> sampled;
+};
+
+static nb200_status sample_oods(nb200_scheme* s, const AirProgram& air, HostChannel& ch, OodsSamples& o) {
+  nb200_ctx* ctx = s->ctx;
   {
     qm31 t = ch.draw_felt();
     qm31 t2 = qm31_sqr(t);
     qm31 ip = qm31_inv(qm31_add(t2, qm31_one()));
-    oods.x = qm31_mul(qm31_sub(qm31_one(), t2), ip);
-    oods.y = qm31_mul(qm31_add(t, t), ip);
+    o.point.x = qm31_mul(qm31_sub(qm31_one(), t2), ip);
+    o.point.y = qm31_mul(qm31_add(t, t), ip);
   }
-  // per tree / column: offsets in declaration order (Components::mask_points)
-  std::vector<std::vector<std::vector<int32_t>>> offs(4);
+  auto& offs = o.offs;
+  offs.resize(4);
   for (int t = 0; t < 4; ++t) offs[t].resize(s->trees[t].cols.size());
   for (const AirComponent& c : air.comps)
     for (const AirMask& m : c.masks) {
-      auto& o = offs[m.tree][m.col];
-      if (std::find(o.begin(), o.end(), m.off) == o.end()) o.push_back(m.off);
+      auto& off = offs[m.tree][m.col];
+      if (std::find(off.begin(), off.end(), m.off) == off.end()) off.push_back(m.off);
     }
-  for (auto& o : offs[3]) o.assign(1, 0);
+  for (auto& off : offs[3]) off.assign(1, 0);
   auto mask_point = [&](u32 log_size, int32_t off) -> qpoint {
-    if (off == 0) return oods;
+    if (off == 0) return o.point;
     u32 step = canonic_step_index(log_size);
     u32 idx = idx_mul(step, (u64)(off < 0 ? -off : off));
     if (off < 0) idx = idx_neg(idx);
-    return qp_add(oods, qp_from_m31(index_to_point(idx)));
+    return qp_add(o.point, qp_from_m31(index_to_point(idx)));
   };
-  std::vector<std::vector<std::vector<qpoint>>> points(4);
-  std::vector<std::vector<std::vector<qm31>>> sampled(4);
+  auto& points = o.points;
+  auto& sampled = o.sampled;
+  points.resize(4); sampled.resize(4);
   std::vector<std::vector<qm31>*> sharded_samples;   // (multi-GPU) sampled-value lists of column-sharded columns, one entry per pushed value
   for (int t = 0; t < 4; ++t) {
     const SchemeTree& tr = s->trees[t];
     points[t].resize(tr.cols.size()); sampled[t].resize(tr.cols.size());
     for (size_t g = 0; g < tr.cols.size(); ++g)
-      for (int32_t o : offs[t][g]) points[t][g].push_back(mask_point(tr.cols[g].log, o));
+      for (int32_t off : offs[t][g]) points[t][g].push_back(mask_point(tr.cols[g].log, off));
     // groups of consecutive columns of one batch with the same offsets -> one eval_at_points launch
     size_t g = 0;
     while (g < tr.cols.size()) {
@@ -872,217 +849,261 @@ nb200_status prove_impl(nb200_scheme* s, nb200_air* air_h, const std::vector<qm3
     for (auto* v : sharded_samples) { const qm31& q = (*v)[seen[v]++]; buf.insert(buf.end(), q.c, q.c + 4); }
     NB_TRY(comm_all_reduce_sum_host(ctx, buf.data(), buf.size()));
     seen.clear();
-    size_t o = 0;
-    for (auto* v : sharded_samples) { (*v)[seen[v]++] = load_param(&buf[o]); o += 4; }
+    size_t pos = 0;
+    for (auto* v : sharded_samples) { (*v)[seen[v]++] = load_param(&buf[pos]); pos += 4; }
   }
   {
     std::vector<qm31> flat;
     for (auto& t : sampled) for (auto& c : t) for (auto& v : c) flat.push_back(v);
     ch.mix_felts(flat.data(), flat.size());
   }
-
   trace_mark(ctx, "oods eval_at_point");
-  // ---------------- DEEP quotients ----------------
+  return NB200_OK;
+}
+
+// the columns FRI commits to and the layers it folds them into: held until their decommitments are taken
+struct FriLayer { ColsPtr cols; TreePtr tree; u32 log; };
+struct FriState {
+  std::vector<ColsPtr> quotients;   // DEEP quotients, 4 coordinate columns each, largest first
+  std::vector<u32> qlogs;
+  TreePtr first_tree;
+  std::vector<FriLayer> inner;
+};
+
+static nb200_status deep_quotients(nb200_scheme* s, const OodsSamples& o, HostChannel& ch, FriState& f) {
+  nb200_ctx* ctx = s->ctx;
   qm31 q_coeff = ch.draw_felt();
   struct CRef { int t; size_t g; u32 log; };
   std::vector<CRef> all;
-  for (int t = 0; t < 4; ++t) for (size_t g = 0; g < s->trees[t].cols.size(); ++g) all.push_back(CRef{t, g, s->trees[t].cols[g].log + blow});
+  for (int t = 0; t < 4; ++t) for (size_t g = 0; g < s->trees[t].cols.size(); ++g) all.push_back(CRef{t, g, s->trees[t].cols[g].log + s->log_blowup});
   std::stable_sort(all.begin(), all.end(), [](const CRef& a, const CRef& b) { return a.log > b.log; });
-  std::vector<nb200_cols*> quotients; std::vector<u32> qlogs;
-  auto free_q = [&]() { for (auto* q : quotients) nb200_cols_free(ctx, q); quotients.clear(); };
   for (size_t i = 0; i < all.size();) {
     size_t j = i; while (j < all.size() && all[j].log == all[i].log) ++j;
     const u32 lg = all[i].log;
     // ColumnSampleBatch::new_vec: group samples by point, first-seen order                   [risk: IndexMap vs BTreeMap]
     std::vector<SampleBatch> hb;
-    bool grp_sharded = false;
+    const SchemeTree* sharded = nullptr;   // a tree whose row slices this group reads
     for (size_t k = i; k < j; ++k) {
       const CRef& r = all[k];
-      for (size_t pi = 0; pi < points[r.t][r.g].size(); ++pi) {
-        const qpoint& p = points[r.t][r.g][pi];
+      for (size_t pi = 0; pi < o.points[r.t][r.g].size(); ++pi) {
+        const qpoint& p = o.points[r.t][r.g][pi];
         size_t b = 0;
         for (; b < hb.size(); ++b) if (qm31_eq(hb[b].p.x, p.x) && qm31_eq(hb[b].p.y, p.y)) break;
         if (b == hb.size()) hb.push_back(SampleBatch{p, {}});
         const SchemeTree& trr = s->trees[r.t];
-        if (trr.sharded && trr.cols[r.g].batch == SchemeTree::BIG) {   // row slice, addressed by the global row
-          grp_sharded = true;
-          hb[b].cols.push_back({trr.big_rows->d + (size_t)trr.cols[r.g].idx * ((size_t)1 << (lg - (u32)comm_log_world(ctx))) - (size_t)comm_rank(ctx) * ((size_t)1 << (lg - (u32)comm_log_world(ctx))),
-                                sampled[r.t][r.g][pi]});
-        } else hb[b].cols.push_back({trr.lde_ptr(r.g), sampled[r.t][r.g][pi]});
+        if (trr.sharded && trr.cols[r.g].batch == SchemeTree::BIG) {
+          sharded = &trr;
+          hb[b].cols.push_back({trr.lde_rows(trr.cols[r.g].idx), o.sampled[r.t][r.g][pi]});
+        } else hb[b].cols.push_back({trr.lde_ptr(r.g), o.sampled[r.t][r.g][pi]});
       }
     }
-    nb200_cols* q = nullptr;
-    nb200_status st = nb200_cols_alloc(ctx, 4, lg, &q);
-    if (st == NB200_OK) {
-      quotients.push_back(q); qlogs.push_back(lg);
-      if (grp_sharded) {   // this rank's rows of the quotient column, then an all-gather: FRI runs replicated on the whole column
-        const size_t Sg = (size_t)1 << (lg - (u32)comm_log_world(ctx));
-        const u32 r0 = (u32)(comm_rank(ctx) * Sg);
-        st = accumulate_quotients(ctx, lg, hb, q_coeff, q->d, r0, Sg);
-        for (int qq = 0; qq < 4 && st == NB200_OK; ++qq) st = comm_all_gather_dev(ctx, q->col(qq) + r0, Sg, q->col(qq));
-      } else st = accumulate_quotients(ctx, lg, hb, q_coeff, q->d);
-    }
-    if (st != NB200_OK) { free_q(); dfree(ctx, d_params); return st; }
+    ColsPtr q;
+    NB_TRY(alloc(ctx, q, 4, lg));
+    if (sharded) {   // this rank's rows of the quotient column, then an all-gather: FRI runs replicated on the whole column
+      const size_t rows = sharded->big_rows->col_len();
+      const u32 r0 = (u32)sharded->row0();
+      NB_TRY(accumulate_quotients(ctx, lg, hb, q_coeff, q->d, r0, rows));
+      for (int qq = 0; qq < 4; ++qq) NB_TRY(comm_all_gather_dev(ctx, q->col(qq) + r0, rows, q->col(qq)));
+    } else NB_TRY(accumulate_quotients(ctx, lg, hb, q_coeff, q->d));
+    f.quotients.push_back(std::move(q)); f.qlogs.push_back(lg);
     i = j;
   }
-
   trace_mark(ctx, "deep quotients");
-  // ---------------- FRI commit phase ----------------
-  struct Layer { nb200_cols* cols; nb200_tree* tree; u32 log; };
-  std::vector<Layer> inner;
-  nb200_tree* first_tree = nullptr;
-  auto cleanup_fri = [&]() { for (auto& l : inner) { if (l.cols) nb200_cols_free(ctx, l.cols); if (l.tree) nb200_tree_free(ctx, l.tree); } inner.clear(); if (first_tree) nb200_tree_free(ctx, first_tree); first_tree = nullptr; free_q(); dfree(ctx, d_params); };
-#define NB_TRYF(expr) do { nb200_status _s = (expr); if (_s != NB200_OK) { cleanup_fri(); return _s; } } while (0)
+  return NB200_OK;
+}
+
+static nb200_status fri_commit(nb200_scheme* s, HostChannel& ch, FriState& f, std::vector<qm31>& last_layer_poly) {
+  nb200_ctx* ctx = s->ctx;
   {
     std::vector<ColRef> refs;
-    for (size_t g = 0; g < quotients.size(); ++g) for (int k = 0; k < 4; ++k) refs.push_back(ColRef{quotients[g]->col(k), qlogs[g]});
-    NB_TRYF(merkle_commit(ctx, refs, &first_tree));
-    ch.mix_root(first_tree->root);
+    for (size_t g = 0; g < f.quotients.size(); ++g) for (int k = 0; k < 4; ++k) refs.push_back(ColRef{f.quotients[g]->col(k), f.qlogs[g]});
+    nb200_tree* tree = nullptr;
+    NB_TRY(merkle_commit(ctx, refs, &tree));
+    f.first_tree.reset(tree);
+    ch.mix_root(tree->root);
   }
   qm31 circle_alpha = ch.draw_felt();
-  const size_t last_domain = (size_t)1 << (s->log_last + blow);
-  u32 L = qlogs[0] - 1;
-  nb200_cols* layer = nullptr;
-  NB_TRYF(nb200_cols_alloc(ctx, 4, L, &layer));
-  if (cudaMemsetAsync(layer->d, 0, (size_t)16 << L, ctx->stream) != cudaSuccess) { nb200_cols_free(ctx, layer); cleanup_fri(); return set_err(ctx, NB200_ERR_CUDA, "memset"); }
+  const size_t last_domain = (size_t)1 << (s->log_last + s->log_blowup);
+  u32 L = f.qlogs[0] - 1;
+  ColsPtr layer;
+  NB_TRY(alloc(ctx, layer, 4, L));
+  NB_CUDA(ctx, cudaMemsetAsync(layer->d, 0, (size_t)16 << L, ctx->stream));
   size_t ci = 0;
-  std::vector<qm31> last_layer_poly;
   while (((size_t)1 << L) > last_domain) {
-    while (ci < quotients.size() && qlogs[ci] - 1 == L) {
-      nb200_status st = fold_circle_into_line(ctx, layer->d, quotients[ci]->d, qlogs[ci], circle_alpha);
-      if (st != NB200_OK) { nb200_cols_free(ctx, layer); cleanup_fri(); return st; }
-      ++ci;
-    }
-    Layer ly{layer, nullptr, L};
-    inner.push_back(ly);
+    for (; ci < f.quotients.size() && f.qlogs[ci] - 1 == L; ++ci) NB_TRY(fold_circle_into_line(ctx, layer->d, f.quotients[ci]->d, f.qlogs[ci], circle_alpha));
     std::vector<ColRef> refs; for (int k = 0; k < 4; ++k) refs.push_back(ColRef{layer->col(k), L});
-    NB_TRYF(merkle_commit(ctx, refs, &inner.back().tree));
-    ch.mix_root(inner.back().tree->root);
+    const u32* folded = layer->d;
+    f.inner.push_back(FriLayer{std::move(layer), nullptr, L});
+    nb200_tree* tree = nullptr;
+    NB_TRY(merkle_commit(ctx, refs, &tree));
+    f.inner.back().tree.reset(tree);
+    ch.mix_root(tree->root);
     qm31 alpha = ch.draw_felt();
-    nb200_cols* next = nullptr;
-    NB_TRYF(nb200_cols_alloc(ctx, 4, L - 1, &next));
-    nb200_status st = fold_line(ctx, next->d, layer->d, L, alpha);
-    if (st != NB200_OK) { nb200_cols_free(ctx, next); cleanup_fri(); return st; }
-    layer = next; L -= 1;
+    NB_TRY(alloc(ctx, layer, 4, L - 1));
+    NB_TRY(fold_line(ctx, layer->d, folded, L, alpha));
+    L -= 1;
   }
-  {
-    // circle columns that fold exactly into the last layer's size would be an upstream assertion failure
-    nb200_status st = NB200_OK;
-    if (ci != quotients.size()) st = set_err(ctx, NB200_ERR_STATE, "fri: not all columns consumed");
-    if (st == NB200_OK && ((size_t)1 << L) != last_domain) st = set_err(ctx, NB200_ERR_STATE, "fri: last layer size");
-    std::vector<u32> host((size_t)4 << L);
-    if (st == NB200_OK && cudaMemcpyAsync(host.data(), layer->d, host.size() * 4, cudaMemcpyDeviceToHost, ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "d2h");
-    if (st == NB200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "sync");
-    nb200_cols_free(ctx, layer); layer = nullptr;
-    if (st != NB200_OK) { cleanup_fri(); return st; }
-    // LineEvaluation::interpolate on the host (the last layer has 2^(log_last + blowup) points)
-    size_t n = (size_t)1 << L;
-    std::vector<qm31> v(n);
-    for (size_t i2 = 0; i2 < n; ++i2) v[bit_reverse_u32((u32)i2, L)] = qm31_make(host[i2], host[n + i2], host[2 * n + i2], host[3 * n + i2]);
-    HLineDomain d = HLineDomain::make(HCoset::half_odds(L));
-    while (d.size() > 1) {
-      size_t ds = d.size();
-      for (size_t c0 = 0; c0 < n; c0 += ds)
-        for (size_t i2 = 0; i2 < ds / 2; ++i2) {
-          u32 xi = m31_inv(d.at(i2));
-          qm31 a = v[c0 + i2], b = v[c0 + ds / 2 + i2];
-          v[c0 + i2] = qm31_add(a, b);
-          v[c0 + ds / 2 + i2] = qm31_mul_m31(qm31_sub(a, b), xi);
-        }
-      d = d.dbl();
-    }
-    u32 sc = m31_inv((u32)(n % P31));
-    for (auto& qv : v) qv = qm31_mul_m31(qv, sc);
-    // v is the LinePoly storage order (bit-reversed); ordered coefficients = bit-reversed again
-    std::vector<qm31> ordered(n);
-    for (size_t i2 = 0; i2 < n; ++i2) ordered[bit_reverse_u32((u32)i2, L)] = v[i2];
-    size_t bound = (size_t)1 << s->log_last;
-    for (size_t i2 = bound; i2 < n; ++i2) if (!qm31_is_zero(ordered[i2])) { cleanup_fri(); return set_err(ctx, NB200_ERR_CONSTRAINTS, "fri: last layer has invalid degree (constraints not satisfied)"); }
-    last_layer_poly.resize(bound);
-    for (size_t i2 = 0; i2 < bound; ++i2) last_layer_poly[bit_reverse_u32((u32)i2, s->log_last)] = ordered[i2];
-    ch.mix_felts(last_layer_poly.data(), last_layer_poly.size());
+  // circle columns that fold exactly into the last layer's size would be an upstream assertion failure
+  if (ci != f.quotients.size()) return set_err(ctx, NB200_ERR_STATE, "fri: not all columns consumed");
+  if (((size_t)1 << L) != last_domain) return set_err(ctx, NB200_ERR_STATE, "fri: last layer size");
+  std::vector<u32> host((size_t)4 << L);
+  NB_CUDA(ctx, cudaMemcpyAsync(host.data(), layer->d, host.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  layer.reset();
+  // LineEvaluation::interpolate on the host (the last layer has 2^(log_last + blowup) points)
+  size_t n = (size_t)1 << L;
+  std::vector<qm31> v(n);
+  for (size_t i2 = 0; i2 < n; ++i2) v[bit_reverse_u32((u32)i2, L)] = qm31_make(host[i2], host[n + i2], host[2 * n + i2], host[3 * n + i2]);
+  HLineDomain d = HLineDomain::make(HCoset::half_odds(L));
+  while (d.size() > 1) {
+    size_t ds = d.size();
+    for (size_t c0 = 0; c0 < n; c0 += ds)
+      for (size_t i2 = 0; i2 < ds / 2; ++i2) {
+        u32 xi = m31_inv(d.at(i2));
+        qm31 a = v[c0 + i2], b = v[c0 + ds / 2 + i2];
+        v[c0 + i2] = qm31_add(a, b);
+        v[c0 + ds / 2 + i2] = qm31_mul_m31(qm31_sub(a, b), xi);
+      }
+    d = d.dbl();
   }
-
+  u32 sc = m31_inv((u32)(n % P31));
+  for (auto& qv : v) qv = qm31_mul_m31(qv, sc);
+  // v is the LinePoly storage order (bit-reversed); ordered coefficients = bit-reversed again
+  std::vector<qm31> ordered(n);
+  for (size_t i2 = 0; i2 < n; ++i2) ordered[bit_reverse_u32((u32)i2, L)] = v[i2];
+  size_t bound = (size_t)1 << s->log_last;
+  for (size_t i2 = bound; i2 < n; ++i2) if (!qm31_is_zero(ordered[i2])) return set_err(ctx, NB200_ERR_CONSTRAINTS, "fri: last layer has invalid degree (constraints not satisfied)");
+  last_layer_poly.resize(bound);
+  for (size_t i2 = 0; i2 < bound; ++i2) last_layer_poly[bit_reverse_u32((u32)i2, s->log_last)] = ordered[i2];
+  ch.mix_felts(last_layer_poly.data(), last_layer_poly.size());
   trace_mark(ctx, "fri commit");
-  // ---------------- proof of work, queries, decommitments ----------------
+  return NB200_OK;
+}
+
+// the parts of the StarkProof that the proof-of-work, query and decommitment stage produces
+struct Decommitments {
   uint64_t nonce = 0;
-  NB_TRYF(grind(ctx, ch.digest.data(), s->pow_bits, &nonce));
-  ch.mix_u64(nonce);
-  const u32 max_log = qlogs[0];
+  FriLayerProof first_layer;
+  std::vector<FriLayerProof> inner_layers;
+  std::vector<std::vector<u32>> queried_values;   // per tree
+  std::vector<Decommitment> trees;                // per tree
+};
+
+static nb200_status decommit(nb200_scheme* s, HostChannel& ch, const FriState& f, Decommitments& out) {
+  nb200_ctx* ctx = s->ctx;
+  const u32 blow = s->log_blowup;
+  NB_TRY(grind(ctx, ch.digest.data(), s->pow_bits, &out.nonce));
+  ch.mix_u64(out.nonce);
+  const u32 max_log = f.qlogs[0];
   Queries queries = Queries::generate(ch, max_log, s->n_queries);
   std::vector<std::pair<u32, std::vector<u64>>> by_log;
-  for (u32 lg : qlogs) by_log.push_back({lg, queries.fold(max_log - lg).positions});
+  for (u32 lg : f.qlogs) by_log.push_back({lg, queries.fold(max_log - lg).positions});
 
-  FriLayerProof first_proof; std::vector<FriLayerProof> inner_proofs(inner.size());
   {
     std::vector<std::pair<u32, std::vector<u64>>> dpos;
-    for (size_t g = 0; g < quotients.size(); ++g) {
+    for (size_t g = 0; g < f.quotients.size(); ++g) {
       std::vector<u64> pos;
-      NB_TRYF(positions_and_witness(ctx, quotients[g], queries.fold(max_log - qlogs[g]).positions, pos, first_proof.fri_witness));
-      dpos.push_back({qlogs[g], pos});
+      NB_TRY(positions_and_witness(ctx, f.quotients[g].get(), queries.fold(max_log - f.qlogs[g]).positions, pos, out.first_layer.fri_witness));
+      dpos.push_back({f.qlogs[g], pos});
     }
     std::vector<ColRef> refs;
-    for (size_t g = 0; g < quotients.size(); ++g) for (int k = 0; k < 4; ++k) refs.push_back(ColRef{quotients[g]->col(k), qlogs[g]});
+    for (size_t g = 0; g < f.quotients.size(); ++g) for (int k = 0; k < 4; ++k) refs.push_back(ColRef{f.quotients[g]->col(k), f.qlogs[g]});
     std::vector<u32> qv;
-    NB_TRYF(merkle_decommit(ctx, first_tree, refs, dpos, qv, first_proof.decommitment.hash_witness, first_proof.decommitment.column_witness));
-    memcpy(first_proof.commitment, first_tree->root, 32);
+    NB_TRY(merkle_decommit(ctx, f.first_tree.get(), refs, dpos, qv, out.first_layer.decommitment.hash_witness, out.first_layer.decommitment.column_witness));
+    memcpy(out.first_layer.commitment, f.first_tree->root, 32);
   }
+  out.inner_layers.resize(f.inner.size());
   {
     Queries lq = queries.fold(1);
-    for (size_t k = 0; k < inner.size(); ++k) {
+    for (size_t k = 0; k < f.inner.size(); ++k) {
+      const FriLayer& ly = f.inner[k];
+      FriLayerProof& lp = out.inner_layers[k];
       std::vector<u64> pos;
-      NB_TRYF(positions_and_witness(ctx, inner[k].cols, lq.positions, pos, inner_proofs[k].fri_witness));
-      std::vector<std::pair<u32, std::vector<u64>>> dpos{{inner[k].log, pos}};
-      std::vector<ColRef> refs; for (int c = 0; c < 4; ++c) refs.push_back(ColRef{inner[k].cols->col(c), inner[k].log});
+      NB_TRY(positions_and_witness(ctx, ly.cols.get(), lq.positions, pos, lp.fri_witness));
+      std::vector<std::pair<u32, std::vector<u64>>> dpos{{ly.log, pos}};
+      std::vector<ColRef> refs; for (int c = 0; c < 4; ++c) refs.push_back(ColRef{ly.cols->col(c), ly.log});
       std::vector<u32> qv;
-      NB_TRYF(merkle_decommit(ctx, inner[k].tree, refs, dpos, qv, inner_proofs[k].decommitment.hash_witness, inner_proofs[k].decommitment.column_witness));
-      memcpy(inner_proofs[k].commitment, inner[k].tree->root, 32);
+      NB_TRY(merkle_decommit(ctx, ly.tree.get(), refs, dpos, qv, lp.decommitment.hash_witness, lp.decommitment.column_witness));
+      memcpy(lp.commitment, ly.tree->root, 32);
       lq = lq.fold(1);
     }
   }
-  std::vector<std::vector<u32>> queried_values(4); std::vector<Decommitment> decommitments(4);
+  out.queried_values.resize(4); out.trees.resize(4);
   for (int t = 0; t < 4; ++t) {
-    std::vector<ColRef> refs;
-    if (!s->trees[t].sharded) for (size_t g = 0; g < s->trees[t].cols.size(); ++g) refs.push_back(ColRef{s->trees[t].lde_ptr(g), s->trees[t].cols[g].log + blow});
-    if (s->trees[t].sharded) NB_TRYF(merkle_decommit_sharded(ctx, s->trees[t], blow, by_log, queried_values[t], decommitments[t].hash_witness, decommitments[t].column_witness));
-    else NB_TRYF(merkle_decommit(ctx, s->trees[t].merkle, refs, by_log, queried_values[t], decommitments[t].hash_witness, decommitments[t].column_witness));
-  }
-  cleanup_fri();
-#undef NB_TRYF
-
-  trace_mark(ctx, "pow + decommit");
-  // ---------------- sanity check: composition(oods) == recomputed from the sampled mask values ----------------
-  {
-    qm31 accumulation = qm31_zero();
-    for (const AirComponent& c : air.comps) {
-      std::vector<qm31> mask(c.masks.size());
-      for (size_t m = 0; m < c.masks.size(); ++m) {
-        const auto& o = offs[c.masks[m].tree][c.masks[m].col];
-        size_t k = std::find(o.begin(), o.end(), c.masks[m].off) - o.begin();
-        mask[m] = sampled[c.masks[m].tree][c.masks[m].col][k];
-      }
-      qm31 dinv = qm31_inv(coset_vanishing_q(c.log_size, oods));
-      std::vector<qm31> br(c.n_base_regs), er(c.n_ext_regs);
-      run_point(c.prog, mask.data(), params, br, er, [&](qm31 v) { accumulation = qm31_add(qm31_mul(accumulation, random_coeff), qm31_mul(dinv, v)); });
+    const SchemeTree& tr = s->trees[t];
+    if (tr.sharded) NB_TRY(merkle_decommit_sharded(ctx, tr, blow, by_log, out.queried_values[t], out.trees[t].hash_witness, out.trees[t].column_witness));
+    else {
+      std::vector<ColRef> refs;
+      for (size_t g = 0; g < tr.cols.size(); ++g) refs.push_back(ColRef{tr.lde_ptr(g), tr.cols[g].log + blow});
+      NB_TRY(merkle_decommit(ctx, tr.merkle.get(), refs, by_log, out.queried_values[t], out.trees[t].hash_witness, out.trees[t].column_witness));
     }
-    qm31 cv[4] = {sampled[3][0][0], sampled[3][1][0], sampled[3][2][0], sampled[3][3][0]};
-    if (!qm31_eq(from_partial_evals(cv), accumulation)) return set_err(ctx, NB200_ERR_CONSTRAINTS, "ConstraintsNotSatisfied");
   }
+  return NB200_OK;
+}
 
-  // ---------------- StarkProof -> postcard ----------------
+// sanity check: composition(oods) == recomputed from the sampled mask values
+static nb200_status check_oods(nb200_ctx* ctx, const AirProgram& air, const std::vector<qm31>& params, qm31 random_coeff, const OodsSamples& o) {
+  qm31 accumulation = qm31_zero();
+  for (const AirComponent& c : air.comps) {
+    std::vector<qm31> mask(c.masks.size());
+    for (size_t m = 0; m < c.masks.size(); ++m) {
+      const auto& off = o.offs[c.masks[m].tree][c.masks[m].col];
+      size_t k = std::find(off.begin(), off.end(), c.masks[m].off) - off.begin();
+      mask[m] = o.sampled[c.masks[m].tree][c.masks[m].col][k];
+    }
+    qm31 dinv = qm31_inv(coset_vanishing_q(c.log_size, o.point));
+    std::vector<qm31> br(c.n_base_regs), er(c.n_ext_regs);
+    run_point(c.prog, mask.data(), params, br, er, [&](qm31 v) { accumulation = qm31_add(qm31_mul(accumulation, random_coeff), qm31_mul(dinv, v)); });
+  }
+  const auto& comp = o.sampled[3];
+  qm31 cv[4] = {comp[0][0], comp[1][0], comp[2][0], comp[3][0]};
+  if (!qm31_eq(from_partial_evals(cv), accumulation)) return set_err(ctx, NB200_ERR_CONSTRAINTS, "ConstraintsNotSatisfied");
+  return NB200_OK;
+}
+
+// StarkProof -> postcard
+static std::vector<uint8_t> serialize_proof(const nb200_scheme* s, const OodsSamples& o, const std::vector<qm31>& last_layer_poly, const Decommitments& d) {
   Postcard pc;
   pc.varint(s->pow_bits); pc.varint(s->log_blowup); pc.varint(s->log_last); pc.varint(s->n_queries);
   pc.varint(4); for (int t = 0; t < 4; ++t) pc.hash(s->trees[t].merkle->root);
   pc.varint(4);
-  for (int t = 0; t < 4; ++t) { pc.varint(sampled[t].size()); for (auto& c : sampled[t]) { pc.varint(c.size()); for (auto& v : c) pc.q(v); } }
-  pc.varint(4); for (int t = 0; t < 4; ++t) put_decommitment(pc, decommitments[t]);
-  pc.varint(4); for (int t = 0; t < 4; ++t) { pc.varint(queried_values[t].size()); for (u32 v : queried_values[t]) pc.varint(v); }
-  pc.varint(nonce);
-  put_fri_layer(pc, first_proof);
-  pc.varint(inner_proofs.size()); for (auto& l : inner_proofs) put_fri_layer(pc, l);
+  for (int t = 0; t < 4; ++t) { pc.varint(o.sampled[t].size()); for (auto& c : o.sampled[t]) { pc.varint(c.size()); for (auto& v : c) pc.q(v); } }
+  pc.varint(4); for (int t = 0; t < 4; ++t) put_decommitment(pc, d.trees[t]);
+  pc.varint(4); for (int t = 0; t < 4; ++t) { pc.varint(d.queried_values[t].size()); for (u32 v : d.queried_values[t]) pc.varint(v); }
+  pc.varint(d.nonce);
+  put_fri_layer(pc, d.first_layer);
+  pc.varint(d.inner_layers.size()); for (auto& l : d.inner_layers) put_fri_layer(pc, l);
   pc.varint(last_layer_poly.size()); for (auto& v : last_layer_poly) pc.q(v);
   pc.varint(s->log_last);
-  proof_bytes.swap(pc.out);
+  return std::move(pc.out);
+}
+
+// stwo::prover::prove
+nb200_status prove_impl(nb200_scheme* s, nb200_air* air_h, const std::vector<qm31>& params, HostChannel& ch, std::vector<uint8_t>& proof_bytes) {
+  nb200_ctx* ctx = s->ctx;
+  const AirProgram& air = air_h->prog;
+  NB_ARG(ctx, s->trees.size() == 3, "prove: the preprocessed, main and interaction trees must be committed first");
+  NB_ARG(ctx, params.size() == air.n_params, "prove: parameter table size");
+  size_t n_total = 0;
+  for (auto& c : air.comps) n_total += c.n_constraints;
+  NB_ARG(ctx, n_total > 0, "prove: no constraints");
+
+  trace_mark(ctx, nullptr);
+  const qm31 random_coeff = ch.draw_felt();
+  NB_TRY(commit_composition(s, air_h, params, random_coeff, n_total, ch));   // tree 3 stays in the scheme even if a later stage fails
+  OodsSamples oods;
+  NB_TRY(sample_oods(s, air, ch, oods));
+  std::vector<qm31> last_layer_poly;
+  Decommitments dec;
+  {
+    FriState fri;
+    NB_TRY(deep_quotients(s, oods, ch, fri));
+    NB_TRY(fri_commit(s, ch, fri, last_layer_poly));
+    NB_TRY(decommit(s, ch, fri, dec));
+  }
+  trace_mark(ctx, "pow + decommit");
+  NB_TRY(check_oods(ctx, air, params, random_coeff, oods));
+  proof_bytes = serialize_proof(s, oods, last_layer_poly, dec);
   trace_mark(ctx, "sanity + serialize");
   return NB200_OK;
 }
@@ -1093,7 +1114,6 @@ nb200_status gen_interaction(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, con
                              const std::vector<qm31>& params, nb200_cols** out, qm31* claimed) {
   const AirProgram& air = air_h->prog;
   NB_ARG(ctx, comp_idx < air.comps.size(), "gen_interaction: component index");
-  if (air_h->jit_logup.size() != air.comps.size()) air_h->jit_logup.resize(air.comps.size());
   const AirComponent& c = air.comps[comp_idx];
   std::vector<std::vector<const u32*>> flat(2);
   std::vector<std::vector<u32>> flog(2);
@@ -1107,27 +1127,17 @@ nb200_status gen_interaction(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, con
     NB_ARG(ctx, flog[mk.tree][mk.col] == c.log_size, "gen_interaction: column size differs from the component's log_size");
     mask_cols[m] = flat[mk.tree][mk.col];
   }
-  u32* d_params = nullptr;
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_params, std::max<size_t>(params.size(), 1) * 16));
-  if (!params.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_params, params.data(), params.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
-  nb200_cols* o = nullptr;
-  NB_TRY(nb200_cols_alloc(ctx, (size_t)4 * c.n_logup_cols(), c.log_size, &o));
+  DevBuf d_params;
+  NB_TRY(upload_params(ctx, params.data(), params.size(), d_params));
+  ColsPtr o;
+  NB_TRY(alloc(ctx, o, (size_t)4 * c.n_logup_cols(), c.log_size));
   trace_mark(ctx, nullptr);
-  JitKernel& jk = air_h->jit_logup[comp_idx];
-  if (!jk.tried) {
-    jk.tried = true;
-    if (c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0 && jit_enabled()) {
-      nb200_status js = jit_compile_logup(ctx, c, &jk);
-      if (js != NB200_OK && ctx->trace) fprintf(stderr, "[nb200] jit unavailable for logup program: %s\n", ctx->err.c_str());
-      trace_mark(ctx, "jit: compile logup (one-time)");
-    }
-  }
-  nb200_status st = logup_generate(ctx, c, mask_cols, d_params, o->d, claimed, jk.kernel ? &jk : nullptr);
+  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, true, true);
+  nb200_status st = logup_generate(ctx, c, mask_cols, d_params.p, o->d, claimed, jk);
   trace_mark(ctx, "logup interaction trace");
   cudaStreamSynchronize(ctx->stream);
-  dfree(ctx, d_params);
-  if (st != NB200_OK) { nb200_cols_free(ctx, o); return st; }
-  *out = o;
+  NB_TRY(st);
+  *out = o.release();
   return NB200_OK;
 }
 
@@ -1138,7 +1148,6 @@ nb200_status gen_interaction_sharded(nb200_scheme* s, nb200_air* air_h, u32 comp
   nb200_ctx* ctx = s->ctx;
   const AirProgram& air = air_h->prog;
   NB_ARG(ctx, comp_idx < air.comps.size() && s->trees.size() >= 2, "gen_interaction_sharded: commit trees 0 and 1 first");
-  if (air_h->jit_logup.size() != air.comps.size()) air_h->jit_logup.resize(air.comps.size());
   const AirComponent& c = air.comps[comp_idx];
   const u32 n = c.log_size, k = (u32)comm_log_world(ctx);
   const int world = comm_world(ctx), rank = comm_rank(ctx);
@@ -1151,24 +1160,22 @@ nb200_status gen_interaction_sharded(nb200_scheme* s, nb200_air* air_h, u32 comp
     if (mk.tree == 2 || mk.off != 0) continue;
     const SchemeTree& tr = s->trees[mk.tree];
     NB_ARG(ctx, tr.sharded && mk.col < tr.cols.size() && tr.cols[mk.col].batch == SchemeTree::BIG && tr.big_eval_rows, "gen_interaction_sharded: the component may only read sharded trace columns (commit with keep_eval_rows)");
-    mask_cols[m] = tr.big_eval_rows->d + (size_t)tr.cols[mk.col].idx * Sn;
+    mask_cols[m] = tr.big_eval_rows->col(tr.cols[mk.col].idx);   // this rank's trace rows
   }
-  JitKernel& jk = air_h->jit_logup[comp_idx];
-  if (!jk.tried) { jk.tried = true; if (jit_enabled()) jit_compile_logup(ctx, c, &jk); }
-  NB_ARG(ctx, jk.kernel != nullptr, "gen_interaction_sharded needs the specialised logup kernel");
-  u32* d_params = nullptr;
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_params, std::max<size_t>(params.size(), 1) * 16));
-  if (!params.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_params, params.data(), params.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
-  ColsGuard rows(ctx), last(ctx), shard(ctx);
-  nb200_status st = nb200_cols_alloc(ctx, total, n - k, &rows.c);
+  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, true, false);
+  NB_ARG(ctx, jk != nullptr, "gen_interaction_sharded needs the specialised logup kernel");
+  DevBuf d_params;
+  NB_TRY(upload_params(ctx, params.data(), params.size(), d_params));
+  ColsPtr rows, last, shard;
+  NB_TRY(alloc(ctx, rows, total, n - k));
   trace_mark(ctx, nullptr);
-  if (st == NB200_OK) st = logup_rows(ctx, c, mask_cols, d_params, rows.c->d, n - k, &jk);
+  NB_TRY(logup_rows(ctx, c, mask_cols, d_params.p, rows->d, n - k, jk));
   // finalize_last on the whole last secure column (every rank, redundantly), then this rank's rows go back into the row batch
-  if (st == NB200_OK) st = nb200_cols_alloc(ctx, 4, n, &last.c);
-  for (int q = 0; q < 4 && st == NB200_OK; ++q) st = comm_all_gather_dev(ctx, rows.c->col(total - 4 + q), Sn, last.c->col(q));
-  if (st == NB200_OK) st = logup_finalize_last(ctx, n, last.c->d, claimed);
-  for (int q = 0; q < 4 && st == NB200_OK; ++q)
-    if (cudaMemcpyAsync(rows.c->col(total - 4 + q), last.c->col(q) + (size_t)rank * Sn, Sn * 4, cudaMemcpyDeviceToDevice, ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "gen_interaction_sharded: copy");
+  NB_TRY(alloc(ctx, last, 4, n));
+  for (int q = 0; q < 4; ++q) NB_TRY(comm_all_gather_dev(ctx, rows->col(total - 4 + q), Sn, last->col(q)));
+  NB_TRY(logup_finalize_last(ctx, n, last->d, claimed));
+  for (int q = 0; q < 4; ++q)
+    NB_CUDA(ctx, cudaMemcpyAsync(rows->col(total - 4 + q), last->col(q) + (size_t)rank * Sn, Sn * 4, cudaMemcpyDeviceToDevice, ctx->stream));
   trace_mark(ctx, "logup interaction trace (sharded rows)");
   // rows -> this rank's column shard
   size_t first = 0, count = 0;
@@ -1176,21 +1183,21 @@ nb200_status gen_interaction_sharded(nb200_scheme* s, nb200_air* air_h, u32 comp
   PeerBuf pb_shard;
   size_t maxc = 0;
   for (int r = 0; r < world; ++r) { size_t f, cn; comm_shard_range(total, world, r, &f, &cn); maxc = std::max(maxc, cn); }
-  if (st == NB200_OK) st = peer_alloc(ctx, s, maxc << n, &pb_shard);      // the same size on every rank (symmetric offsets)
-  if (st == NB200_OK && pb_shard.d) {
+  NB_TRY(peer_alloc(ctx, s, maxc << n, &pb_shard));      // the same size on every rank (symmetric offsets)
+  if (pb_shard.d) {
     // peer heap: my rows of rank q's columns go straight into q's shard (copy engines over NVLink); valid until the scheme is freed
-    st = nb200_cols_from_device(ctx, pb_shard.d, count, n, &shard.c);
-    if (st == NB200_OK) st = comm_barrier_stream(ctx);
-    if (st == NB200_OK) st = peer_rows_to_cols(ctx, ctx->stream, rows.c->d, total, N, pb_shard);
-    if (st == NB200_OK) st = comm_barrier_stream(ctx);
+    nb200_cols* sc = nullptr;
+    NB_TRY(nb200_cols_from_device(ctx, pb_shard.d, count, n, &sc));
+    shard.reset(sc);
+    NB_TRY(comm_barrier_stream(ctx));
+    NB_TRY(peer_rows_to_cols(ctx, ctx->stream, rows->d, total, N, pb_shard));
+    NB_TRY(comm_barrier_stream(ctx));
   } else {
-    if (st == NB200_OK) st = nb200_cols_alloc(ctx, count, n, &shard.c);
-    if (st == NB200_OK) st = exchange_rows_to_cols(ctx, rows.c->d, total, N, shard.c->d);
+    NB_TRY(alloc(ctx, shard, count, n));
+    NB_TRY(exchange_rows_to_cols(ctx, rows->d, total, N, shard->d));
   }
   cudaStreamSynchronize(ctx->stream);
   trace_mark(ctx, "logup: rows -> columns exchange");
-  dfree(ctx, d_params);
-  if (st != NB200_OK) return st;
   *shard_out = shard.release();
   return NB200_OK;
 }
@@ -1281,7 +1288,7 @@ uint32_t nb200_air_max_log_expand(const nb200_air* a) {
 }
 void nb200_scheme_free(nb200_scheme* s) {
   if (!s) return;
-  for (auto& t : s->trees) free_tree(s->ctx, t);
+  s->trees.clear();
   peer_heap_release(s->ctx, s);
   delete s;
 }
@@ -1332,12 +1339,11 @@ nb200_status nb200_fold_line(nb200_ctx* ctx, const nb200_cols* src, const uint32
   if (!ctx || !src || !alpha || !dst_out) return NB200_ERR_ARG;
   NB_ARG(ctx, src->n_cols == 4 && src->log_size >= 1, "fold_line: src must be a secure column (4 coordinate columns) of at least 2 values");
   NB_TRY(twiddles_prepare(ctx, src->log_size + 1));
-  nb200_cols* d = nullptr;
-  NB_TRY(nb200_cols_alloc(ctx, 4, src->log_size - 1, &d));
+  ColsPtr d;
+  NB_TRY(alloc(ctx, d, 4, src->log_size - 1));
   qm31 a; memcpy(a.c, alpha, 16);
-  nb200_status st = fold_line(ctx, d->d, src->d, src->log_size, a);
-  if (st != NB200_OK) { nb200_cols_free(ctx, d); return st; }
-  *dst_out = d;
+  NB_TRY(fold_line(ctx, d->d, src->d, src->log_size, a));
+  *dst_out = d.release();
   return NB200_OK;
 }
 nb200_status nb200_fold_circle_into_line(nb200_ctx* ctx, nb200_cols* dst, const nb200_cols* src, const uint32_t alpha[4]) {
@@ -1377,11 +1383,10 @@ nb200_status nb200_fri_quotients(nb200_ctx* ctx, const nb200_cols* const* batche
     }
   }
   qm31 rc; memcpy(rc.c, random_coeff, 16);
-  nb200_cols* q = nullptr;
-  NB_TRY(nb200_cols_alloc(ctx, 4, log_size, &q));
-  nb200_status st = accumulate_quotients(ctx, log_size, hb, rc, q->d);
-  if (st != NB200_OK) { nb200_cols_free(ctx, q); return st; }
-  *out = q;
+  ColsPtr q;
+  NB_TRY(alloc(ctx, q, 4, log_size));
+  NB_TRY(accumulate_quotients(ctx, log_size, hb, rc, q->d));
+  *out = q.release();
   return NB200_OK;
 }
 nb200_status nb200_constraint_quotients(nb200_scheme* s, const nb200_air* air, uint32_t component, const uint32_t* params, size_t n_params,
@@ -1391,15 +1396,12 @@ nb200_status nb200_constraint_quotients(nb200_scheme* s, const nb200_air* air, u
   NB_ARG(ctx, n_params == air->prog.n_params, "constraint quotients: parameter table size");
   std::vector<qm31> cf(n_coeffs);
   if (n_coeffs) memcpy(cf.data(), coeffs, n_coeffs * 16);
-  u32* d_params = nullptr;
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_params, std::max<size_t>(n_params, 1) * 16));
-  nb200_status st = NB200_OK;
-  if (n_params && cudaMemcpyAsync(d_params, params, n_params * 16, cudaMemcpyHostToDevice, ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "h2d");
-  if (st == NB200_OK) st = component_quotients(s, const_cast<nb200_air*>(air), component, d_params, cf, Q_FULL, accum, nullptr);
+  DevBuf d_params;
+  NB_TRY(upload_params(ctx, params, n_params, d_params));
+  NB_TRY(component_quotients(s, const_cast<nb200_air*>(air), component, d_params.p, cf, Q_FULL, accum, nullptr));
   // params is caller memory: make sure the copy has been consumed before returning
-  if (st == NB200_OK && cudaStreamSynchronize(ctx->stream) != cudaSuccess) st = set_err(ctx, NB200_ERR_CUDA, "sync");
-  dfree(ctx, d_params);
-  return st;
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return NB200_OK;
 }
 
 }  // extern "C"
