@@ -16,6 +16,8 @@
 #include <cstdio>
 #include <nvrtc.h>
 #include <sstream>
+#include <functional>
+#include <map>
 #include <cstdlib>
 
 namespace nb {
@@ -142,53 +144,217 @@ void emit_op(std::ostringstream& o, const AirInstr& in, Ld ld) {
 // registers alive somewhere (shared selectors such as IsTypeR), and copying all 90 words in and out of local memory at each of its 19 chunk
 // boundaries cost more than the arithmetic (the synthetic ADD machine has 4 + 4 and never showed it).
 struct ChunkLive { std::vector<std::vector<u32>> in_b, in_e, out_b, out_e; };
-static void instr_regs(const AirInstr& in, std::vector<u32>& rb, std::vector<u32>& re, int& wb, int& we) {
-  wb = we = -1;
-  switch (in.op) {
-    case OP_LOADM: case OP_CONSTB: wb = (int)in.dst; break;
-    case OP_ADDB: case OP_SUBB: case OP_MULB: rb = {in.a, in.b}; wb = (int)in.dst; break;
-    case OP_NEGB: rb = {in.a}; wb = (int)in.dst; break;
-    case OP_PARAME: case OP_LOADME: we = (int)in.dst; break;
-    case OP_ADDE: case OP_SUBE: case OP_MULE: re = {in.a, in.b}; we = (int)in.dst; break;
-    case OP_NEGE: re = {in.a}; we = (int)in.dst; break;
-    case OP_ADDEB: case OP_SUBEB: case OP_MULEB: re = {in.a}; rb = {in.b}; we = (int)in.dst; break;
-    case OP_BTOE: rb = {in.a}; we = (int)in.dst; break;
-    case OP_CONSTRB: rb = {in.a}; break;
-    case OP_CONSTRE: re = {in.a}; break;
-    case OP_FRAC: re = {in.a, in.b}; break;
+struct Regs { std::vector<u32> rb, re; int wb = -1, we = -1; };   // registers a statement reads and writes (base / secure)
+// register kind ('b' base, 'e' secure, 0 none) of operands a and b and of the destination
+static void operand_kinds(u32 op, char& ka, char& kb, char& kd) {
+  ka = kb = kd = 0;
+  switch (op) {
+    case OP_LOADM: case OP_CONSTB: kd = 'b'; break;
+    case OP_ADDB: case OP_SUBB: case OP_MULB: ka = kb = kd = 'b'; break;
+    case OP_NEGB: ka = kd = 'b'; break;
+    case OP_PARAME: case OP_LOADME: kd = 'e'; break;
+    case OP_ADDE: case OP_SUBE: case OP_MULE: ka = kb = kd = 'e'; break;
+    case OP_NEGE: ka = kd = 'e'; break;
+    case OP_ADDEB: case OP_SUBEB: case OP_MULEB: ka = kd = 'e'; kb = 'b'; break;
+    case OP_BTOE: ka = 'b'; kd = 'e'; break;
+    case OP_CONSTRB: ka = 'b'; break;
+    case OP_CONSTRE: ka = 'e'; break;
+    case OP_FRAC: ka = kb = 'e'; break;
     default: break;
   }
 }
-static ChunkLive chunk_liveness(const std::vector<AirInstr>& prog, size_t CH, u32 nb, u32 ne) {
-  const size_t n_chunks = (prog.size() + CH - 1) / CH;
+static Regs instr_regs(const AirInstr& in) {
+  Regs r;
+  char ka, kb, kd;
+  operand_kinds(in.op, ka, kb, kd);
+  if (ka) (ka == 'b' ? r.rb : r.re).push_back(in.a);
+  if (kb) (kb == 'b' ? r.rb : r.re).push_back(in.b);
+  if (kd) (kd == 'b' ? r.wb : r.we) = (int)in.dst;
+  return r;
+}
+// stmts[begin[ci] .. begin[ci + 1]) make up chunk ci
+static ChunkLive chunk_liveness(const std::vector<Regs>& stmts, const std::vector<size_t>& begin, u32 nb, u32 ne) {
+  const size_t n_chunks = begin.size() - 1;
   ChunkLive L; L.in_b.resize(n_chunks); L.in_e.resize(n_chunks); L.out_b.resize(n_chunks); L.out_e.resize(n_chunks);
   std::vector<char> lb(nb + 1, 0), le(ne + 1, 0);
   std::vector<std::vector<char>> after_b(n_chunks), after_e(n_chunks);   // live sets at the END of each chunk
   for (size_t ci = n_chunks; ci-- > 0;) {
     after_b[ci] = lb; after_e[ci] = le;
-    for (size_t pc = std::min(prog.size(), (ci + 1) * CH); pc-- > ci * CH;) {
-      std::vector<u32> rb, re; int wb, we;
-      instr_regs(prog[pc], rb, re, wb, we);
-      if (wb >= 0) lb[wb] = 0;
-      if (we >= 0) le[we] = 0;
-      for (u32 r : rb) lb[r] = 1;
-      for (u32 r : re) le[r] = 1;
+    for (size_t pc = begin[ci + 1]; pc-- > begin[ci];) {
+      const Regs& r = stmts[pc];
+      if (r.wb >= 0) lb[r.wb] = 0;
+      if (r.we >= 0) le[r.we] = 0;
+      for (u32 x : r.rb) lb[x] = 1;
+      for (u32 x : r.re) le[x] = 1;
     }
     for (u32 r = 0; r < nb; ++r) if (lb[r]) L.in_b[ci].push_back(r);
     for (u32 r = 0; r < ne; ++r) if (le[r]) L.in_e[ci].push_back(r);
   }
   for (size_t ci = 0; ci < n_chunks; ++ci) {
     std::vector<char> wrb(nb + 1, 0), wre(ne + 1, 0);
-    for (size_t pc = ci * CH; pc < std::min(prog.size(), (ci + 1) * CH); ++pc) {
-      std::vector<u32> rb, re; int wb, we;
-      instr_regs(prog[pc], rb, re, wb, we);
-      if (wb >= 0) wrb[wb] = 1;
-      if (we >= 0) wre[we] = 1;
+    for (size_t pc = begin[ci]; pc < begin[ci + 1]; ++pc) {
+      if (stmts[pc].wb >= 0) wrb[stmts[pc].wb] = 1;
+      if (stmts[pc].we >= 0) wre[stmts[pc].we] = 1;
     }
     for (u32 r = 0; r < nb; ++r) if (wrb[r] && after_b[ci][r]) L.out_b[ci].push_back(r);
     for (u32 r = 0; r < ne; ++r) if (wre[r] && after_e[ci][r]) L.out_e[ci].push_back(r);
   }
   return L;
+}
+// one statement per instruction, chunks of CH instructions
+static ChunkLive prog_liveness(const std::vector<AirInstr>& prog, size_t CH, u32 nb, u32 ne) {
+  std::vector<Regs> regs;
+  for (const AirInstr& in : prog) regs.push_back(instr_regs(in));
+  std::vector<size_t> begin;
+  for (size_t pc = 0; pc < prog.size(); pc += CH) begin.push_back(pc);
+  begin.push_back(prog.size());
+  return chunk_liveness(regs, begin, nb, ne);
+}
+
+// ---- folding the random coefficient into LogUp denominators
+// finalize_logup_batched (air.py) emits every LogUp constraint of a single fraction as coeff * (diff * den - num), where
+// den = sum_i alpha^i v_i - z is linear in the parameters with base-field v_i, and num is a base value.  In the field
+//   coeff * (diff * den - num) = diff * (coeff * den) - coeff * num,   coeff * den = sum_i (coeff alpha^i) v_i - coeff z,
+// so once the products coeff * alpha^i and coeff * z are known, coeff * den costs the 4 products per term that den costs and the
+// constraint's full QM31 product by its coefficient disappears (16 products and 4 reductions per row).  The kernel computes those
+// products once per CTA into shared memory (nbfold); field arithmetic is exact, so every accumulator word stays the same.
+// A constraint folds when, by reaching definitions (registers are reused, so a register number alone names nothing):
+//   CONSTRE(SUBE(MULE(diff, den) or MULE(den, diff), BTOE(base))), den an ADDE / SUBE tree over MULEB(PARAME, base) and PARAME,
+// and the SUBE and MULE results have no other reader.  Fractions batched in pairs (den a product of two denominators) do not.
+// The den's own terms and partial sums may be shared with other constraints (air.py merges equal nodes), so they are not scaled in
+// place: coeff * den is summed afresh at the MULE from the base values the den read, and a base value whose register is rewritten
+// before that point is first copied to a register of its own.  Whatever only the folded dens read is then dropped as dead code.
+struct Stmt { std::string code; Regs r; bool effect = false; };   // effect: adds to rr (never removed as dead)
+struct ConstraintPlan {
+  std::vector<std::vector<Stmt>> at;               // the statements emitted at each program position
+  u32 nb = 0;                                      // base registers, the copies of folded base values included
+  std::vector<std::pair<u32, u32>> slots;          // nbfold[i] = coeff[slots[i].first] * params[slots[i].second]
+};
+
+template <class Ld>
+static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32 ne) {
+  const std::vector<AirInstr>& prog = c.prog;
+  const int n = (int)prog.size();
+  // def_a / def_b[pc]: position of the instruction whose result operand a / b of prog[pc] reads (-1: none);
+  // uses[d]: readers of the result of d; next_def[d]: position of the next write to d's destination register
+  std::vector<int> def_a(n, -1), def_b(n, -1), uses(n, 0), next_def(n, n);
+  {
+    std::vector<int> cur_b(nb, -1), cur_e(ne, -1);
+    for (int pc = 0; pc < n; ++pc) {
+      const AirInstr& in = prog[pc];
+      char ka, kb, kd;
+      operand_kinds(in.op, ka, kb, kd);
+      if (ka) { def_a[pc] = (ka == 'b' ? cur_b : cur_e)[in.a]; if (def_a[pc] >= 0) ++uses[def_a[pc]]; }
+      if (kb) { def_b[pc] = (kb == 'b' ? cur_b : cur_e)[in.b]; if (def_b[pc] >= 0) ++uses[def_b[pc]]; }
+      if (kd) {
+        int& cur = (kd == 'b' ? cur_b : cur_e)[in.dst];
+        if (cur >= 0) next_def[cur] = pc;
+        cur = pc;
+      }
+    }
+  }
+  ConstraintPlan pl;
+  pl.nb = nb;
+  pl.at.resize(n);
+  u32 k = 0;
+  std::vector<u32> coeff_of(n, 0);   // constraint index of each CONSTRB / CONSTRE
+  for (int pc = 0; pc < n; ++pc) {
+    const AirInstr& in = prog[pc];
+    std::ostringstream o;
+    bool effect = false;
+    switch (in.op) {
+      case OP_CONSTRB: o << "rr = qadd(rr, qmulb(ldq(coeff + " << JIT_COEFF_WORDS * k << "), b[" << in.a << "]));"; coeff_of[pc] = k++; effect = true; break;
+      case OP_CONSTRE: o << "rr = qmac_tab(rr, e[" << in.a << "], coeff + " << JIT_COEFF_WORDS * k << ");"; coeff_of[pc] = k++; effect = true; break;
+      default: emit_op(o, in, ld); break;
+    }
+    pl.at[pc].push_back(Stmt{o.str(), instr_regs(in), effect});
+  }
+
+  struct Term { bool neg; u32 param; int bdef; };   // -/+ params[param] * (bdef < 0 ? 1 : the base value prog[bdef] wrote)
+  std::function<bool(int, bool, std::vector<Term>&)> linear = [&](int q, bool neg, std::vector<Term>& t) {
+    if (q < 0) return false;
+    switch (prog[q].op) {
+      case OP_PARAME: t.push_back(Term{neg, prog[q].a, -1}); return true;
+      case OP_MULEB:
+        if (def_a[q] < 0 || prog[def_a[q]].op != OP_PARAME || def_b[q] < 0) return false;
+        t.push_back(Term{neg, prog[def_a[q]].a, def_b[q]});
+        return true;
+      case OP_ADDE: return linear(def_a[q], neg, t) && linear(def_b[q], neg, t);
+      case OP_SUBE: return linear(def_a[q], neg, t) && linear(def_b[q], !neg, t);
+      default: return false;
+    }
+  };
+  std::map<std::pair<u32, u32>, u32> slot_of;
+  std::map<int, u32> copy_of;   // base value (defining position) -> the register that keeps it for a later fold
+  for (int pc = 0; pc < n; ++pc) {
+    if (prog[pc].op != OP_CONSTRE) continue;
+    const int s = def_a[pc];
+    if (s < 0 || prog[s].op != OP_SUBE || uses[s] != 1) continue;
+    const int m = def_a[s], nu = def_b[s];
+    if (m < 0 || prog[m].op != OP_MULE || uses[m] != 1 || nu < 0 || prog[nu].op != OP_BTOE || def_a[nu] < 0) continue;
+    std::vector<Term> t;
+    u32 diff = prog[m].a;
+    if (!linear(def_b[m], false, t)) {
+      t.clear();
+      diff = prog[m].b;
+      if (!linear(def_a[m], false, t)) continue;
+    }
+    const u32 kc = coeff_of[pc];
+    // at the MULE: rr += diff * (coeff * den), coeff * den summed from the folded products and the base values the den read
+    std::ostringstream o;
+    Regs r;
+    r.re.push_back(diff);
+    o << "{ Q cd;";
+    for (size_t i = 0; i < t.size(); ++i) {
+      auto key = std::make_pair(kc, t[i].param);
+      auto it = slot_of.find(key);
+      if (it == slot_of.end()) { it = slot_of.emplace(key, (u32)pl.slots.size()).first; pl.slots.push_back(key); }
+      std::string v = "ldf(" + std::to_string(it->second) + ")";
+      if (t[i].bdef >= 0) {
+        const int d = t[i].bdef;
+        u32 reg = prog[d].dst;
+        if (next_def[d] < m) {   // the register is rewritten before the MULE: keep the value in a register of its own
+          auto ci = copy_of.find(d);
+          if (ci == copy_of.end()) {
+            ci = copy_of.emplace(d, pl.nb++).first;
+            Regs cr; cr.rb.push_back(reg); cr.wb = (int)ci->second;
+            pl.at[d].push_back(Stmt{"b[" + std::to_string(ci->second) + "] = b[" + std::to_string(reg) + "];", cr, false});
+          }
+          reg = ci->second;
+        }
+        v = "qmulb(" + v + ", b[" + std::to_string(reg) + "])";
+        r.rb.push_back(reg);
+      }
+      if (i == 0) o << " cd = " << (t[i].neg ? "qneg(" + v + ")" : v) << ";";
+      else o << " cd = " << (t[i].neg ? "qsub" : "qadd") << "(cd, " << v << ");";
+    }
+    o << " rr = qmacq(rr, e[" << diff << "], cd); }";
+    pl.at[m] = {Stmt{o.str(), r, true}};
+    // at the SUBE: rr -= coeff * num (a constant 0 or 1 needs no product)
+    const AirInstr& bv = prog[def_a[nu]];
+    pl.at[s].clear();
+    std::ostringstream q;
+    Regs qr;
+    const std::string cf = "ldq(coeff + " + std::to_string(JIT_COEFF_WORDS * kc) + ")";
+    if (bv.op == OP_CONSTB && bv.a == 1) q << "rr = qsub(rr, " << cf << ");";
+    else if (bv.op == OP_CONSTB) q << "rr = qsub(rr, qmulb(" << cf << ", " << bv.a << "u));";
+    else { q << "rr = qsub(rr, qmulb(" << cf << ", e[" << prog[s].b << "].c0));"; qr.re.push_back(prog[s].b); }
+    if (!(bv.op == OP_CONSTB && bv.a == 0)) pl.at[s].push_back(Stmt{q.str(), qr, true});
+    pl.at[pc].clear();
+  }
+  // dead code: a statement stays if it adds to rr or a later statement reads what it writes
+  std::vector<char> need_b(pl.nb + 1, 0), need_e(ne + 1, 0);
+  for (int pc = n; pc-- > 0;) {
+    for (size_t i = pl.at[pc].size(); i-- > 0;) {
+      Stmt& st = pl.at[pc][i];
+      if (!st.effect && !(st.r.wb >= 0 && need_b[st.r.wb]) && !(st.r.we >= 0 && need_e[st.r.we])) { st = Stmt(); continue; }
+      if (st.r.wb >= 0) need_b[st.r.wb] = 0;
+      if (st.r.we >= 0) need_e[st.r.we] = 0;
+      for (u32 x : st.r.rb) need_b[x] = 1;
+      for (u32 x : st.r.re) need_e[x] = 1;
+    }
+  }
+  return pl;
 }
 
 std::string gen_source(const AirComponent& c) {
@@ -201,21 +367,39 @@ std::string gen_source(const AirComponent& c) {
     << "  if (prev < half) { v = ((long long)prev + step) % (long long)half; if (v < 0) v += half; }\n"
     << "  else { v = ((long long)prev - step) % (long long)half; if (v < 0) v += half; v += half; }\n"
     << "  return __brev((u32)v) >> (32 - EL); }\n";
-  const u32 nb = c.n_base_regs ? c.n_base_regs : 1, ne = c.n_ext_regs ? c.n_ext_regs : 1;
-  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; Q rr; };\n";
-  // column base pointers live in constant memory (filled before every launch): an access costs no pointer load from global memory
-  // (the real AIR reads 2765 mask values per row: one dependent global load less per value)
-  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
+  const u32 ne = c.n_ext_regs ? c.n_ext_regs : 1;
   auto ld = [&](u32 m) {
     std::ostringstream s;
     if (c.masks[m].off == 0) s << "__ldg(ccols[" << m << "] + row)";
     else s << "__ldg(ccols[" << m << "] + offrow(row, " << c.masks[m].off << ", EL))";
     return s.str();
   };
+  const ConstraintPlan pl = plan_constraints(c, ld, c.n_base_regs ? c.n_base_regs : 1, ne);
+  const u32 nb = pl.nb;
+  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; Q rr; };\n";
+  // column base pointers live in constant memory (filled before every launch): an access costs no pointer load from global memory
+  // (the real AIR reads 2765 mask values per row: one dependent global load less per value)
+  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
+  if (!pl.slots.empty()) {
+    // the folded products coeff_k * params[p]: (k, p) per slot, and their values, computed by each CTA before the first chunk
+    o << "#ifndef __CUDACC__\n#define __shared__\n#endif\n#define NB_NFOLD " << pl.slots.size() << "\n__constant__ const uint2 nbfold_src[NB_NFOLD] = {";
+    for (size_t i = 0; i < pl.slots.size(); ++i) o << (i ? ", " : "") << "{" << pl.slots[i].first << "u, " << pl.slots[i].second << "u}";
+    o << "};\n__shared__ uint4 nbfold[NB_NFOLD];\n"
+      << "__device__ __forceinline__ Q ldf(u32 i) { const uint4 v = nbfold[i]; return Q{v.x, v.y, v.z, v.w}; }\n"
+      << "__device__ __forceinline__ Q qmacq(Q acc, Q x, Q y) {\n"
+      << "  u32 gp = add(add(y.c3, y.c3), y.c2), g = sub(add(y.c2, y.c2), y.c3);\n"
+      << "  return qmac(acc, x, y.c0, y.c1, y.c2, y.c3, P31 - y.c1, P31 - y.c3, g, gp, P31 - gp);\n}\n";
+  }
   const size_t CH = 250;
-  size_t n_chunks = (c.prog.size() + CH - 1) / CH;
-  const ChunkLive live = chunk_liveness(c.prog, CH, nb, ne);
-  u32 k = 0;
+  const size_t n_chunks = (c.prog.size() + CH - 1) / CH;
+  std::vector<Regs> regs;
+  std::vector<size_t> begin;
+  for (size_t pc = 0; pc < c.prog.size(); ++pc) {
+    if (pc % CH == 0) begin.push_back(regs.size());
+    for (const Stmt& st : pl.at[pc]) regs.push_back(st.r);
+  }
+  begin.push_back(regs.size());
+  const ChunkLive live = chunk_liveness(regs, begin, nb, ne);
   for (size_t ci = 0; ci < n_chunks; ++ci) {
     o << "__device__ __noinline__ void chunk" << ci << "(St& s, const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff, u32 row, u32 EL) {\n";
     o << "  u32 b[" << nb << "]; Q e[" << ne << "]; Q rr = s.rr;\n";
@@ -223,13 +407,8 @@ std::string gen_source(const AirComponent& c) {
     for (u32 r : live.in_e[ci]) o << "  e[" << r << "] = s.e[" << r << "];";
     o << "\n";
     for (size_t pc = ci * CH; pc < std::min(c.prog.size(), (ci + 1) * CH); ++pc) {
-      const AirInstr& in = c.prog[pc];
       o << "  ";
-      switch (in.op) {
-        case OP_CONSTRB: o << "rr = qadd(rr, qmulb(ldq(coeff + " << JIT_COEFF_WORDS * k << "), b[" << in.a << "]));"; ++k; break;
-        case OP_CONSTRE: o << "rr = qmac_tab(rr, e[" << in.a << "], coeff + " << JIT_COEFF_WORDS * k << ");"; ++k; break;
-        default: emit_op(o, in, ld); break;
-      }
+      for (size_t i = 0; i < pl.at[pc].size(); ++i) o << (i ? " " : "") << pl.at[pc][i].code;
       o << "\n";
     }
     for (u32 r : live.out_b[ci]) o << "  s.b[" << r << "] = b[" << r << "];";
@@ -243,6 +422,10 @@ std::string gen_source(const AirComponent& c) {
     << "    const u32* __restrict__ dinv, u32* __restrict__ a0, u32* __restrict__ a1, u32* __restrict__ a2, u32* __restrict__ a3, u32 EL, u32 row0) {\n"
     << "  const u32 row = row0 + blockIdx.x * blockDim.x + threadIdx.x;   // row0: a rank of a multi-GPU proof evaluates its slice of the domain's rows\n  St s;\n"
     << "  for (int i = 0; i < " << nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n  s.rr = Q{0u, 0u, 0u, 0u};\n";
+  if (!pl.slots.empty())
+    o << "  for (u32 i = threadIdx.x; i < NB_NFOLD; i += blockDim.x) {\n"
+      << "    const Q f = qmac_tab(Q{0u, 0u, 0u, 0u}, ldq(params + 4 * nbfold_src[i].y), coeff + " << JIT_COEFF_WORDS << " * nbfold_src[i].x);\n"
+      << "    nbfold[i] = uint4{f.c0, f.c1, f.c2, f.c3};\n  }\n  __syncthreads();\n";
   for (size_t ci = 0; ci < n_chunks; ++ci) o << "  chunk" << ci << "(s, cols, params, coeff, row, EL);\n  __syncthreads();\n";
   o << "  const u32 di = __ldg(dinv + (row >> " << DL << "));\n"
     << "  a0[row] = add(a0[row], mul(s.rr.c0, di)); a1[row] = add(a1[row], mul(s.rr.c1, di));\n"
@@ -268,7 +451,7 @@ std::string gen_logup_source(const AirComponent& c) {
   };
   size_t CH = 150;
   size_t n_chunks = (c.logup_prog.size() + CH - 1) / CH;
-  const ChunkLive live = chunk_liveness(c.logup_prog, CH, nb, ne);
+  const ChunkLive live = prog_liveness(c.logup_prog, CH, nb, ne);
   // The QM31 inverse (one per batch of fractions; 38 M31 products for x^(P-2) alone) is batched over G consecutive batches of the same
   // row: prefix products, ONE inverse, back-substitution (3 products per extra batch).  The inverse is unique, so the values are the
   // interpreter's.  `pending` batches wait in pfn/pfd until the group is full; the running row sum is then advanced batch by batch.
