@@ -191,10 +191,15 @@ void nb200_air_free(nb200_air*);
 uint32_t nb200_air_n_params(const nb200_air*);
 uint32_t nb200_air_n_components(const nb200_air*);
 /* the CUDA C source a component's programs are specialised to at first use (NVRTC, sm_90a): which = 0 the constraint
- * program, 1 the logup (interaction trace) program.  malloc'ed, NUL-terminated, free with nb200_free.  Works without a
+ * program, 1 the logup (interaction trace) program, 2 the constraints of degree above 2 alone (evaluated on the extra half
+ * coset of a component with log_expand = log_blowup + 1).  malloc'ed, NUL-terminated, free with nb200_free.  Works without a
  * device (ctx may have been NULL at nb200_air_load).  NB200_ERR_STATE (and *out = NULL): the program is too short to be
- * specialised and runs on the bytecode interpreter. */
+ * specialised and runs on the bytecode interpreter, or (which = 2) the component has no constraint of degree above 2. */
 nb200_status nb200_air_kernel_source(const nb200_air*, uint32_t component, int which, char** out);
+/* degree of each of the component's n constraints in the trace columns (masks 1, constants and parameters 0, products add,
+ * sums take the maximum), and which of its n masks the constraints of degree above 2 read (flags[m] = 1) */
+nb200_status nb200_air_constraint_degrees(const nb200_air*, uint32_t component, uint32_t* degrees, size_t n);
+nb200_status nb200_air_d2_masks(const nb200_air*, uint32_t component, uint8_t* flags, size_t n);
 /* file name (16 hex digits + ".cubin") under which that kernel is looked up in the cubin cache: <library dir>/jit_cache or
  * $NB200_JIT_CACHE.  `python -m nexus_zkvm_b200.build` pre-compiles the shipped machines' kernels there with nvcc. */
 uint64_t nb200_kernel_source_key(const char* source);
@@ -207,8 +212,9 @@ nb200_status nb200_scheme_new(nb200_ctx*, uint32_t pow_bits, uint32_t log_blowup
 void nb200_scheme_free(nb200_scheme*);
 /* Optional hint: log2 of the AIR's constraint degree bound relative to the trace (the reference's LOG_CONSTRAINT_DEGREE,
  * prover/src/components/mod.rs:12; = max log_expand of the loaded AIR, nb200_air_max_log_expand).  When it equals
- * log_blowup + 1, commits from HOST columns also evaluate the polynomials on the extra half-size coset the quotient step
- * needs, in the shadow of the PCIe copy.  Results never depend on the hint. */
+ * log_blowup + 1, the sharded commit (nb200_scheme_commit_sharded) also evaluates the polynomials on the extra half-size coset
+ * the quotient step needs.  Single-GPU commits ignore it: there the quotient step extends only the few columns its
+ * constraints of degree above 2 read.  Results never depend on the hint. */
 nb200_status nb200_scheme_set_constraint_log_degree(nb200_scheme*, uint32_t log_expand);
 uint32_t nb200_air_max_log_expand(const nb200_air*);
 /* tree_builder.extend_evals(batches...); tree_builder.commit(channel)  (machine.rs:208-263): interpolate, LDE,

@@ -99,7 +99,7 @@ def kernel_sources(words):
         raise RuntimeError("nb200_air_load failed")
     out = []
     for comp in range(L.nb200_air_n_components(air)):
-        for which in (0, 1):
+        for which in (0, 1, 2):   # constraints, LogUp program, constraints of degree > 2 (the half coset D2)
             p = C.c_void_p()
             if L.nb200_air_kernel_source(air, C.c_uint32(comp), C.c_int(which), C.byref(p)) != 0 or not p:
                 continue

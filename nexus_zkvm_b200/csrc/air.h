@@ -100,4 +100,69 @@ inline AirProgram air_parse(const u32* w, size_t n) {
   return a;
 }
 
+// Degree of each constraint (declaration order) in the trace polynomials, walked over the constraint program: a mask has degree 1,
+// a constant or a parameter 0, a product the sum of its operands' degrees and a sum or difference their maximum.
+inline std::vector<u32> constraint_degrees(const AirComponent& c) {
+  std::vector<u32> db(c.n_base_regs + 1, 0), de(c.n_ext_regs + 1, 0), out;
+  auto mx = [](u32 x, u32 y) { return x > y ? x : y; };
+  for (const AirInstr& in : c.prog) {
+    switch (in.op) {
+      case OP_LOADM: db[in.dst] = 1; break;
+      case OP_CONSTB: db[in.dst] = 0; break;
+      case OP_ADDB: case OP_SUBB: db[in.dst] = mx(db[in.a], db[in.b]); break;
+      case OP_MULB: db[in.dst] = db[in.a] + db[in.b]; break;
+      case OP_NEGB: db[in.dst] = db[in.a]; break;
+      case OP_PARAME: de[in.dst] = 0; break;
+      case OP_LOADME: de[in.dst] = 1; break;
+      case OP_ADDE: case OP_SUBE: de[in.dst] = mx(de[in.a], de[in.b]); break;
+      case OP_MULE: de[in.dst] = de[in.a] + de[in.b]; break;
+      case OP_NEGE: de[in.dst] = de[in.a]; break;
+      case OP_ADDEB: case OP_SUBEB: de[in.dst] = mx(de[in.a], db[in.b]); break;
+      case OP_MULEB: de[in.dst] = de[in.a] + db[in.b]; break;
+      case OP_BTOE: de[in.dst] = db[in.a]; break;
+      case OP_CONSTRB: out.push_back(db[in.a]); break;
+      case OP_CONSTRE: out.push_back(de[in.a]); break;
+      default: break;
+    }
+  }
+  return out;
+}
+
+// A constraint of degree d has a quotient C / Z of circle degree (d - 1) 2^log_size: for d <= 2 it lies in the span of the first
+// 2^(log_size + 2) circle-FFT basis vectors, the part of the composition a Q_HALF component interpolates from the committed LDE domain
+// alone (prove.cu, component_quotients).  Only the constraints above that bound contribute to the upper half.
+static const u32 AIR_LOW_DEGREE = 2;
+inline std::vector<char> high_constraints(const AirComponent& c) {
+  std::vector<char> h;
+  for (u32 d : constraint_degrees(c)) h.push_back(d > AIR_LOW_DEGREE ? 1 : 0);
+  return h;
+}
+inline size_t count_high(const std::vector<char>& high) { size_t n = 0; for (char x : high) n += x ? 1 : 0; return n; }
+
+// The masks the constraints flagged in `keep` read (directly or through shared subexpressions, at any row offset): a backward walk over
+// the program from those constraints' sinks.
+inline std::vector<char> masks_read_by(const AirComponent& c, const std::vector<char>& keep) {
+  std::vector<char> nb(c.n_base_regs + 1, 0), ne(c.n_ext_regs + 1, 0), used(c.masks.size(), 0);
+  u32 k = c.n_constraints;
+  for (size_t pc = c.prog.size(); pc-- > 0;) {
+    const AirInstr& in = c.prog[pc];
+    switch (in.op) {
+      case OP_CONSTRB: if (keep[--k]) nb[in.a] = 1; break;
+      case OP_CONSTRE: if (keep[--k]) ne[in.a] = 1; break;
+      case OP_LOADM: if (nb[in.dst]) used[in.a] = 1; nb[in.dst] = 0; break;
+      case OP_CONSTB: nb[in.dst] = 0; break;
+      case OP_ADDB: case OP_SUBB: case OP_MULB: if (nb[in.dst]) { nb[in.dst] = 0; nb[in.a] = nb[in.b] = 1; } break;
+      case OP_NEGB: if (nb[in.dst]) { nb[in.dst] = 0; nb[in.a] = 1; } break;
+      case OP_PARAME: ne[in.dst] = 0; break;
+      case OP_LOADME: if (ne[in.dst]) for (u32 i = 0; i < 4; ++i) used[in.a + i] = 1; ne[in.dst] = 0; break;
+      case OP_ADDE: case OP_SUBE: case OP_MULE: if (ne[in.dst]) { ne[in.dst] = 0; ne[in.a] = ne[in.b] = 1; } break;
+      case OP_NEGE: if (ne[in.dst]) { ne[in.dst] = 0; ne[in.a] = 1; } break;
+      case OP_ADDEB: case OP_SUBEB: case OP_MULEB: if (ne[in.dst]) { ne[in.dst] = 0; ne[in.a] = 1; nb[in.b] = 1; } break;
+      case OP_BTOE: if (ne[in.dst]) { ne[in.dst] = 0; nb[in.a] = 1; } break;
+      default: break;
+    }
+  }
+  return used;
+}
+
 }  // namespace nb

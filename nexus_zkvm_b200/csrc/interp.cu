@@ -290,7 +290,8 @@ static nb200_status launch_interp(nb200_ctx* ctx, InterpArgs& a, u32 domain_log)
 // Evaluate the component's constraints on its evaluation domain and accumulate  sum_k coeff_k * c_k / vanishing  into acc.
 // mask_cols[m]: device pointer of mask m's column evaluated on CanonicCoset(eval_log).circle_domain().
 nb200_status constraint_eval(nb200_ctx* ctx, const AirComponent& c, const std::vector<const u32*>& mask_cols, const u32* d_params,
-                             const std::vector<qm31>& coeffs, u32* const acc[4], const JitKernel* jk, u32 rows_log, u32 dom_log, u32 row0, size_t n_rows) {
+                             const std::vector<qm31>& coeffs, u32* const acc[4], const JitKernel* jk, u32 rows_log, u32 dom_log, u32 row0, size_t n_rows,
+                             u32* const acc_high[4]) {
   NB_ARG(ctx, mask_cols.size() == c.masks.size() && coeffs.size() == c.n_constraints, "constraint_eval: shape");
   // rows [0, 2^rows_log) of CanonicCoset(dom_log).circle_domain() in bit-reversed order: the whole domain or its first half
   if (rows_log == 0 && dom_log == 0) rows_log = dom_log = c.eval_log();
@@ -321,8 +322,10 @@ nb200_status constraint_eval(nb200_ctx* ctx, const AirComponent& c, const std::v
   NB_CUDA(ctx, dmalloc(ctx, (void**)&d_dinv, dinv.size() * 4));
   NB_CUDA(ctx, cudaMemcpyAsync(d_dinv, dinv.data(), dinv.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
   nb200_status st;
-  if (row0 != 0 || n_rows != 0) NB_ARG(ctx, jk && jk->kernel && jk->log_size == c.log_size, "constraint_eval: a row range needs the specialised kernel");
-  if (jk && jk->kernel && jk->log_size == c.log_size && ((size_t)1 << rows_log) >= JIT_BLOCK) {
+  const bool use_jit = jit_usable(jk, c, rows_log);
+  if (row0 != 0 || n_rows != 0) NB_ARG(ctx, use_jit, "constraint_eval: a row range needs the specialised kernel");
+  NB_ARG(ctx, !acc_high || use_jit, "constraint_eval: the high-degree accumulators need the specialised kernel");
+  if (use_jit) {
     // NVRTC-specialised kernel (jit.cu): same arithmetic, registers instead of the shared-memory register file
     const u32** d_cols = nullptr;
     NB_CUDA(ctx, dmalloc(ctx, (void**)&d_cols, mask_cols.size() * sizeof(u32*)));
@@ -332,7 +335,7 @@ nb200_status constraint_eval(nb200_ctx* ctx, const AirComponent& c, const std::v
     u32* d_tab = nullptr;
     NB_CUDA(ctx, dmalloc(ctx, (void**)&d_tab, tab.size() * 4 + 16));
     NB_CUDA(ctx, cudaMemcpyAsync(d_tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-    st = jit_launch_constraints(ctx, *jk, d_cols, d_params, d_tab, d_dinv, acc, rows_log, dom_log, row0, n_rows);
+    st = jit_launch_constraints(ctx, *jk, d_cols, d_params, d_tab, d_dinv, acc, rows_log, dom_log, row0, n_rows, acc_high);
     cudaStreamSynchronize(ctx->stream);
     dfree(ctx, (void*)d_cols); dfree(ctx, d_tab);
   } else {

@@ -224,15 +224,16 @@ static ChunkLive prog_liveness(const std::vector<AirInstr>& prog, size_t CH, u32
 // The den's own terms and partial sums may be shared with other constraints (air.py merges equal nodes), so they are not scaled in
 // place: coeff * den is summed afresh at the MULE from the base values the den read, and a base value whose register is rewritten
 // before that point is first copied to a register of its own.  Whatever only the folded dens read is then dropped as dead code.
-struct Stmt { std::string code; Regs r; bool effect = false; };   // effect: adds to rr (never removed as dead)
+struct Stmt { std::string code; Regs r; bool effect = false; int constr = -1; };   // effect: adds constraint `constr` to rr (never removed as dead)
 struct ConstraintPlan {
   std::vector<std::vector<Stmt>> at;               // the statements emitted at each program position
   u32 nb = 0;                                      // base registers, the copies of folded base values included
   std::vector<std::pair<u32, u32>> slots;          // nbfold[i] = coeff[slots[i].first] * params[slots[i].second]
 };
 
+// `keep[k] == 0`: constraint k is left out (with everything only it reads)
 template <class Ld>
-static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32 ne) {
+static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32 ne, const std::vector<char>& keep) {
   const std::vector<AirInstr>& prog = c.prog;
   const int n = (int)prog.size();
   // def_a / def_b[pc]: position of the instruction whose result operand a / b of prog[pc] reads (-1: none);
@@ -261,13 +262,14 @@ static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32
   for (int pc = 0; pc < n; ++pc) {
     const AirInstr& in = prog[pc];
     std::ostringstream o;
-    bool effect = false;
+    int constr = -1;
     switch (in.op) {
-      case OP_CONSTRB: o << "rr = qadd(rr, qmulb(ldq(coeff + " << JIT_COEFF_WORDS * k << "), b[" << in.a << "]));"; coeff_of[pc] = k++; effect = true; break;
-      case OP_CONSTRE: o << "rr = qmac_tab(rr, e[" << in.a << "], coeff + " << JIT_COEFF_WORDS * k << ");"; coeff_of[pc] = k++; effect = true; break;
+      case OP_CONSTRB: o << "rr = qadd(rr, qmulb(ldq(coeff + " << JIT_COEFF_WORDS * k << "), b[" << in.a << "]));"; coeff_of[pc] = k; constr = (int)k++; break;
+      case OP_CONSTRE: o << "rr = qmac_tab(rr, e[" << in.a << "], coeff + " << JIT_COEFF_WORDS * k << ");"; coeff_of[pc] = k; constr = (int)k++; break;
       default: emit_op(o, in, ld); break;
     }
-    pl.at[pc].push_back(Stmt{o.str(), instr_regs(in), effect});
+    if (constr >= 0 && !keep[constr]) continue;
+    pl.at[pc].push_back(Stmt{o.str(), instr_regs(in), constr >= 0, constr});
   }
 
   struct Term { bool neg; u32 param; int bdef; };   // -/+ params[param] * (bdef < 0 ? 1 : the base value prog[bdef] wrote)
@@ -287,7 +289,7 @@ static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32
   std::map<std::pair<u32, u32>, u32> slot_of;
   std::map<int, u32> copy_of;   // base value (defining position) -> the register that keeps it for a later fold
   for (int pc = 0; pc < n; ++pc) {
-    if (prog[pc].op != OP_CONSTRE) continue;
+    if (prog[pc].op != OP_CONSTRE || !keep[coeff_of[pc]]) continue;
     const int s = def_a[pc];
     if (s < 0 || prog[s].op != OP_SUBE || uses[s] != 1) continue;
     const int m = def_a[s], nu = def_b[s];
@@ -329,7 +331,7 @@ static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32
       else o << " cd = " << (t[i].neg ? "qsub" : "qadd") << "(cd, " << v << ");";
     }
     o << " rr = qmacq(rr, e[" << diff << "], cd); }";
-    pl.at[m] = {Stmt{o.str(), r, true}};
+    pl.at[m] = {Stmt{o.str(), r, true, (int)kc}};
     // at the SUBE: rr -= coeff * num (a constant 0 or 1 needs no product)
     const AirInstr& bv = prog[def_a[nu]];
     pl.at[s].clear();
@@ -339,7 +341,7 @@ static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32
     if (bv.op == OP_CONSTB && bv.a == 1) q << "rr = qsub(rr, " << cf << ");";
     else if (bv.op == OP_CONSTB) q << "rr = qsub(rr, qmulb(" << cf << ", " << bv.a << "u));";
     else { q << "rr = qsub(rr, qmulb(" << cf << ", e[" << prog[s].b << "].c0));"; qr.re.push_back(prog[s].b); }
-    if (!(bv.op == OP_CONSTB && bv.a == 0)) pl.at[s].push_back(Stmt{q.str(), qr, true});
+    if (!(bv.op == OP_CONSTB && bv.a == 0)) pl.at[s].push_back(Stmt{q.str(), qr, true, (int)kc});
     pl.at[pc].clear();
   }
   // dead code: a statement stays if it adds to rr or a later statement reads what it writes
@@ -357,8 +359,13 @@ static ConstraintPlan plan_constraints(const AirComponent& c, Ld ld, u32 nb, u32
   return pl;
 }
 
-std::string gen_source(const AirComponent& c) {
+// d2 = false: every constraint, summed into a0..a3; when h0..h3 are given, the constraints of degree above AIR_LOW_DEGREE are also
+//             summed on their own into h0..h3 (for the committed LDE domain D1 of a Q_HALF component: prove.cu, component_quotients).
+// d2 = true:  the constraints of degree above AIR_LOW_DEGREE only, into a0..a3 (for the half coset D2); the masks no such constraint
+//             reads are never loaded and may be null.
+std::string gen_source(const AirComponent& c, bool d2) {
   std::ostringstream o;
+  if (d2) o << "// constraint quotients on D2: the constraints of degree > " << AIR_LOW_DEGREE << " only\n";
   o << kPrelude;
   const u32 DL = c.log_size;  // EL (the canonic domain the rows belong to) is a kernel argument: whole domains and half domains share the kernel
   // offset_bit_reversed_circle_domain_index with the domain sizes baked in
@@ -374,9 +381,16 @@ std::string gen_source(const AirComponent& c) {
     else s << "__ldg(ccols[" << m << "] + offrow(row, " << c.masks[m].off << ", EL))";
     return s.str();
   };
-  const ConstraintPlan pl = plan_constraints(c, ld, c.n_base_regs ? c.n_base_regs : 1, ne);
+  const std::vector<char> high = high_constraints(c);
+  ConstraintPlan pl = plan_constraints(c, ld, c.n_base_regs ? c.n_base_regs : 1, ne, d2 ? high : std::vector<char>(c.n_constraints, 1));
   const u32 nb = pl.nb;
-  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; Q rr; };\n";
+  // rh: the high constraints' part of rr, taken as the change of rr across their statements (no products of its own)
+  const bool track_high = !d2 && count_high(high) > 0;
+  if (track_high)
+    for (auto& at : pl.at)
+      for (Stmt& st : at)
+        if (st.effect && high[st.constr]) st.code = "{ const Q r0 = rr; " + st.code + " rh = qadd(rh, qsub(rr, r0)); }";
+  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; Q rr;" << (track_high ? " Q rh;" : "") << " };\n";
   // column base pointers live in constant memory (filled before every launch): an access costs no pointer load from global memory
   // (the real AIR reads 2765 mask values per row: one dependent global load less per value)
   o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
@@ -400,9 +414,13 @@ std::string gen_source(const AirComponent& c) {
   }
   begin.push_back(regs.size());
   const ChunkLive live = chunk_liveness(regs, begin, nb, ne);
+  std::vector<char> has_code(n_chunks, 0);   // the D2 kernel leaves out most statements: chunks left empty are not emitted
+  for (size_t pc = 0; pc < c.prog.size(); ++pc)
+    for (const Stmt& st : pl.at[pc]) if (!st.code.empty()) has_code[pc / CH] = 1;
   for (size_t ci = 0; ci < n_chunks; ++ci) {
+    if (!has_code[ci]) continue;
     o << "__device__ __noinline__ void chunk" << ci << "(St& s, const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff, u32 row, u32 EL) {\n";
-    o << "  u32 b[" << nb << "]; Q e[" << ne << "]; Q rr = s.rr;\n";
+    o << "  u32 b[" << nb << "]; Q e[" << ne << "]; Q rr = s.rr;" << (track_high ? " Q rh = s.rh;" : "") << "\n";
     for (u32 r : live.in_b[ci]) o << "  b[" << r << "] = s.b[" << r << "];";
     for (u32 r : live.in_e[ci]) o << "  e[" << r << "] = s.e[" << r << "];";
     o << "\n";
@@ -413,23 +431,31 @@ std::string gen_source(const AirComponent& c) {
     }
     for (u32 r : live.out_b[ci]) o << "  s.b[" << r << "] = b[" << r << "];";
     for (u32 r : live.out_e[ci]) o << "  s.e[" << r << "] = e[" << r << "];";
-    o << "\n  s.rr = rr;\n}\n";
+    o << "\n  s.rr = rr;" << (track_high ? " s.rh = rh;" : "") << "\n}\n";
   }
   // The CTAs re-converge (__syncthreads) after every chunk: the warps of a CTA then execute the same few tens of KB of straight-line
   // code at a time and the instruction cache serves them from one fetch.  Without the barriers the warps drift apart over the ~0.7 MB
   // program and the kernel becomes instruction-fetch bound.
   o << "extern \"C\" __global__ void __launch_bounds__(" << JIT_BLOCK << ", 1) nbjit(const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff,\n"
-    << "    const u32* __restrict__ dinv, u32* __restrict__ a0, u32* __restrict__ a1, u32* __restrict__ a2, u32* __restrict__ a3, u32 EL, u32 row0) {\n"
+    << "    const u32* __restrict__ dinv, u32* __restrict__ a0, u32* __restrict__ a1, u32* __restrict__ a2, u32* __restrict__ a3, u32 EL, u32 row0,\n"
+    << "    u32* __restrict__ h0 = nullptr, u32* __restrict__ h1 = nullptr, u32* __restrict__ h2 = nullptr, u32* __restrict__ h3 = nullptr) {\n"
     << "  const u32 row = row0 + blockIdx.x * blockDim.x + threadIdx.x;   // row0: a rank of a multi-GPU proof evaluates its slice of the domain's rows\n  St s;\n"
     << "  for (int i = 0; i < " << nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n  s.rr = Q{0u, 0u, 0u, 0u};\n";
+  if (track_high) o << "  s.rh = Q{0u, 0u, 0u, 0u};\n";
   if (!pl.slots.empty())
     o << "  for (u32 i = threadIdx.x; i < NB_NFOLD; i += blockDim.x) {\n"
       << "    const Q f = qmac_tab(Q{0u, 0u, 0u, 0u}, ldq(params + 4 * nbfold_src[i].y), coeff + " << JIT_COEFF_WORDS << " * nbfold_src[i].x);\n"
       << "    nbfold[i] = uint4{f.c0, f.c1, f.c2, f.c3};\n  }\n  __syncthreads();\n";
-  for (size_t ci = 0; ci < n_chunks; ++ci) o << "  chunk" << ci << "(s, cols, params, coeff, row, EL);\n  __syncthreads();\n";
+  for (size_t ci = 0; ci < n_chunks; ++ci)
+    if (has_code[ci]) o << "  chunk" << ci << "(s, cols, params, coeff, row, EL);\n  __syncthreads();\n";
   o << "  const u32 di = __ldg(dinv + (row >> " << DL << "));\n"
     << "  a0[row] = add(a0[row], mul(s.rr.c0, di)); a1[row] = add(a1[row], mul(s.rr.c1, di));\n"
-    << "  a2[row] = add(a2[row], mul(s.rr.c2, di)); a3[row] = add(a3[row], mul(s.rr.c3, di));\n}\n";
+    << "  a2[row] = add(a2[row], mul(s.rr.c2, di)); a3[row] = add(a3[row], mul(s.rr.c3, di));\n";
+  if (track_high)
+    o << "  if (h0) {\n"
+      << "    h0[row] = add(h0[row], mul(s.rh.c0, di)); h1[row] = add(h1[row], mul(s.rh.c1, di));\n"
+      << "    h2[row] = add(h2[row], mul(s.rh.c2, di)); h3[row] = add(h3[row], mul(s.rh.c3, di));\n  }\n";
+  o << "}\n";
   return o.str();
 }
 
@@ -517,7 +543,7 @@ std::string gen_logup_source(const AirComponent& c) {
 }
 }  // namespace
 
-std::string jit_source(const AirComponent& c) { return gen_source(c); }
+std::string jit_source(const AirComponent& c, bool d2) { return gen_source(c, d2); }
 std::string jit_logup_source(const AirComponent& c) { return gen_logup_source(c); }
 
 bool jit_enabled() {
@@ -531,11 +557,12 @@ void jit_release(JitKernel& jk) {
 }
 
 static nb200_status jit_compile_source(nb200_ctx* ctx, const AirComponent& c, const std::string& src, JitKernel* out);
-nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_source(c), out); }
+nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, bool d2, JitKernel* out) { return jit_compile_source(ctx, c, gen_source(c, d2), out); }
 nb200_status jit_compile_logup(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_logup_source(c), out); }
 // ---- cubin cache: <directory of this library>/jit_cache/<key>.cubin (or $NB200_JIT_CACHE).  `python -m nexus_zkvm_b200.build`
 // fills it for the shipped machines with nvcc, so a fresh box neither loads libnvrtc nor compiles; kernels compiled at run time are
-// added when the directory is writable.  The key covers the generated source and the target.
+// added when the directory is writable.  The key covers the generated source and the target; the D2 variant of a constraint kernel
+// starts with a line of its own, so it never shares a key with the D1 variant.
 uint64_t jit_source_key(const std::string& src) {
   uint64_t h = 1469598103934665603ull;
   auto mix = [&](const char* p, size_t n) { for (size_t i = 0; i < n; ++i) { h ^= (unsigned char)p[i]; h *= 1099511628211ull; } };
@@ -651,13 +678,16 @@ nb200_status jit_launch_logup(nb200_ctx* ctx, const JitKernel& jk, const u32* co
 }
 
 nb200_status jit_launch_constraints(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, const u32* d_coeff, const u32* d_dinv, u32* const acc[4],
-                                    u32 rows_log, u32 dom_log, u32 row0, size_t n_rows) {
+                                    u32 rows_log, u32 dom_log, u32 row0, size_t n_rows, u32* const acc_high[4]) {
   size_t rows = n_rows ? n_rows : (size_t)1 << rows_log;
   if (rows < JIT_BLOCK || rows % JIT_BLOCK != 0) return set_err(ctx, NB200_ERR_STATE, "jit: row range too small");
   NB_TRY(jit_set_cols(ctx, jk, d_cols));
   u32 el = dom_log;
   u32* a0 = acc[0]; u32* a1 = acc[1]; u32* a2 = acc[2]; u32* a3 = acc[3];
-  void* args[] = {(void*)&d_cols, (void*)&d_params, (void*)&d_coeff, (void*)&d_dinv, (void*)&a0, (void*)&a1, (void*)&a2, (void*)&a3, (void*)&el, (void*)&row0};
+  u32* h[4] = {nullptr, nullptr, nullptr, nullptr};
+  if (acc_high) for (int k = 0; k < 4; ++k) h[k] = acc_high[k];
+  void* args[] = {(void*)&d_cols, (void*)&d_params, (void*)&d_coeff, (void*)&d_dinv, (void*)&a0, (void*)&a1, (void*)&a2, (void*)&a3, (void*)&el, (void*)&row0,
+                  (void*)&h[0], (void*)&h[1], (void*)&h[2], (void*)&h[3]};
   cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args, 0, ctx->stream);
   ctx->launches += 1;
   if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));

@@ -21,15 +21,22 @@ struct JitKernel {
   bool tried = false;      // compilation attempted (failed attempts fall back to the interpreter)
 };
 
+// the specialised kernel jk runs constraint_eval on 2^rows_log rows (else the bytecode interpreter does)
+inline bool jit_usable(const JitKernel* jk, const AirComponent& c, u32 rows_log) {
+  return jk && jk->kernel && jk->log_size == c.log_size && ((size_t)1 << rows_log) >= JIT_BLOCK;
+}
 bool jit_enabled();
 uint64_t jit_source_key(const std::string& src);   // name of the kernel's file in the cubin cache
-std::string jit_source(const AirComponent& c);  // the CUDA C the component is specialised to (inspection / offline ptxas checks)
-nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, JitKernel* out);
+// the CUDA C the component's constraints are specialised to (inspection / offline ptxas checks): d2 = false every constraint (with the
+// high-degree part on the side, jit.cu gen_source), d2 = true the constraints of degree above AIR_LOW_DEGREE only
+std::string jit_source(const AirComponent& c, bool d2 = false);
+nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, bool d2, JitKernel* out);
 nb200_status jit_compile_logup(nb200_ctx* ctx, const AirComponent& c, JitKernel* out);
 nb200_status jit_launch_logup(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, u32* d_out, u32 log_size);
 std::string jit_logup_source(const AirComponent& c);
 nb200_status jit_launch_constraints(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, const u32* d_coeff,
-                                    const u32* d_dinv, u32* const acc[4], u32 rows_log, u32 dom_log, u32 row0 = 0, size_t n_rows = 0);
+                                    const u32* d_dinv, u32* const acc[4], u32 rows_log, u32 dom_log, u32 row0 = 0, size_t n_rows = 0,
+                                    u32* const acc_high[4] = nullptr);
 void jit_release(JitKernel& jk);
 void jit_coeff_table(const std::vector<qm31>& coeffs, std::vector<u32>& out);
 

@@ -28,7 +28,8 @@ nb200_status grind(nb200_ctx* ctx, const uint8_t digest[32], u32 pow_bits, uint6
 // the domain; 0, 0 = the component's whole evaluation domain.  mask_cols are the columns evaluated on exactly those rows.
 nb200_status constraint_eval(nb200_ctx* ctx, const AirComponent& c, const std::vector<const u32*>& mask_cols, const u32* d_params,
                              const std::vector<qm31>& coeffs, u32* const acc[4], const JitKernel* jk = nullptr, u32 rows_log = 0, u32 dom_log = 0,
-                             u32 row0 = 0, size_t n_rows = 0);   // row0 / n_rows: only the rows [row0, row0 + n_rows) (pointers stay indexed by the global row)
+                             u32 row0 = 0, size_t n_rows = 0,    // row0 / n_rows: only the rows [row0, row0 + n_rows) (pointers stay indexed by the global row)
+                             u32* const acc_high[4] = nullptr);  // also: the constraints of degree above AIR_LOW_DEGREE alone (needs jit_usable)
 nb200_status sub_scale_top_twiddle(nb200_ctx* ctx, u32* a, const u32* b, size_t n, u32 tw_log);  // a = (a - b) / (top-layer twiddle of canonic(tw_log))
 nb200_status add_cols_strided(nb200_ctx* ctx, u32* dst, size_t dst_stride, const u32* src, size_t src_stride, size_t len, size_t n_cols);
 nb200_status logup_generate(nb200_ctx* ctx, const AirComponent& c, const std::vector<const u32*>& mask_cols, const u32* d_params,

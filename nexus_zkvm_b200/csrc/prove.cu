@@ -18,9 +18,10 @@ struct nb200_channel { nb::HostChannel ch; };
 struct nb200_air {
   nb::AirProgram prog;
   // per component, compiled on first use (NVRTC); empty kernel = bytecode interpreter
-  std::vector<nb::JitKernel> jit;        // constraint program
+  std::vector<nb::JitKernel> jit;        // constraint program (D1 and whole domains)
+  std::vector<nb::JitKernel> jit_d2;     // its constraints of degree above AIR_LOW_DEGREE (D2 of the half-domain route)
   std::vector<nb::JitKernel> jit_logup;  // logup (interaction trace) program
-  ~nb200_air() { for (auto& j : jit) nb::jit_release(j); for (auto& j : jit_logup) nb::jit_release(j); }
+  ~nb200_air() { for (auto* v : {&jit, &jit_d2, &jit_logup}) for (auto& j : *v) nb::jit_release(j); }
 };
 
 namespace nb {
@@ -28,7 +29,7 @@ namespace nb {
 struct SchemeTree {
   std::vector<ColsPtr> coeffs, ldes;      // batches, commitment order
   std::vector<ColsPtr> half_ext;          // per batch or empty: the polynomials on the first half of CanonicCoset(lde log + 1).circle_domain(),
-                                          // precomputed at commit time when the scheme was told the AIR's degree bound (see component_quotients)
+                                          // precomputed by the sharded commit when the scheme was told the AIR's degree bound (see component_quotients)
   struct ColLoc { u32 batch, idx, log; };
   std::vector<ColLoc> cols;               // global column index -> (batch, index in batch, polynomial log size)
   TreePtr merkle;
@@ -74,22 +75,24 @@ static nb200_status upload_params(nb200_ctx* ctx, const void* params, size_t n_p
   return NB200_OK;
 }
 
-// The component's specialised kernel (constraints, or the LogUp program when `logup`), compiled on first use; nullptr = none.
+// The component's specialised kernel, compiled on first use; nullptr = none.
 // `interp_fallback`: the caller can run the bytecode interpreter, so programs shorter than JIT_MIN_INSTR are not compiled and a failed
 // compile is only logged (NB200_TRACE).  The sharded row kernels have no interpreter: they try every program and reject a nullptr.
-static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp_idx, bool logup, bool interp_fallback) {
-  std::vector<JitKernel>& v = logup ? air_h->jit_logup : air_h->jit;
+enum JitKind { JIT_CONSTRAINTS, JIT_D2, JIT_LOGUP };
+static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp_idx, JitKind kind, bool interp_fallback) {
+  std::vector<JitKernel>& v = kind == JIT_LOGUP ? air_h->jit_logup : kind == JIT_D2 ? air_h->jit_d2 : air_h->jit;
   if (v.size() != air_h->prog.comps.size()) v.resize(air_h->prog.comps.size());
   JitKernel& jk = v[comp_idx];
   if (!jk.tried) {
     jk.tried = true;
     const AirComponent& c = air_h->prog.comps[comp_idx];
-    const bool worth_it = logup ? (c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0) : c.prog.size() >= JIT_MIN_INSTR;
+    const bool worth_it = kind == JIT_LOGUP ? (c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0) : c.prog.size() >= JIT_MIN_INSTR;
     if ((worth_it || !interp_fallback) && jit_enabled()) {
-      nb200_status st = logup ? jit_compile_logup(ctx, c, &jk) : jit_compile_constraints(ctx, c, &jk);
+      nb200_status st = kind == JIT_LOGUP ? jit_compile_logup(ctx, c, &jk) : jit_compile_constraints(ctx, c, kind == JIT_D2, &jk);
       if (interp_fallback) {
-        if (st != NB200_OK && ctx->trace) fprintf(stderr, "[nb200] jit unavailable for %s: %s\n", logup ? "logup program" : "component", ctx->err.c_str());
-        trace_mark(ctx, logup ? "jit: compile logup (one-time)" : "jit: compile (one-time)");
+        static const char* what[] = {"component", "component (D2)", "logup program"};
+        if (st != NB200_OK && ctx->trace) fprintf(stderr, "[nb200] jit unavailable for %s: %s\n", what[kind], ctx->err.c_str());
+        trace_mark(ctx, kind == JIT_LOGUP ? "jit: compile logup (one-time)" : "jit: compile (one-time)");
       }
     }
   }
@@ -119,22 +122,14 @@ nb200_status scheme_commit_evals(nb200_scheme* s, const nb200_cols* const* evals
   if (max_log >= 1) NB_TRY(twiddles_prepare(ctx, max_log));
   trace_mark(ctx, nullptr);
   SchemeTree t;
+  // (the half coset D2 is not evaluated here: the quotient step extends only the few columns its high-degree constraints read)
   for (size_t b = 0; b < n; ++b) {
-    ColsPtr co, lde, hx;
+    ColsPtr co, lde;
     NB_TRY(alloc(ctx, co, evals[b]->n_cols, evals[b]->log_size));
     NB_TRY(alloc(ctx, lde, evals[b]->n_cols, evals[b]->log_size + s->log_blowup));
-    // when the AIR's degree bound says the quotient step will need these polynomials on the half coset D2 (component_quotients, Q_HALF),
-    // the fused pipeline emits them from the coefficient tiles it already holds in shared memory (if the memory is there)
-    const u32 lde_log = lde->log_size;
-    if (s->hint_log_expand == s->log_blowup + 1 && lde_log > 8) {
-      const size_t need = (co->n_cols << lde_log) * 4;
-      if (ctx->live_bytes + need + ((size_t)40 << 30) < ctx->total_mem && twiddles_prepare(ctx, lde_log + 1) == NB200_OK)
-        alloc(ctx, hx, co->n_cols, lde_log);   // without it the quotient step extends the columns itself
-    }
-    NB_TRY(commit_transforms(ctx, evals[b]->d, co->d, lde->d, hx ? hx->d : nullptr, co->n_cols, co->log_size, s->log_blowup));
+    NB_TRY(commit_transforms(ctx, evals[b]->d, co->d, lde->d, nullptr, co->n_cols, co->log_size, s->log_blowup));
     t.coeffs.push_back(std::move(co));
     t.ldes.push_back(std::move(lde));
-    t.half_ext.push_back(std::move(hx));
   }
   trace_mark(ctx, "commit: ifft+lde");
   NB_TRY(finish_tree(ctx, t, ch));
@@ -166,22 +161,14 @@ nb200_status scheme_commit_host(nb200_scheme* s, const void* const* host, const 
     pre_leaf.reset(sink.tree);
   }
   for (size_t b = 0; b < n; ++b) {
-    ColsPtr co, lde, hx;
+    ColsPtr co, lde;
     NB_TRY(alloc(ctx, evals[b], n_cols[b], log_sizes[b]));
     NB_TRY(alloc(ctx, co, n_cols[b], log_sizes[b]));
     NB_TRY(alloc(ctx, lde, n_cols[b], log_sizes[b] + s->log_blowup));
-    // The copy from the host is PCIe-bound and leaves the SMs mostly idle: if the AIR's degree bound is known to need the half-coset
-    // evaluations of these polynomials later (component_quotients, Q_HALF), compute them now, chunk by chunk, in that shadow.
-    const u32 lde_log = log_sizes[b] + s->log_blowup;
-    if (s->hint_log_expand == s->log_blowup + 1 && lde_log > 8) {
-      NB_TRY(twiddles_prepare(ctx, lde_log + 1));
-      NB_TRY(alloc(ctx, hx, n_cols[b], lde_log));
-    }
-    NB_TRY(upload_transform_pipelined(ctx, host[b], n_cols[b], log_sizes[b], coset_order, s->log_blowup, evals[b]->d, co->d, lde->d, hx ? hx->d : nullptr,
+    NB_TRY(upload_transform_pipelined(ctx, host[b], n_cols[b], log_sizes[b], coset_order, s->log_blowup, evals[b]->d, co->d, lde->d, nullptr,
                                       (long)b == leaf_batch ? &sink : nullptr, elem_bytes ? elem_bytes[b] : 4u));
     t.coeffs.push_back(std::move(co));
     t.ldes.push_back(std::move(lde));
-    t.half_ext.push_back(std::move(hx));
   }
   trace_mark(ctx, "commit(host): h2d+ifft+lde");
   NB_TRY(finish_tree(ctx, t, ch, pre_leaf.release()));   // merkle_commit consumes the leaf layer, also when it fails
@@ -556,7 +543,10 @@ static qm31 load_param(const u32* p) { return qm31_make(p[0], p[1], p[2], p[3]);
 //            at all) and on D2 = the first half of CanonicCoset(eval_log).circle_domain() (a half-size transform).  In the circle-FFT
 //            basis a polynomial with coefficients [lo | hi] is lo + pi^(eval_log-2)(x) * hi, and pi^(eval_log-2)(x) vanishes on D1 and is
 //            the constant top-layer twiddle t on D2, so  lo = interpolate_D1(q|D1)  and  hi = interpolate_D2((q|D2 - lo|D2) / t).
-//            Halves the extension work (the largest stage of prove at 2^20 rows).
+//            A constraint of degree d <= AIR_LOW_DEGREE (air.h) has a quotient of circle degree at most 2^(eval_log - 2): its hi part is
+//            zero.  By linearity hi(q) = hi(q_high), q_high the sum over the constraints of higher degree only, so D2 needs only those
+//            constraints and only the columns they read:  hi = interpolate_D2((q_high|D2 - lo(q_high)|D2) / t),  lo(q_high) taken from
+//            q_high|D1, which the D1 kernel sums on the side.  (The bytecode interpreter evaluates every constraint on D2: q_high = q.)
 enum QuotMode { Q_FULL = 0, Q_HALF = 1 };
 static QuotMode quotient_mode(const nb200_scheme* s, const AirComponent& c) {
   const u32 lde = c.log_size + s->log_blowup;
@@ -566,22 +556,33 @@ static QuotMode quotient_mode(const nb200_scheme* s, const AirComponent& c) {
 // ComponentProver::evaluate_constraint_quotients_on_domain for one component: bring every column the component reads onto
 // the evaluation rows, run the (JIT-specialised or interpreted) constraint kernel, ADD into the accumulators.
 //   Q_FULL: accum = 4 columns of 2^eval_log (evaluations on the canonic domain);
-//   Q_HALF: accum = q on D1, accum_hi = q on D2, each 4 columns of 2^(eval_log - 1).
+//   Q_HALF: accum = q on D1, accum_hi = q_high on D2, accum_sub = q_high on D1, each 4 columns of 2^(eval_log - 1).
 nb200_status component_quotients(nb200_scheme* s, nb200_air* air_h, size_t comp_idx, const u32* d_params, const std::vector<qm31>& coeff,
-                                 QuotMode mode, nb200_cols* accum, nb200_cols* accum_hi) {
+                                 QuotMode mode, nb200_cols* accum, nb200_cols* accum_hi, nb200_cols* accum_sub) {
   nb200_ctx* ctx = s->ctx;
   const AirProgram& air = air_h->prog;
   NB_ARG(ctx, comp_idx < air.comps.size(), "constraint quotients: component index");
   const AirComponent& c = air.comps[comp_idx];
   const u32 elog = c.eval_log(), lde_log = c.log_size + s->log_blowup;
-  if (mode == Q_HALF) NB_ARG(ctx, elog == lde_log + 1 && accum && accum_hi && accum->n_cols == 4 && accum_hi->n_cols == 4 && accum->log_size == lde_log && accum_hi->log_size == lde_log,
-                             "constraint quotients: half-domain accumulators");
+  auto half_acc = [&](const nb200_cols* a) { return a && a->n_cols == 4 && a->log_size == lde_log; };
+  if (mode == Q_HALF) NB_ARG(ctx, elog == lde_log + 1 && half_acc(accum) && half_acc(accum_hi) && half_acc(accum_sub), "constraint quotients: half-domain accumulators");
   else NB_ARG(ctx, accum && accum->n_cols == 4 && accum->log_size == elog, "constraint quotients: accumulator must be 4 columns of the evaluation domain size");
   NB_ARG(ctx, coeff.size() == c.n_constraints, "constraint quotients: one coefficient per constraint");
   NB_TRY(twiddles_prepare(ctx, elog));
   const bool reuse_lde = (mode == Q_FULL && elog == lde_log);
+  const JitKernel* jp = ensure_jit(ctx, air_h, comp_idx, JIT_CONSTRAINTS, true);
+  // Q_HALF: with the specialised kernels D2 evaluates the high-degree constraints only (none: D2 is skipped), else every constraint
+  const std::vector<char> high = high_constraints(c);
+  const JitKernel* jd2 = nullptr;
+  bool split = false;
+  if (mode == Q_HALF && jit_usable(jp, c, lde_log)) {
+    jd2 = count_high(high) ? ensure_jit(ctx, air_h, comp_idx, JIT_D2, true) : nullptr;
+    split = !count_high(high) || jd2;
+  }
+  const std::vector<char> on_d2 = split ? masks_read_by(c, high) : std::vector<char>(c.masks.size(), mode == Q_HALF ? 1 : 0);
   std::map<std::pair<u32, u32>, ColsPtr> ext;
-  std::vector<const u32*> mask_cols(c.masks.size()), mask_lde(c.masks.size());
+  std::map<std::pair<u32, u32>, u32> d2_slot;   // Q_HALF: (tree, column) -> its column in d2_ext
+  std::vector<const u32*> mask_cols(c.masks.size(), nullptr), mask_lde(c.masks.size());
   for (size_t m = 0; m < c.masks.size(); ++m) {
     const AirMask& mk = c.masks[m];
     NB_ARG(ctx, mk.tree < s->trees.size() && mk.col < s->trees[mk.tree].cols.size(), "prove: AIR references a column that was not committed");
@@ -590,26 +591,48 @@ nb200_status component_quotients(nb200_scheme* s, nb200_air* air_h, size_t comp_
     NB_ARG(ctx, loc.log == c.log_size, "prove: column size differs from its component's log_size");
     mask_lde[m] = tr.ldes[loc.batch]->col(loc.idx);
     if (reuse_lde) { mask_cols[m] = mask_lde[m]; continue; }
-    if (mode == Q_HALF && loc.batch < tr.half_ext.size() && tr.half_ext[loc.batch]) {
-      mask_cols[m] = tr.half_ext[loc.batch]->col(loc.idx);   // precomputed at commit time
+    if (mode == Q_HALF) {
+      if (!on_d2[m]) continue;
+      if (loc.batch < tr.half_ext.size() && tr.half_ext[loc.batch]) mask_cols[m] = tr.half_ext[loc.batch]->col(loc.idx);   // precomputed at commit time
+      else d2_slot.emplace(std::make_pair(mk.tree, mk.col), (u32)d2_slot.size());
       continue;
     }
     ColsPtr& e = ext[std::make_pair(mk.tree, loc.batch)];
     if (!e) {
       const nb200_cols* co = tr.coeffs[loc.batch].get();
-      NB_TRY(alloc(ctx, e, co->n_cols, mode == Q_HALF ? lde_log : elog));
-      if (mode == Q_HALF) NB_TRY(fft_evaluate(ctx, co->d, co->log_size, e->d, lde_log, co->n_cols, elog));   // first half of canonic(elog)
-      else NB_TRY(fft_evaluate(ctx, co->d, co->log_size, e->d, elog, co->n_cols));
+      NB_TRY(alloc(ctx, e, co->n_cols, elog));
+      NB_TRY(fft_evaluate(ctx, co->d, co->log_size, e->d, elog, co->n_cols));
     }
     mask_cols[m] = e->col(loc.idx);
   }
+  // Q_HALF: the columns D2 reads, gathered from the committed coefficients into one batch and evaluated on the first half of canonic(elog)
+  ColsPtr d2_ext;
+  if (!d2_slot.empty()) {
+    ColsPtr gathered;
+    NB_TRY(alloc(ctx, gathered, d2_slot.size(), c.log_size));
+    for (auto& kv : d2_slot)
+      NB_CUDA(ctx, cudaMemcpyAsync(gathered->col(kv.second), s->trees[kv.first.first].coeff_ptr(kv.first.second), (size_t)4 << c.log_size,
+                                   cudaMemcpyDeviceToDevice, ctx->stream));
+    NB_TRY(alloc(ctx, d2_ext, d2_slot.size(), lde_log));
+    NB_TRY(fft_evaluate(ctx, gathered->d, c.log_size, d2_ext->d, lde_log, d2_slot.size(), elog));
+    for (size_t m = 0; m < c.masks.size(); ++m) {
+      auto it = d2_slot.find(std::make_pair(c.masks[m].tree, c.masks[m].col));
+      if (on_d2[m] && it != d2_slot.end()) mask_cols[m] = d2_ext->col(it->second);
+    }
+  }
   trace_mark(ctx, "constraints: extend columns");
-  const JitKernel* jp = ensure_jit(ctx, air_h, comp_idx, false, true);
   if (mode == Q_HALF) {
     u32* lo[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
     u32* hi[4] = {accum_hi->col(0), accum_hi->col(1), accum_hi->col(2), accum_hi->col(3)};
-    NB_TRY(constraint_eval(ctx, c, mask_lde, d_params, coeff, lo, jp, lde_log, lde_log));                        // D1: the committed LDE
-    NB_TRY(constraint_eval(ctx, c, mask_cols, d_params, coeff, hi, jp, lde_log, elog));     // D2: first half of canonic(elog)
+    u32* sub[4] = {accum_sub->col(0), accum_sub->col(1), accum_sub->col(2), accum_sub->col(3)};
+    if (split) {
+      NB_TRY(constraint_eval(ctx, c, mask_lde, d_params, coeff, lo, jp, lde_log, lde_log, 0, 0, sub));   // D1: the committed LDE; q and q_high
+      if (jd2) NB_TRY(constraint_eval(ctx, c, mask_cols, d_params, coeff, hi, jd2, lde_log, elog));      // D2: first half of canonic(elog)
+    } else {
+      NB_TRY(constraint_eval(ctx, c, mask_lde, d_params, coeff, lo, jp, lde_log, lde_log));
+      NB_TRY(constraint_eval(ctx, c, mask_lde, d_params, coeff, sub, jp, lde_log, lde_log));
+      NB_TRY(constraint_eval(ctx, c, mask_cols, d_params, coeff, hi, jp, lde_log, elog));
+    }
   } else {
     u32* accp[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
     NB_TRY(constraint_eval(ctx, c, mask_cols, d_params, coeff, accp, jp, elog, elog));
@@ -627,11 +650,12 @@ static bool component_is_sharded(const nb200_scheme* s, const AirComponent& c) {
 // evaluate_constraint_quotients_on_domain of the sharded (main) component: this rank evaluates ITS rows of D1 (from the LDE row slices) and of D2
 // (from the D2 row slices) — masks at a row offset read the replicated full columns — and the accumulator columns are all-gathered in place.
 static nb200_status component_quotients_sharded(nb200_scheme* s, nb200_air* air_h, size_t comp_idx, const u32* d_params, const std::vector<qm31>& coeff,
-                                                nb200_cols* accum, nb200_cols* accum_hi) {
+                                                nb200_cols* accum, nb200_cols* accum_hi, nb200_cols* accum_sub) {
   nb200_ctx* ctx = s->ctx;
   const AirComponent& c = air_h->prog.comps[comp_idx];
   const u32 elog = c.eval_log(), lde_log = c.log_size + s->log_blowup, k = (u32)comm_log_world(ctx);
-  NB_ARG(ctx, elog == lde_log + 1 && accum && accum_hi && accum->log_size == lde_log && accum_hi->log_size == lde_log, "sharded constraint quotients: the component must use the half-domain route");
+  NB_ARG(ctx, elog == lde_log + 1 && accum && accum_hi && accum_sub && accum->log_size == lde_log && accum_hi->log_size == lde_log && accum_sub->log_size == lde_log,
+         "sharded constraint quotients: the component must use the half-domain route");
   NB_ARG(ctx, coeff.size() == c.n_constraints, "constraint quotients: one coefficient per constraint");
   const size_t S = (size_t)1 << (lde_log - k);
   const u32 row0 = (u32)(comm_rank(ctx) * S);
@@ -649,26 +673,36 @@ static nb200_status component_quotients_sharded(nb200_scheme* s, nb200_air* air_
       m_lde[m] = f->second->d; m_hx[m] = h->second->d;
     }
   }
-  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, false, false);
-  NB_ARG(ctx, jk != nullptr, "sharded constraint quotients need the specialised kernel");
+  // the same split as component_quotients: D1 sums q and q_high, D2 evaluates the high-degree constraints only (from every column's D2 rows,
+  // which the sharded commit still computes)
+  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, JIT_CONSTRAINTS, false);
+  const bool any_high = count_high(high_constraints(c)) > 0;
+  const JitKernel* jd2 = any_high ? ensure_jit(ctx, air_h, comp_idx, JIT_D2, false) : nullptr;
+  NB_ARG(ctx, jk != nullptr && (!any_high || jd2 != nullptr), "sharded constraint quotients need the specialised kernel");
+  const std::vector<char> on_d2 = masks_read_by(c, high_constraints(c));
+  for (size_t m = 0; m < c.masks.size(); ++m) if (!on_d2[m]) m_hx[m] = nullptr;
   u32* lo[4] = {accum->col(0), accum->col(1), accum->col(2), accum->col(3)};
   u32* hi[4] = {accum_hi->col(0), accum_hi->col(1), accum_hi->col(2), accum_hi->col(3)};
-  NB_TRY(constraint_eval(ctx, c, m_lde, d_params, coeff, lo, jk, lde_log, lde_log, row0, S));
-  NB_TRY(constraint_eval(ctx, c, m_hx, d_params, coeff, hi, jk, lde_log, elog, row0, S));
-  for (int q = 0; q < 4; ++q) { NB_TRY(comm_all_gather_dev(ctx, lo[q] + row0, S, lo[q])); NB_TRY(comm_all_gather_dev(ctx, hi[q] + row0, S, hi[q])); }
+  u32* sub[4] = {accum_sub->col(0), accum_sub->col(1), accum_sub->col(2), accum_sub->col(3)};
+  NB_TRY(constraint_eval(ctx, c, m_lde, d_params, coeff, lo, jk, lde_log, lde_log, row0, S, sub));
+  if (jd2) NB_TRY(constraint_eval(ctx, c, m_hx, d_params, coeff, hi, jd2, lde_log, elog, row0, S));
+  for (int q = 0; q < 4; ++q)
+    for (u32* a : {lo[q], hi[q], sub[q]}) NB_TRY(comm_all_gather_dev(ctx, a + row0, S, a));
   trace_mark(ctx, "constraints: row kernel (sharded) + all-gather");
   return NB200_OK;
 }
 
-// coefficients (4 columns of 2^elog, circle-FFT basis) of the quotient polynomial held by a Q_HALF accumulator pair; lo/hi are consumed
-static nb200_status half_to_coeffs(nb200_ctx* ctx, nb200_cols* lo, nb200_cols* hi, u32 elog, u32* out /* 4 columns */, size_t out_stride /* >= 2^elog */) {
+// coefficients (4 columns of 2^elog, circle-FFT basis) of the quotient polynomial held by a Q_HALF accumulator triple (q|D1, q_high|D2,
+// q_high|D1: see quotient_mode); they are consumed
+static nb200_status half_to_coeffs(nb200_ctx* ctx, nb200_cols* lo, nb200_cols* hi, nb200_cols* sub, u32 elog, u32* out /* 4 columns */, size_t out_stride /* >= 2^elog */) {
   const u32 h = elog - 1;
   const size_t hl = (size_t)1 << h;
   NB_TRY(fft_interpolate(ctx, lo->d, lo->d, 4, h));                 // lo = coefficients of q mod pi^(elog-2)
+  NB_TRY(fft_interpolate(ctx, sub->d, sub->d, 4, h));               // lo(q_high)
   ColsPtr t;
   NB_TRY(alloc(ctx, t, 4, h));
-  NB_TRY(fft_evaluate(ctx, lo->d, h, t->d, h, 4, elog));            // lo evaluated on D2
-  NB_TRY(sub_scale_top_twiddle(ctx, hi->d, t->d, 4 * hl, elog));    // (q|D2 - lo|D2) / t
+  NB_TRY(fft_evaluate(ctx, sub->d, h, t->d, h, 4, elog));           // lo(q_high) evaluated on D2
+  NB_TRY(sub_scale_top_twiddle(ctx, hi->d, t->d, 4 * hl, elog));    // (q_high|D2 - lo(q_high)|D2) / t
   NB_TRY(fft_interpolate(ctx, hi->d, hi->d, 4, h, elog));           // hi coefficients
   // the composition's coefficient columns are 2^comp_log apart; this accumulator's polynomial may be smaller (a machine whose largest
   // evaluation domain belongs to another component): found by the prover2-shaped machine, tests/test_gpu_prove_parity.py
@@ -730,8 +764,8 @@ static nb200_status commit_composition(nb200_scheme* s, nb200_air* air_h, const 
   DevBuf d_params;
   NB_TRY(upload_params(ctx, params.data(), params.size(), d_params));
 
-  // accumulators per (evaluation log, mode): Q_FULL -> {evals on canonic(elog), -}; Q_HALF -> {q on D1, q on D2}
-  struct Acc { ColsPtr a, b; };
+  // accumulators per (evaluation log, mode): Q_FULL -> {evals on canonic(elog), -, -}; Q_HALF -> {q on D1, q_high on D2, q_high on D1}
+  struct Acc { ColsPtr a, b, c; };
   std::map<std::pair<u32, int>, Acc> acc;
   size_t g0 = 0;
   for (const AirComponent& c : air.comps) {
@@ -740,13 +774,13 @@ static nb200_status commit_composition(nb200_scheme* s, nb200_air* air_h, const 
     Acc& a = acc[std::make_pair(elog, (int)mode)];
     if (!a.a) {
       NB_TRY(zeroed(ctx, mode == Q_HALF ? elog - 1 : elog, a.a));
-      if (mode == Q_HALF) NB_TRY(zeroed(ctx, elog - 1, a.b));
+      if (mode == Q_HALF) { NB_TRY(zeroed(ctx, elog - 1, a.b)); NB_TRY(zeroed(ctx, elog - 1, a.c)); }
     }
     std::vector<qm31> coeff(c.n_constraints);
     for (u32 k = 0; k < c.n_constraints; ++k) coeff[k] = powers[n_total - 1 - (g0 + k)];
     const size_t comp_idx = &c - &air.comps[0];
-    if (component_is_sharded(s, c)) NB_TRY(component_quotients_sharded(s, air_h, comp_idx, d_params.p, coeff, a.a.get(), a.b.get()));
-    else NB_TRY(component_quotients(s, air_h, comp_idx, d_params.p, coeff, mode, a.a.get(), a.b.get()));
+    if (component_is_sharded(s, c)) NB_TRY(component_quotients_sharded(s, air_h, comp_idx, d_params.p, coeff, a.a.get(), a.b.get(), a.c.get()));
+    else NB_TRY(component_quotients(s, air_h, comp_idx, d_params.p, coeff, mode, a.a.get(), a.b.get(), a.c.get()));
     g0 += c.n_constraints;
   }
   // DomainEvaluationAccumulator::finalize.  Upstream folds the per-size accumulators upwards (evaluate the running polynomial on the next
@@ -756,7 +790,7 @@ static nb200_status commit_composition(nb200_scheme* s, nb200_air* air_h, const 
   for (auto& kv : acc) {
     const u32 elog = kv.first.first;
     nb200_cols* a = kv.second.a.get();
-    if (kv.first.second == Q_HALF) NB_TRY(half_to_coeffs(ctx, a, kv.second.b.get(), elog, cur->d, (size_t)1 << comp_log));
+    if (kv.first.second == Q_HALF) NB_TRY(half_to_coeffs(ctx, a, kv.second.b.get(), kv.second.c.get(), elog, cur->d, (size_t)1 << comp_log));
     else {
       NB_TRY(fft_interpolate(ctx, a->d, a->d, 4, elog));
       NB_TRY(add_cols_strided(ctx, cur->d, (size_t)1 << comp_log, a->d, (size_t)1 << elog, (size_t)1 << elog, 4));
@@ -1132,7 +1166,7 @@ nb200_status gen_interaction(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, con
   ColsPtr o;
   NB_TRY(alloc(ctx, o, (size_t)4 * c.n_logup_cols(), c.log_size));
   trace_mark(ctx, nullptr);
-  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, true, true);
+  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, JIT_LOGUP, true);
   nb200_status st = logup_generate(ctx, c, mask_cols, d_params.p, o->d, claimed, jk);
   trace_mark(ctx, "logup interaction trace");
   cudaStreamSynchronize(ctx->stream);
@@ -1162,7 +1196,7 @@ nb200_status gen_interaction_sharded(nb200_scheme* s, nb200_air* air_h, u32 comp
     NB_ARG(ctx, tr.sharded && mk.col < tr.cols.size() && tr.cols[mk.col].batch == SchemeTree::BIG && tr.big_eval_rows, "gen_interaction_sharded: the component may only read sharded trace columns (commit with keep_eval_rows)");
     mask_cols[m] = tr.big_eval_rows->col(tr.cols[mk.col].idx);   // this rank's trace rows
   }
-  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, true, false);
+  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, JIT_LOGUP, false);
   NB_ARG(ctx, jk != nullptr, "gen_interaction_sharded needs the specialised logup kernel");
   DevBuf d_params;
   NB_TRY(upload_params(ctx, params.data(), params.size(), d_params));
@@ -1254,12 +1288,28 @@ void nb200_air_free(nb200_air* a) { delete a; }
 uint32_t nb200_air_n_params(const nb200_air* a) { return a ? a->prog.n_params : 0; }
 uint32_t nb200_air_n_components(const nb200_air* a) { return a ? (uint32_t)a->prog.comps.size() : 0; }
 uint64_t nb200_kernel_source_key(const char* src) { return src ? jit_source_key(src) : 0; }
+nb200_status nb200_air_constraint_degrees(const nb200_air* a, uint32_t component, uint32_t* degrees, size_t n) {
+  if (!a || component >= a->prog.comps.size() || (n && !degrees)) return NB200_ERR_ARG;
+  const std::vector<u32> d = constraint_degrees(a->prog.comps[component]);
+  if (n != d.size()) return NB200_ERR_ARG;
+  std::copy(d.begin(), d.end(), degrees);
+  return NB200_OK;
+}
+nb200_status nb200_air_d2_masks(const nb200_air* a, uint32_t component, uint8_t* flags, size_t n) {
+  if (!a || component >= a->prog.comps.size()) return NB200_ERR_ARG;
+  const AirComponent& c = a->prog.comps[component];
+  if (n != c.masks.size() || (n && !flags)) return NB200_ERR_ARG;
+  const std::vector<char> used = masks_read_by(c, high_constraints(c));
+  for (size_t m = 0; m < n; ++m) flags[m] = used[m] ? 1 : 0;
+  return NB200_OK;
+}
 nb200_status nb200_air_kernel_source(const nb200_air* a, uint32_t component, int which, char** out) {
-  if (!a || !out || component >= a->prog.comps.size() || which < 0 || which > 1) return NB200_ERR_ARG;
+  if (!a || !out || component >= a->prog.comps.size() || which < 0 || which > 2) return NB200_ERR_ARG;
   const AirComponent& c = a->prog.comps[component];
   *out = nullptr;
-  if ((which == 0 ? c.prog.size() : c.logup_prog.size()) < JIT_MIN_INSTR || (which == 1 && c.n_logup_cols() == 0)) return NB200_ERR_STATE;  // runs on the interpreter
-  std::string src = (which == 0) ? jit_source(c) : jit_logup_source(c);
+  if ((which == 1 ? c.logup_prog.size() : c.prog.size()) < JIT_MIN_INSTR || (which == 1 && c.n_logup_cols() == 0)) return NB200_ERR_STATE;  // runs on the interpreter
+  if (which == 2 && count_high(high_constraints(c)) == 0) return NB200_ERR_STATE;   // nothing to evaluate on D2
+  std::string src = which == 1 ? jit_logup_source(c) : jit_source(c, which == 2);
   char* o = (char*)malloc(src.size() + 1);
   if (!o) return NB200_ERR_OOM;
   memcpy(o, src.c_str(), src.size() + 1);
@@ -1398,7 +1448,7 @@ nb200_status nb200_constraint_quotients(nb200_scheme* s, const nb200_air* air, u
   if (n_coeffs) memcpy(cf.data(), coeffs, n_coeffs * 16);
   DevBuf d_params;
   NB_TRY(upload_params(ctx, params, n_params, d_params));
-  NB_TRY(component_quotients(s, const_cast<nb200_air*>(air), component, d_params.p, cf, Q_FULL, accum, nullptr));
+  NB_TRY(component_quotients(s, const_cast<nb200_air*>(air), component, d_params.p, cf, Q_FULL, accum, nullptr, nullptr));
   // params is caller memory: make sure the copy has been consumed before returning
   NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return NB200_OK;

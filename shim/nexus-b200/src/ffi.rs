@@ -104,6 +104,8 @@ extern "C" {
     pub fn nb200_air_n_components(air: *const nb200_air) -> u32;
     pub fn nb200_air_kernel_source(air: *const nb200_air, component: u32, which: c_int, out: *mut *mut c_char) -> c_int;
     pub fn nb200_kernel_source_key(source: *const c_char) -> u64;
+    pub fn nb200_air_constraint_degrees(air: *const nb200_air, component: u32, degrees: *mut u32, n: usize) -> c_int;
+    pub fn nb200_air_d2_masks(air: *const nb200_air, component: u32, flags: *mut u8, n: usize) -> c_int;
     pub fn nb200_air_max_log_expand(air: *const nb200_air) -> u32;
     // ---- CommitmentSchemeProver / prove
     pub fn nb200_scheme_new(ctx: *mut nb200_ctx, pow_bits: u32, log_blowup: u32, log_last_layer_degree_bound: u32, n_queries: u32, out: *mut *mut nb200_scheme) -> c_int;
