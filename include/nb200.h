@@ -190,11 +190,15 @@ nb200_status nb200_air_load(nb200_ctx*, const uint32_t* words, size_t n_words, n
 void nb200_air_free(nb200_air*);
 uint32_t nb200_air_n_params(const nb200_air*);
 uint32_t nb200_air_n_components(const nb200_air*);
+/* the component's constraint count, LogUp constraints included (0 for an unknown component) */
+uint32_t nb200_air_n_constraints(const nb200_air*, uint32_t component);
 /* the CUDA C source a component's programs are specialised to at first use (NVRTC, sm_90a): which = 0 the constraint
  * program, 1 the logup (interaction trace) program, 2 the constraints of degree above 2 alone (evaluated on the extra half
  * coset of a component with log_expand = log_blowup + 1).  malloc'ed, NUL-terminated, free with nb200_free.  Works without a
  * device (ctx may have been NULL at nb200_air_load).  NB200_ERR_STATE (and *out = NULL): the program is too short to be
- * specialised and runs on the bytecode interpreter, or (which = 2) the component has no constraint of degree above 2. */
+ * specialised and runs on the bytecode interpreter, or (which = 2) the component has no constraint of degree above 2.
+ * which = 3: the constraint check of nb200_check_constraints (any program length; NB200_ERR_STATE only when the component has
+ * no constraint). */
 nb200_status nb200_air_kernel_source(const nb200_air*, uint32_t component, int which, char** out);
 /* degree of each of the component's n constraints in the trace columns (masks 1, constants and parameters 0, products add,
  * sums take the maximum), and which of its n masks the constraints of degree above 2 read (flags[m] = 1) */
@@ -239,6 +243,18 @@ nb200_status nb200_gen_interaction_trace(nb200_ctx*, const nb200_air*, uint32_t 
  * Returns NB200_ERR_CONSTRAINTS for ProvingError::ConstraintsNotSatisfied. */
 nb200_status nb200_prove(nb200_scheme*, const nb200_air*, const uint32_t* params, size_t n_params, nb200_channel*,
                          uint8_t** proof_out, size_t* proof_len);
+/* assert_constraints_on_polys (stwo-constraint-framework) for one component, on the GPU: every constraint is evaluated on every row of
+ * the trace domain CanonicCoset(log_size) and tested for zero.  tree0 / tree1 / tree2 = the evaluation batches of the three committed
+ * trees (commitment order, as committed); params = the table nb200_prove takes (lookup elements, cumsum shifts).  For constraint k
+ * (declaration order as in nb200_air_constraint_degrees, the LogUp constraints last; n = the component's constraint count):
+ * n_failing[k] = the rows where it does not hold, first_row[k] = the first of them in trace (coset) order — the index into the host
+ * column before finalize_columns — or UINT64_MAX when it holds everywhere.  Returns NB200_OK whether or not a constraint fails
+ * (also for a component without constraints, n = 0);
+ * NB200_ERR_ARG for a missing or wrongly sized column, NB200_ERR_STATE when the generated check kernel is unavailable (NB200_JIT=0). */
+nb200_status nb200_check_constraints(nb200_ctx*, const nb200_air*, uint32_t component,
+                                     const nb200_cols* const* tree0, size_t n0, const nb200_cols* const* tree1, size_t n1,
+                                     const nb200_cols* const* tree2, size_t n2, const uint32_t* params, size_t n_params,
+                                     uint64_t* n_failing, uint64_t* first_row, size_t n);
 
 /* ---- one PROOF over N GPUs ---------------------------------------------------------------------------------------------------
  * Every rank calls the same sequence (the Machine::prove order, machine.rs:197-290) with its own shard; transcript, roots and proof

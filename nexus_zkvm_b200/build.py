@@ -83,8 +83,10 @@ SHIPPED_MULTI = [list(range(4, 12)), list(range(4, 18)), list(range(4, 22))]
 SHIPPED_NEXUS_V1 = [8, 9, 12, 16, 18, 20, 22, 24]   # 18 / 24: the sharded large-proof test (default size / configs[3])
 
 
-def kernel_sources(words):
-    """[(cache key, CUDA C source)] of the kernels the library specialises for an AIR (no GPU needed)."""
+def kernel_sources(words, short_checks=False):
+    """[(cache key, CUDA C source)] of the kernels the library specialises for an AIR (no GPU needed).  The constraint check (which = 3) is
+    listed for the components whose constraint program is specialised; `short_checks` adds it for the short programs too (small table
+    components, whose check kernel is often the same source in several machines)."""
     import ctypes as C
     import numpy as np
     L = C.CDLL(LIB)
@@ -99,10 +101,14 @@ def kernel_sources(words):
         raise RuntimeError("nb200_air_load failed")
     out = []
     for comp in range(L.nb200_air_n_components(air)):
-        for which in (0, 1, 2):   # constraints, LogUp program, constraints of degree > 2 (the half coset D2)
+        specialised = False
+        for which in (0, 1, 2, 3):   # constraints, LogUp program, constraints of degree > 2 (the half coset D2), constraint check
+            if which == 3 and not (specialised or short_checks):
+                continue
             p = C.c_void_p()
             if L.nb200_air_kernel_source(air, C.c_uint32(comp), C.c_int(which), C.byref(p)) != 0 or not p:
                 continue
+            specialised = specialised or which == 0
             src = C.string_at(p)
             L.nb200_free(p)
             out.append((int(L.nb200_kernel_source_key(src)), src))
@@ -121,7 +127,7 @@ def precompile_kernels(machines=SHIPPED_MACHINES, verbose=False):
     from .nexus_v1 import NexusV1Machine
     ms += [NexusV1Machine(ls) for ls in SHIPPED_NEXUS_V1]
     for m in ms:
-        for key, src in kernel_sources(m.words):
+        for key, src in kernel_sources(m.words, short_checks=True):
             path = os.path.join(JIT_CACHE, f"{key:016x}.cubin")
             if not os.path.exists(path):
                 todo[path] = src

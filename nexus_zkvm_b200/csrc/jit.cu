@@ -541,10 +541,81 @@ std::string gen_logup_source(const AirComponent& c) {
   o << "}\n";
   return o.str();
 }
+
+// The constraint check (the GPU counterpart of stwo's assert_constraints_on_polys): the plain constraint program on the trace domain
+// CanonicCoset(log_size) itself, one thread per row, with no random coefficients and no vanishing division — every CONSTRB / CONSTRE sink
+// tests its own value for zero.  A warp counts its failing rows with one ballot and finds the first one (in coset order) with one
+// min-reduction, so a constraint costs one atomicAdd and one atomicMin per warp that sees a failure, none per row.
+std::string gen_check_source(const AirComponent& c) {
+  std::ostringstream o;
+  o << "// constraint check on the trace domain: each constraint tested for zero on every row\n";
+  o << kPrelude;
+  const u32 DL = c.log_size;
+  // Columns are in bit-reversed circle-domain order.  Position i holds circle-domain index brev(i), which is coset (trace) row
+  // 2j for circle index j < N/2 and 2N - 2j - 1 above (the inverse of coset_index_to_circle_domain_index); a mask at offset `off`
+  // reads coset row (r + off) mod N, wrapping at both ends as assert_constraints_on_polys does.
+  o << "#define NB_DL " << DL << "u\n#define NB_N (1u << NB_DL)\n"
+    << "__device__ __forceinline__ u32 pos_to_row(u32 i) { const u32 j = __brev(i) >> (32 - NB_DL); return j < NB_N / 2 ? 2 * j : 2 * NB_N - 2 * j - 1; }\n"
+    << "__device__ __forceinline__ u32 row_to_pos(u32 r) { const u32 j = (r & 1) ? NB_N - (r + 1) / 2 : r / 2; return __brev(j) >> (32 - NB_DL); }\n"
+    << "__device__ __forceinline__ u32 offrow(u32 r, int off) { return row_to_pos((r + (u32)off) & (NB_N - 1)); }   // N divides 2^32\n"
+    // every prelude operation returns a canonical residue; P is also taken as zero for a constraint that is a raw (unreduced) cell
+    << "__device__ __forceinline__ bool nzb(u32 v) { return v != 0u && v != P31; }\n"
+    << "__device__ __forceinline__ bool nze(Q v) { return nzb(v.c0) || nzb(v.c1) || nzb(v.c2) || nzb(v.c3); }\n"
+    // one warp: count the failing rows, the first of them in coset order; rows past the domain (live = false) never fail
+    << "__device__ __forceinline__ void check(u32 k, bool bad, u32 r, u32* __restrict__ nfail, u32* __restrict__ first) {\n"
+    << "  const unsigned am = __activemask();\n"
+    << "  const unsigned m = __ballot_sync(am, bad);\n"
+    << "  if (m) {\n"
+    << "    const u32 lo = __reduce_min_sync(am, bad ? r : 0xffffffffu);\n"
+    << "    if ((threadIdx.x & 31u) == (u32)(__ffs(am) - 1)) { atomicAdd(nfail + k, (u32)__popc(m)); atomicMin(first + k, lo); }\n"
+    << "  }\n}\n";
+  const u32 nb = c.n_base_regs ? c.n_base_regs : 1, ne = c.n_ext_regs ? c.n_ext_regs : 1;
+  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; };\n";
+  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
+  auto ld = [&](u32 m) {
+    std::ostringstream s;
+    if (c.masks[m].off == 0) s << "__ldg(ccols[" << m << "] + pos)";
+    else s << "__ldg(ccols[" << m << "] + offrow(r, " << c.masks[m].off << "))";
+    return s.str();
+  };
+  const size_t CH = 250;
+  const size_t n_chunks = (c.prog.size() + CH - 1) / CH;
+  const ChunkLive live = prog_liveness(c.prog, CH, nb, ne);
+  u32 k = 0;
+  for (size_t ci = 0; ci < n_chunks; ++ci) {
+    o << "__device__ __noinline__ void chunk" << ci << "(St& s, const u32* __restrict__ params, u32* __restrict__ nfail, u32* __restrict__ first, u32 pos, u32 r, bool live) {\n";
+    o << "  u32 b[" << nb << "]; Q e[" << ne << "];\n";
+    for (u32 x : live.in_b[ci]) o << "  b[" << x << "] = s.b[" << x << "];";
+    for (u32 x : live.in_e[ci]) o << "  e[" << x << "] = s.e[" << x << "];";
+    o << "\n";
+    for (size_t pc = ci * CH; pc < std::min(c.prog.size(), (ci + 1) * CH); ++pc) {
+      const AirInstr& in = c.prog[pc];
+      o << "  ";
+      if (in.op == OP_CONSTRB) o << "check(" << k++ << "u, live && nzb(b[" << in.a << "]), r, nfail, first);";
+      else if (in.op == OP_CONSTRE) o << "check(" << k++ << "u, live && nze(e[" << in.a << "]), r, nfail, first);";
+      else emit_op(o, in, ld);
+      o << "\n";
+    }
+    for (u32 x : live.out_b[ci]) o << "  s.b[" << x << "] = b[" << x << "];";
+    for (u32 x : live.out_e[ci]) o << "  s.e[" << x << "] = e[" << x << "];";
+    o << "\n}\n";
+  }
+  // nfail[k] / first[k]: rows on which constraint k is non-zero and the first of them in coset order (0xffffffff: none)
+  o << "extern \"C\" __global__ void __launch_bounds__(" << JIT_BLOCK << ", 1) nbjit(const u32* __restrict__ params, u32* __restrict__ nfail, u32* __restrict__ first) {\n"
+    << "  const u32 gid = blockIdx.x * blockDim.x + threadIdx.x;\n"
+    << "  const bool live = gid < NB_N;\n"
+    << "  const u32 pos = live ? gid : 0u;   // a thread past the domain runs row 0 with its results masked: every thread reaches the barriers\n"
+    << "  const u32 r = pos_to_row(pos);\n  St s;\n"
+    << "  for (int i = 0; i < " << nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n";
+  for (size_t ci = 0; ci < n_chunks; ++ci) o << "  chunk" << ci << "(s, params, nfail, first, pos, r, live);\n  __syncthreads();\n";
+  o << "}\n";
+  return o.str();
+}
 }  // namespace
 
 std::string jit_source(const AirComponent& c, bool d2) { return gen_source(c, d2); }
 std::string jit_logup_source(const AirComponent& c) { return gen_logup_source(c); }
+std::string jit_check_source(const AirComponent& c) { return gen_check_source(c); }
 
 bool jit_enabled() {
   const char* e = getenv("NB200_JIT");
@@ -559,10 +630,11 @@ void jit_release(JitKernel& jk) {
 static nb200_status jit_compile_source(nb200_ctx* ctx, const AirComponent& c, const std::string& src, JitKernel* out);
 nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, bool d2, JitKernel* out) { return jit_compile_source(ctx, c, gen_source(c, d2), out); }
 nb200_status jit_compile_logup(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_logup_source(c), out); }
+nb200_status jit_compile_check(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_check_source(c), out); }
 // ---- cubin cache: <directory of this library>/jit_cache/<key>.cubin (or $NB200_JIT_CACHE).  `python -m nexus_zkvm_b200.build`
 // fills it for the shipped machines with nvcc, so a fresh box neither loads libnvrtc nor compiles; kernels compiled at run time are
 // added when the directory is writable.  The key covers the generated source and the target; the D2 variant of a constraint kernel
-// starts with a line of its own, so it never shares a key with the D1 variant.
+// and the constraint check start with a line of their own, so they never share a key with the D1 variant.
 uint64_t jit_source_key(const std::string& src) {
   uint64_t h = 1469598103934665603ull;
   auto mix = [&](const char* p, size_t n) { for (size_t i = 0; i < n; ++i) { h ^= (unsigned char)p[i]; h *= 1099511628211ull; } };
@@ -672,6 +744,18 @@ nb200_status jit_launch_logup(nb200_ctx* ctx, const JitKernel& jk, const u32* co
   NB_TRY(jit_set_cols(ctx, jk, d_cols));
   void* args[] = {(void*)&d_cols, (void*)&d_params, (void*)&d_out, (void*)&log_size};
   cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args, 0, ctx->stream);
+  ctx->launches += 1;
+  if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
+  return NB200_OK;
+}
+
+nb200_status jit_launch_check(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, u32* d_nfail, u32* d_first) {
+  // one thread per trace row; a domain smaller than a CTA (MultiMachine has 2^4-row components) runs as one CTA of exactly its rows
+  const size_t rows = (size_t)1 << jk.log_size;
+  const u32 block = (u32)std::min<size_t>(rows, JIT_LAUNCH_BLOCK);
+  NB_TRY(jit_set_cols(ctx, jk, d_cols));
+  void* args[] = {(void*)&d_params, (void*)&d_nfail, (void*)&d_first};
+  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)((rows + block - 1) / block)), dim3(block), args, 0, ctx->stream);
   ctx->launches += 1;
   if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
   return NB200_OK;

@@ -19,6 +19,7 @@ struct JitKernel {
   void* kernel = nullptr;  // cudaKernel_t
   u32 log_size = 0, eval_log = 0;
   bool tried = false;      // compilation attempted (failed attempts fall back to the interpreter)
+  std::string err;         // why the attempt failed (empty: it did not, or was not made)
 };
 
 // the specialised kernel jk runs constraint_eval on 2^rows_log rows (else the bytecode interpreter does)
@@ -34,6 +35,11 @@ nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, bool
 nb200_status jit_compile_logup(nb200_ctx* ctx, const AirComponent& c, JitKernel* out);
 nb200_status jit_launch_logup(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, u32* d_out, u32 log_size);
 std::string jit_logup_source(const AirComponent& c);
+// the constraint check on the trace domain (jit.cu gen_check_source): per constraint, the count of rows where it is non-zero and the
+// first such row in coset order, accumulated into d_nfail / d_first (zeros / 0xffffffff before the launch)
+std::string jit_check_source(const AirComponent& c);
+nb200_status jit_compile_check(nb200_ctx* ctx, const AirComponent& c, JitKernel* out);
+nb200_status jit_launch_check(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, u32* d_nfail, u32* d_first);
 nb200_status jit_launch_constraints(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, const u32* d_coeff,
                                     const u32* d_dinv, u32* const acc[4], u32 rows_log, u32 dom_log, u32 row0 = 0, size_t n_rows = 0,
                                     u32* const acc_high[4] = nullptr);

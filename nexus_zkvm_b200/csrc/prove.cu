@@ -21,7 +21,8 @@ struct nb200_air {
   std::vector<nb::JitKernel> jit;        // constraint program (D1 and whole domains)
   std::vector<nb::JitKernel> jit_d2;     // its constraints of degree above AIR_LOW_DEGREE (D2 of the half-domain route)
   std::vector<nb::JitKernel> jit_logup;  // logup (interaction trace) program
-  ~nb200_air() { for (auto* v : {&jit, &jit_d2, &jit_logup}) for (auto& j : *v) nb::jit_release(j); }
+  std::vector<nb::JitKernel> jit_check;  // constraint check on the trace domain (nb200_check_constraints)
+  ~nb200_air() { for (auto* v : {&jit, &jit_d2, &jit_logup, &jit_check}) for (auto& j : *v) nb::jit_release(j); }
 };
 
 namespace nb {
@@ -77,10 +78,11 @@ static nb200_status upload_params(nb200_ctx* ctx, const void* params, size_t n_p
 
 // The component's specialised kernel, compiled on first use; nullptr = none.
 // `interp_fallback`: the caller can run the bytecode interpreter, so programs shorter than JIT_MIN_INSTR are not compiled and a failed
-// compile is only logged (NB200_TRACE).  The sharded row kernels have no interpreter: they try every program and reject a nullptr.
-enum JitKind { JIT_CONSTRAINTS, JIT_D2, JIT_LOGUP };
+// compile is only logged (NB200_TRACE).  The sharded row kernels and the constraint check have no interpreter: they try every program and
+// reject a nullptr.
+enum JitKind { JIT_CONSTRAINTS, JIT_D2, JIT_LOGUP, JIT_CHECK };
 static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp_idx, JitKind kind, bool interp_fallback) {
-  std::vector<JitKernel>& v = kind == JIT_LOGUP ? air_h->jit_logup : kind == JIT_D2 ? air_h->jit_d2 : air_h->jit;
+  std::vector<JitKernel>& v = kind == JIT_CHECK ? air_h->jit_check : kind == JIT_LOGUP ? air_h->jit_logup : kind == JIT_D2 ? air_h->jit_d2 : air_h->jit;
   if (v.size() != air_h->prog.comps.size()) v.resize(air_h->prog.comps.size());
   JitKernel& jk = v[comp_idx];
   if (!jk.tried) {
@@ -88,9 +90,11 @@ static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp
     const AirComponent& c = air_h->prog.comps[comp_idx];
     const bool worth_it = kind == JIT_LOGUP ? (c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0) : c.prog.size() >= JIT_MIN_INSTR;
     if ((worth_it || !interp_fallback) && jit_enabled()) {
-      nb200_status st = kind == JIT_LOGUP ? jit_compile_logup(ctx, c, &jk) : jit_compile_constraints(ctx, c, kind == JIT_D2, &jk);
+      nb200_status st = kind == JIT_CHECK ? jit_compile_check(ctx, c, &jk)
+                      : kind == JIT_LOGUP ? jit_compile_logup(ctx, c, &jk) : jit_compile_constraints(ctx, c, kind == JIT_D2, &jk);
+      if (st != NB200_OK) jk.err = ctx->err;   // kept with the kernel: a later call that finds it missing reports why
       if (interp_fallback) {
-        static const char* what[] = {"component", "component (D2)", "logup program"};
+        static const char* what[] = {"component", "component (D2)", "logup program", "constraint check"};
         if (st != NB200_OK && ctx->trace) fprintf(stderr, "[nb200] jit unavailable for %s: %s\n", what[kind], ctx->err.c_str());
         trace_mark(ctx, kind == JIT_LOGUP ? "jit: compile logup (one-time)" : "jit: compile (one-time)");
       }
@@ -1175,6 +1179,56 @@ nb200_status gen_interaction(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, con
   return NB200_OK;
 }
 
+// assert_constraints_on_polys for one component on the GPU: every constraint evaluated on every row of its trace domain, from the trace
+// evaluations of the three committed trees (the caller's batches, commitment order).  Per constraint: the number of rows where it does not
+// hold and the first of them in coset order (UINT64_MAX: none).
+nb200_status check_constraints(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, const nb200_cols* const* const trees[3], const size_t n_trees[3],
+                               const u32* params, size_t n_params, uint64_t* n_failing, uint64_t* first_row, size_t n) {
+  const AirProgram& air = air_h->prog;
+  NB_ARG(ctx, comp_idx < air.comps.size(), "check_constraints: component index");
+  const AirComponent& c = air.comps[comp_idx];
+  NB_ARG(ctx, n == c.n_constraints, "check_constraints: n must be the component's constraint count");
+  NB_ARG(ctx, n_params == air.n_params, "check_constraints: parameter table size");
+  if (n == 0) return NB200_OK;   // nothing to check: an empty report
+  std::vector<std::vector<const u32*>> flat(3);
+  std::vector<std::vector<u32>> flog(3);
+  for (int t = 0; t < 3; ++t)
+    for (size_t b = 0; b < n_trees[t]; ++b) {
+      NB_ARG(ctx, trees[t][b], "check_constraints: null batch");
+      for (size_t k = 0; k < trees[t][b]->n_cols; ++k) { flat[t].push_back(trees[t][b]->col(k)); flog[t].push_back(trees[t][b]->log_size); }
+    }
+  std::vector<const u32*> mask_cols(c.masks.size(), nullptr);
+  for (size_t m = 0; m < c.masks.size(); ++m) {
+    const AirMask& mk = c.masks[m];
+    NB_ARG(ctx, mk.col < flat[mk.tree].size(), "check_constraints: AIR references a missing trace column");
+    NB_ARG(ctx, flog[mk.tree][mk.col] == c.log_size, "check_constraints: column size differs from the component's log_size");
+    mask_cols[m] = flat[mk.tree][mk.col];
+  }
+  const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, JIT_CHECK, false);
+  if (!jk)
+    return set_err(ctx, NB200_ERR_STATE, jit_enabled() ? "check_constraints: the constraint-check kernel could not be compiled: " + air_h->jit_check[comp_idx].err
+                                                       : std::string("check_constraints: the constraint check runs only as a generated kernel (NB200_JIT=0)"));
+  // device side: the parameter table, the column pointers (copied into the kernel's constant table) and one count + one row per constraint
+  DevBuf d_params, d_cols, d_res;
+  NB_TRY(upload_params(ctx, params, n_params, d_params));
+  NB_TRY(alloc(ctx, d_cols, std::max<size_t>(mask_cols.size(), 1) * 2));
+  if (!mask_cols.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_cols.p, mask_cols.data(), mask_cols.size() * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream));
+  NB_TRY(alloc(ctx, d_res, 2 * n));
+  NB_CUDA(ctx, cudaMemsetAsync(d_res.p, 0, n * 4, ctx->stream));
+  NB_CUDA(ctx, cudaMemsetAsync(d_res.p + n, 0xff, n * 4, ctx->stream));
+  trace_mark(ctx, nullptr);
+  NB_TRY(jit_launch_check(ctx, *jk, (const u32* const*)d_cols.p, d_params.p, d_res.p, d_res.p + n));
+  std::vector<u32> res(2 * n);
+  NB_CUDA(ctx, cudaMemcpyAsync(res.data(), d_res.p, 2 * n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // also: the host tables above have been consumed
+  trace_mark(ctx, "constraint check");
+  for (size_t k = 0; k < n; ++k) {
+    n_failing[k] = res[k];
+    first_row[k] = res[n + k] == 0xffffffffu ? UINT64_MAX : (uint64_t)res[n + k];
+  }
+  return NB200_OK;
+}
+
 // LogupTraceGenerator of the sharded (main) component: this rank runs the row kernel on ITS trace rows (all columns: the row slices kept by
 // nb200_scheme_commit_sharded), the last secure column is all-gathered for the global claimed sum / coset-order prefix sum (finalize_last),
 // and one rows -> columns exchange hands every rank its COLUMN shard of the 4 * n_logup interaction columns, ready for the next sharded commit.
@@ -1288,6 +1342,9 @@ void nb200_air_free(nb200_air* a) { delete a; }
 uint32_t nb200_air_n_params(const nb200_air* a) { return a ? a->prog.n_params : 0; }
 uint32_t nb200_air_n_components(const nb200_air* a) { return a ? (uint32_t)a->prog.comps.size() : 0; }
 uint64_t nb200_kernel_source_key(const char* src) { return src ? jit_source_key(src) : 0; }
+uint32_t nb200_air_n_constraints(const nb200_air* a, uint32_t component) {
+  return a && component < a->prog.comps.size() ? a->prog.comps[component].n_constraints : 0;
+}
 nb200_status nb200_air_constraint_degrees(const nb200_air* a, uint32_t component, uint32_t* degrees, size_t n) {
   if (!a || component >= a->prog.comps.size() || (n && !degrees)) return NB200_ERR_ARG;
   const std::vector<u32> d = constraint_degrees(a->prog.comps[component]);
@@ -1304,12 +1361,13 @@ nb200_status nb200_air_d2_masks(const nb200_air* a, uint32_t component, uint8_t*
   return NB200_OK;
 }
 nb200_status nb200_air_kernel_source(const nb200_air* a, uint32_t component, int which, char** out) {
-  if (!a || !out || component >= a->prog.comps.size() || which < 0 || which > 2) return NB200_ERR_ARG;
+  if (!a || !out || component >= a->prog.comps.size() || which < 0 || which > 3) return NB200_ERR_ARG;
   const AirComponent& c = a->prog.comps[component];
   *out = nullptr;
-  if ((which == 1 ? c.logup_prog.size() : c.prog.size()) < JIT_MIN_INSTR || (which == 1 && c.n_logup_cols() == 0)) return NB200_ERR_STATE;  // runs on the interpreter
+  if (which == 3 && c.n_constraints == 0) return NB200_ERR_STATE;   // nothing to check (the check has no interpreter: any length is compiled)
+  if (which != 3 && ((which == 1 ? c.logup_prog.size() : c.prog.size()) < JIT_MIN_INSTR || (which == 1 && c.n_logup_cols() == 0))) return NB200_ERR_STATE;  // runs on the interpreter
   if (which == 2 && count_high(high_constraints(c)) == 0) return NB200_ERR_STATE;   // nothing to evaluate on D2
-  std::string src = which == 1 ? jit_logup_source(c) : jit_source(c, which == 2);
+  std::string src = which == 3 ? jit_check_source(c) : which == 1 ? jit_logup_source(c) : jit_source(c, which == 2);
   char* o = (char*)malloc(src.size() + 1);
   if (!o) return NB200_ERR_OOM;
   memcpy(o, src.c_str(), src.size() + 1);
@@ -1380,6 +1438,14 @@ nb200_status nb200_prove(nb200_scheme* s, const nb200_air* air, const uint32_t* 
   memcpy(o, bytes.data(), bytes.size());
   *proof_out = o; *proof_len = bytes.size();
   return NB200_OK;
+}
+nb200_status nb200_check_constraints(nb200_ctx* ctx, const nb200_air* air, uint32_t component, const nb200_cols* const* tree0, size_t n0,
+                                     const nb200_cols* const* tree1, size_t n1, const nb200_cols* const* tree2, size_t n2, const uint32_t* params,
+                                     size_t n_params, uint64_t* n_failing, uint64_t* first_row, size_t n) {
+  if (!ctx || !air || (n0 && !tree0) || (n1 && !tree1) || (n2 && !tree2) || (n_params && !params) || (n && (!n_failing || !first_row))) return NB200_ERR_ARG;
+  const nb200_cols* const* trees[3] = {tree0, tree1, tree2};
+  const size_t n_trees[3] = {n0, n1, n2};
+  return check_constraints(ctx, const_cast<nb200_air*>(air), component, trees, n_trees, params, n_params, n_failing, first_row, n);
 }
 
 // ---- backend-trait level operations (the per-trait surface a `CudaBackend` shim binds; the coarse nb200_prove runs the same code) ----

@@ -146,6 +146,24 @@ def prove(machine, backend, main_cols, mult, config=None, associated_data=b"", r
     """The Machine::prove sequence (machine.rs:130-297) over `backend`.  Returns (proof_bytes, claimed_sums, aux).
     `resident` = (tree0 device batches, tree1 device batches) commits evaluations that are already on the device (finalized
     order) instead of uploading `main_cols` — the HBM-resident variant bench.py's `value` times."""
+    ch, prover, params, claimed, roots, log_sizes = _commit_trees(machine, backend, main_cols, mult, config, associated_data, resident)
+    aux = {"channel_at_prove": ch.clone(), "params": params, "roots": roots, "log_sizes": log_sizes,
+           "associated_data": bytes(associated_data)}
+    proof = prover.prove(ch, params)
+    return proof, claimed, aux
+
+
+def check_constraints(machine, backend, main_cols, mult, associated_data=b""):
+    """assert_constraints_on_polys for every component (the reference's `assert_chip` / `assert_component`) on the GPU: the trees are committed
+    as `prove` commits them, then each component's constraints are evaluated on every row of its trace domain.  Returns
+    ({component: [(constraint, degree, failing rows, first failing row in trace order)]}, whether the claimed LogUp sums cancel)."""
+    _ch, prover, params, claimed, _roots, _ls = _commit_trees(machine, backend, main_cols, mult, None, associated_data, None)
+    report = {k: prover.check_constraints(k, params) for k in range(len(machine.air.components))}
+    return report, verify_claimed_sums(claimed)
+
+
+def _commit_trees(machine, backend, main_cols, mult, config, associated_data, resident):
+    """Machine::prove up to and including the tree-2 commit: (channel, prover, params, claimed sums, roots, log sizes)."""
     config = config or dict(pow_bits=5, log_blowup=1, log_last=0, n_queries=3)
     air = machine.air
     ch = backend.channel()
@@ -177,10 +195,7 @@ def prove(machine, backend, main_cols, mult, config=None, associated_data=b"", r
         params[comp.cumsum_shift_param] = F.qm31_mul_m31(cs, inv_n)
     ch.mix_felts(claimed)
     roots.append(prover.commit_interaction(inter, ch))
-    aux = {"channel_at_prove": ch.clone(), "params": params, "roots": roots, "log_sizes": log_sizes,
-           "associated_data": bytes(associated_data)}
-    proof = prover.prove(ch, params)
-    return proof, claimed, aux
+    return ch, prover, params, claimed, roots, log_sizes
 
 
 def shard_host_tree(machine, prover, host_cols, rank, world):

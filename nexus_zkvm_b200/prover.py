@@ -213,6 +213,25 @@ class CommitmentSchemeProver:
         self.ctx._chk(lib().nb200_constraint_quotients(self._h, self.air._h, C.c_uint32(comp), p.ctypes.data_as(u32p), C.c_size_t(p.shape[0]),
                                                        cf.ctypes.data_as(u32p), C.c_size_t(cf.shape[0]), accum._h))
 
+    def check_constraints(self, comp, params):
+        """assert_constraints_on_polys for component `comp` on the GPU (nb200_check_constraints), over the three committed trees' batches.
+        Returns the failing constraints as [(constraint index, degree, failing rows, first failing row in trace order)]."""
+        p = np.ascontiguousarray(np.array(params, dtype=np.uint32).reshape(-1, 4))
+        trees = [(C.c_void_p * max(len(t), 1))(*[b._h for b in t]) for t in self.tree_evals[:3]]
+        assert len(trees) == 3, "commit the three trees first"
+        lib().nb200_air_n_constraints.restype = C.c_uint32
+        n_constraints = int(lib().nb200_air_n_constraints(self.air._h, C.c_uint32(comp)))
+        deg = np.zeros(max(n_constraints, 1), np.uint32)
+        self.ctx._chk(lib().nb200_air_constraint_degrees(self.air._h, C.c_uint32(comp), deg.ctypes.data_as(u32p), C.c_size_t(n_constraints)))
+        n_failing = np.zeros(max(n_constraints, 1), np.uint64)
+        first_row = np.zeros(max(n_constraints, 1), np.uint64)
+        u64p = C.POINTER(C.c_uint64)
+        self.ctx._chk(lib().nb200_check_constraints(self.ctx._h, self.air._h, C.c_uint32(comp),
+                                                    trees[0], C.c_size_t(len(self.tree_evals[0])), trees[1], C.c_size_t(len(self.tree_evals[1])),
+                                                    trees[2], C.c_size_t(len(self.tree_evals[2])), p.ctypes.data_as(u32p), C.c_size_t(p.shape[0]),
+                                                    n_failing.ctypes.data_as(u64p), first_row.ctypes.data_as(u64p), C.c_size_t(n_constraints)))
+        return [(k, int(deg[k]), int(n_failing[k]), int(first_row[k])) for k in range(n_constraints) if n_failing[k]]
+
     def prove(self, ch, params):
         p = np.ascontiguousarray(np.array(params, dtype=np.uint32).reshape(-1, 4))
         out = u8p(); ln = C.c_size_t()

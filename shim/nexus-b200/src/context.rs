@@ -123,6 +123,18 @@ impl Context {
                                                         p.as_ptr(), params.len(), &mut out, cs.as_mut_ptr()) })?;
         Ok((Columns { ctx: self.clone(), h: out }, words_to_secure(&cs)))
     }
+    /// `assert_constraints_on_polys` of one component on the device: for every constraint that fails somewhere,
+    /// `(constraint index, failing rows, first failing row in trace order)`.  An empty vector: every constraint holds on every row.
+    pub fn check_constraints(&self, air: &Air, component: u32, tree0: &[&Columns], tree1: &[&Columns], tree2: &[&Columns], params: &[SecureField])
+        -> Result<Vec<(usize, u64, u64)>> {
+        let t: Vec<Vec<*const nb200_cols>> = [tree0, tree1, tree2].iter().map(|tr| tr.iter().map(|c| c.h as *const _).collect()).collect();
+        let n = unsafe { nb200_air_n_constraints(air.h, component) } as usize;
+        let p = secure_to_words(params);
+        let (mut failing, mut first) = (vec![0u64; n], vec![0u64; n]);
+        self.check(unsafe { nb200_check_constraints(self.raw(), air.h, component, t[0].as_ptr(), t[0].len(), t[1].as_ptr(), t[1].len(),
+                                                    t[2].as_ptr(), t[2].len(), p.as_ptr(), params.len(), failing.as_mut_ptr(), first.as_mut_ptr(), n) })?;
+        Ok((0..n).filter(|&k| failing[k] != 0).map(|k| (k, failing[k], first[k])).collect())
+    }
 }
 
 /// `PcsConfig { pow_bits, fri_config: FriConfig { log_blowup_factor, log_last_layer_degree_bound, n_queries } }`

@@ -102,6 +102,7 @@ extern "C" {
     pub fn nb200_air_free(air: *mut nb200_air);
     pub fn nb200_air_n_params(air: *const nb200_air) -> u32;
     pub fn nb200_air_n_components(air: *const nb200_air) -> u32;
+    pub fn nb200_air_n_constraints(air: *const nb200_air, component: u32) -> u32;
     pub fn nb200_air_kernel_source(air: *const nb200_air, component: u32, which: c_int, out: *mut *mut c_char) -> c_int;
     pub fn nb200_kernel_source_key(source: *const c_char) -> u64;
     pub fn nb200_air_constraint_degrees(air: *const nb200_air, component: u32, degrees: *mut u32, n: usize) -> c_int;
@@ -122,6 +123,9 @@ extern "C" {
                                        out: *mut *mut nb200_cols, claimed_sum: *mut u32) -> c_int;
     pub fn nb200_prove(s: *mut nb200_scheme, air: *const nb200_air, params: *const u32, n_params: usize, ch: *mut nb200_channel,
                        proof_out: *mut *mut u8, proof_len: *mut usize) -> c_int;
+    pub fn nb200_check_constraints(ctx: *mut nb200_ctx, air: *const nb200_air, component: u32, tree0: *const *const nb200_cols, n0: usize,
+                                   tree1: *const *const nb200_cols, n1: usize, tree2: *const *const nb200_cols, n2: usize,
+                                   params: *const u32, n_params: usize, n_failing: *mut u64, first_row: *mut u64, n: usize) -> c_int;
     // ---- backend-trait level operations
     pub fn nb200_constraint_quotients(s: *mut nb200_scheme, air: *const nb200_air, component: u32, params: *const u32, n_params: usize,
                                       coeffs: *const u32, n_coeffs: usize, accum: *mut nb200_cols) -> c_int;
