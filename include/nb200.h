@@ -284,6 +284,17 @@ nb200_status nb200_gen_interaction_trace_sharded(nb200_scheme*, const nb200_air*
  * coeffs = n_coeffs QM31 (= the component's n_constraints random-coefficient powers, first constraint first). */
 nb200_status nb200_constraint_quotients(nb200_scheme*, const nb200_air*, uint32_t component, const uint32_t* params, size_t n_params,
                                         const uint32_t* coeffs, size_t n_coeffs, nb200_cols* accum);
+/* The half-domain route nb200_prove takes (Q_HALF) for a component with log_expand = log_blowup + 1 whose LDE has more than 2^8 rows: ADDs
+ * into three accumulators of 4 columns x 2^lde_log each (lde_log = log_size + log_blowup):
+ *   q_d1      = every constraint's quotient on the committed LDE domain D1 = CanonicCoset(lde_log).circle_domain();
+ *   q_high_d2 = the quotient of the constraints of degree > 2 alone on D2 = rows [0, 2^lde_log) of CanonicCoset(lde_log + 1).circle_domain()
+ *               (bit-reversed);
+ *   q_high_d1 = the same on D1.
+ * Where the bytecode interpreter evaluates the component instead of the generated kernels (NB200_JIT=0, or an LDE of fewer than 2^10 rows)
+ * every constraint counts as a high one: q_high_d2 and q_high_d1 then hold q itself.
+ * NB200_ERR_ARG for a component that nb200_prove evaluates with Q_FULL (nb200_constraint_quotients). */
+nb200_status nb200_constraint_quotients_half(nb200_scheme*, const nb200_air*, uint32_t component, const uint32_t* params, size_t n_params,
+                                             const uint32_t* coeffs, size_t n_coeffs, nb200_cols* q_d1, nb200_cols* q_high_d2, nb200_cols* q_high_d1);
 /* AccumulationOps::accumulate: a += b (element-wise, M31), same shapes */
 nb200_status nb200_accumulate(nb200_ctx*, nb200_cols* a, const nb200_cols* b);
 /* QuotientOps::accumulate_quotients (DEEP quotients) on CanonicCoset(log_size).circle_domain(): columns are numbered

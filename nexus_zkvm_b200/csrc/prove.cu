@@ -1519,5 +1519,20 @@ nb200_status nb200_constraint_quotients(nb200_scheme* s, const nb200_air* air, u
   NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return NB200_OK;
 }
+nb200_status nb200_constraint_quotients_half(nb200_scheme* s, const nb200_air* air, uint32_t component, const uint32_t* params, size_t n_params,
+                                             const uint32_t* coeffs, size_t n_coeffs, nb200_cols* q_d1, nb200_cols* q_high_d2, nb200_cols* q_high_d1) {
+  if (!s || !air || !q_d1 || !q_high_d2 || !q_high_d1 || (!coeffs && n_coeffs)) return NB200_ERR_ARG;
+  nb200_ctx* ctx = s->ctx;
+  NB_ARG(ctx, component < air->prog.comps.size(), "constraint quotients: component index");
+  NB_ARG(ctx, quotient_mode(s, air->prog.comps[component]) == Q_HALF, "constraint quotients (half domains): nb200_prove evaluates this component with Q_FULL");
+  NB_ARG(ctx, n_params == air->prog.n_params, "constraint quotients: parameter table size");
+  std::vector<qm31> cf(n_coeffs);
+  if (n_coeffs) memcpy(cf.data(), coeffs, n_coeffs * 16);
+  DevBuf d_params;
+  NB_TRY(upload_params(ctx, params, n_params, d_params));
+  NB_TRY(component_quotients(s, const_cast<nb200_air*>(air), component, d_params.p, cf, Q_HALF, q_d1, q_high_d2, q_high_d1));
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  return NB200_OK;
+}
 
 }  // extern "C"

@@ -213,6 +213,16 @@ class CommitmentSchemeProver:
         self.ctx._chk(lib().nb200_constraint_quotients(self._h, self.air._h, C.c_uint32(comp), p.ctypes.data_as(u32p), C.c_size_t(p.shape[0]),
                                                        cf.ctypes.data_as(u32p), C.c_size_t(cf.shape[0]), accum._h))
 
+    def constraint_quotients_half(self, comp, params, coeffs, q_d1, q_high_d2, q_high_d1):
+        """The half-domain route prove takes for a degree-4 component (nb200_constraint_quotients_half): q_d1 += every constraint's quotient on
+        the committed LDE domain, q_high_d2 / q_high_d1 += the degree > 2 constraints' quotient on the first half of the next larger canonic domain
+        and on the LDE domain; each a 4-column batch of the LDE size.  Where the bytecode interpreter evaluates the component (NB200_JIT=0, an LDE
+        of fewer than 2^10 rows) every constraint counts as a high one."""
+        p = np.ascontiguousarray(np.array(params, dtype=np.uint32).reshape(-1, 4))
+        cf = np.ascontiguousarray(np.array(coeffs, dtype=np.uint32).reshape(-1, 4))
+        self.ctx._chk(lib().nb200_constraint_quotients_half(self._h, self.air._h, C.c_uint32(comp), p.ctypes.data_as(u32p), C.c_size_t(p.shape[0]),
+                                                            cf.ctypes.data_as(u32p), C.c_size_t(cf.shape[0]), q_d1._h, q_high_d2._h, q_high_d1._h))
+
     def check_constraints(self, comp, params):
         """assert_constraints_on_polys for component `comp` on the GPU (nb200_check_constraints), over the three committed trees' batches.
         Returns the failing constraints as [(constraint index, degree, failing rows, first failing row in trace order)]."""

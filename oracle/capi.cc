@@ -356,17 +356,20 @@ uint64_t orc_grind(const uint8_t digest[32], uint32_t pow_bits) {
   return grind(ch, pow_bits);
 }
 
-// ComponentProver::evaluate_constraint_quotients_on_domain for component `comp` over the prover's committed trees:
+// ComponentProver::evaluate_constraint_quotients_on_domain for component `comp` over the prover's committed trees, on
+// CanonicCoset(eval_log).circle_domain() (eval_log = 0: the component's own, log_size + log_expand; any eval_log > log_size):
 // accum (4 coordinate columns of 2^eval_log, in/out) += quotients
-int orc_prover_constraint_quotients(void* pp, uint32_t comp, const uint32_t* params, size_t n_params, const uint32_t* coeffs /*4 per constraint*/, uint32_t* accum) {
+int orc_prover_constraint_quotients(void* pp, uint32_t comp, uint32_t eval_log, const uint32_t* params, size_t n_params, const uint32_t* coeffs /*4 per constraint*/,
+                                    uint32_t* accum) {
   try {
     OrcProver* p = (OrcProver*)pp;
     const Component& c = p->air.comps.at(comp);
-    size_t en = (size_t)1 << c.eval_log();
+    if (eval_log == 0) eval_log = c.eval_log();
+    size_t en = (size_t)1 << eval_log;
     SecureCol acc = read_secure(accum, en);
     std::vector<QM31> coeff(c.n_constraints);
     for (uint32_t k = 0; k < c.n_constraints; ++k) coeff[k] = read_q(coeffs + 4 * k);
-    component_quotients(c, p->trees, read_params(params, n_params), coeff, acc);
+    component_quotients(c, p->trees, read_params(params, n_params), coeff, acc, eval_log);
     write_secure(acc, accum);
     return 0;
   } catch (std::exception& e) { g_err = e.what(); return 1; }

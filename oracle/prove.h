@@ -257,9 +257,12 @@ inline std::pair<std::vector<Col>, QM31> gen_interaction_trace(const Component& 
 inline std::vector<QM31> secure_powers(QM31 x, size_t n) { std::vector<QM31> p(n); QM31 a = QM31::one(); for (size_t i = 0; i < n; ++i) { p[i] = a; a = a * x; } return p; }
 
 // ComponentProver::evaluate_constraint_quotients_on_domain for one component: acc[row] += (sum_k coeff[k] * constraint_k(row)) / vanishing(row)
-// on CanonicCoset(eval_log).circle_domain() (bit-reversed); `coeff` are the random-coefficient powers assigned to this component.
-inline void component_quotients(const Component& c, const std::vector<Tree>& trees, const std::vector<QM31>& params, const std::vector<QM31>& coeff, SecureCol& acc) {
-  uint32_t elog = c.eval_log();
+// on CanonicCoset(elog).circle_domain() (bit-reversed); `coeff` are the random-coefficient powers assigned to this component.  elog = 0 means the
+// component's own eval_log (the prover's domain); any elog > log_size gives the same quotient polynomial on another domain.
+inline void component_quotients(const Component& c, const std::vector<Tree>& trees, const std::vector<QM31>& params, const std::vector<QM31>& coeff, SecureCol& acc,
+                                uint32_t elog = 0) {
+  if (elog == 0) elog = c.eval_log();
+  if (elog <= c.log_size) throw std::runtime_error("constraint quotients: the evaluation domain must be larger than the trace domain");
   size_t en = (size_t)1 << elog;
   CircleDomain eval_domain = CanonicCoset(elog).circle_domain();
   // evaluate every referenced column on the eval domain
@@ -272,7 +275,7 @@ inline void component_quotients(const Component& c, const std::vector<Tree>& tre
   for (size_t m = 0; m < c.masks.size(); ++m) mcol[m] = &ext[{c.masks[m].tree, c.masks[m].col}];
   // denominators: coset_vanishing(trace coset, eval_domain.at(i)) for i < 2^log_expand, bit reversed, inverted
   Coset trace_coset = CanonicCoset(c.log_size).coset;
-  std::vector<M31> dinv((size_t)1 << c.log_expand);
+  std::vector<M31> dinv((size_t)1 << (elog - c.log_size));
   for (size_t i = 0; i < dinv.size(); ++i) dinv[i] = inv(coset_vanishing<M31>(trace_coset, eval_domain.at(i)));
   bit_reverse(dinv);
 #pragma omp parallel

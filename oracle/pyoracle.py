@@ -258,6 +258,23 @@ class OracleError(RuntimeError):
     pass
 
 
+def _component_eval_log(words, comp):
+    """log_size + log_expand of component `comp`, read from the AIR bytecode (layout: nexus_zkvm_b200/air.py)."""
+    w = [int(x) for x in words]
+    i = 4
+    for k in range(w[3]):
+        if k == comp:
+            return w[i] + w[i + 1]
+        i += 3
+        i += 1 + 3 * w[i] + 2            # masks, register counts
+        i += 1 + 4 * w[i]                # constraint program
+        n_fracs = w[i]
+        i += 3
+        i += 1 + 4 * w[i]                # logup program
+        i += n_fracs + 2
+    raise IndexError(comp)
+
+
 class Prover:
     """Oracle restatement of CommitmentSchemeProver + stwo::prover::prove over a bytecode AIR."""
 
@@ -306,12 +323,18 @@ class Prover:
         return bytes(buf[:ln.value])
 
     def constraint_quotients(self, comp, eval_log, params, coeffs, accum=None):
-        """ComponentProver::evaluate_constraint_quotients_on_domain for one component; returns accum (4 x 2^eval_log) + quotients."""
+        """ComponentProver::evaluate_constraint_quotients_on_domain for one component on CanonicCoset(eval_log).circle_domain(); returns
+        accum (4 x 2^eval_log) + quotients.  eval_log=None is the component's own domain (log_size + log_expand, where the prover evaluates);
+        any eval_log > log_size gives the same quotient polynomial elsewhere, e.g. on the committed LDE domain."""
         params = np.ascontiguousarray(params, dtype=np.uint32).reshape(-1, 4)
         coeffs = np.ascontiguousarray(coeffs, dtype=np.uint32).reshape(-1, 4)
+        if eval_log is None:
+            eval_log = _component_eval_log(self.air_words, comp)
         acc = np.zeros((4, 1 << eval_log), np.uint32) if accum is None else np.ascontiguousarray(accum, dtype=np.uint32).copy()
-        st = lib().orc_prover_constraint_quotients(self._h, C.c_uint32(comp), params.ctypes.data_as(u32p), C.c_size_t(params.shape[0]),
-                                                   coeffs.ctypes.data_as(u32p), acc.ctypes.data_as(u32p))
+        if acc.shape != (4, 1 << eval_log):
+            raise OracleError(f"constraint quotients: accumulator shape {acc.shape}, want (4, {1 << eval_log})")
+        st = lib().orc_prover_constraint_quotients(self._h, C.c_uint32(comp), C.c_uint32(eval_log), params.ctypes.data_as(u32p),
+                                                   C.c_size_t(params.shape[0]), coeffs.ctypes.data_as(u32p), acc.ctypes.data_as(u32p))
         if st:
             raise OracleError(last_error())
         return acc

@@ -129,6 +129,9 @@ extern "C" {
     // ---- backend-trait level operations
     pub fn nb200_constraint_quotients(s: *mut nb200_scheme, air: *const nb200_air, component: u32, params: *const u32, n_params: usize,
                                       coeffs: *const u32, n_coeffs: usize, accum: *mut nb200_cols) -> c_int;
+    pub fn nb200_constraint_quotients_half(s: *mut nb200_scheme, air: *const nb200_air, component: u32, params: *const u32, n_params: usize,
+                                           coeffs: *const u32, n_coeffs: usize, q_d1: *mut nb200_cols, q_high_d2: *mut nb200_cols,
+                                           q_high_d1: *mut nb200_cols) -> c_int;
     pub fn nb200_accumulate(ctx: *mut nb200_ctx, a: *mut nb200_cols, b: *const nb200_cols) -> c_int;
     pub fn nb200_fri_quotients(ctx: *mut nb200_ctx, batches: *const *const nb200_cols, n_batches: usize, log_size: u32,
                                sample_batches: *const nb200_sample_batch, n_sample_batches: usize, entries: *const nb200_sample_entry, n_entries: usize,
