@@ -74,7 +74,7 @@ def build(force=False, verbose=False):
 JIT_CACHE = os.path.join(HERE, "jit_cache")
 # (log_size, n_lanes, logup_in_pairs): bench.py / tools/prove_trace.py, __graft_entry__.smoke and the machines of tests/test_gpu_*.py
 SHIPPED_MACHINES = [(20, 21, False), (22, 21, False), (16, 21, False), (8, 1, False), (8, 2, False), (8, 2, True), (8, 3, False), (9, 1, False), (9, 2, False),
-                    (9, 2, True), (10, 1, False), (12, 3, False)]
+                    (9, 2, True), (10, 1, False), (12, 3, False)] + [(ls, 1, False) for ls in range(16, 23)]   # the fused commit sizes
 
 
 # prover2-shaped machines (machine.MultiMachine) of tests/test_gpu_prove_parity.py and bench.py --multi: component log sizes
