@@ -53,13 +53,14 @@ inline void merkle_verify(const Hash32& root, const std::vector<uint32_t>& col_l
 }
 
 inline QM31 line_poly_eval(const std::vector<QM31>& coeffs_bitrev, uint32_t log_size, QM31 x) {
-  // LinePoly::eval_at_point: fold(coeffs, [x, pi(x), ...]) with the first factor applied to the top split
+  // LinePoly::eval_at_point: fold(coeffs, [x, pi(x), ...]) with the first factor applied to the top split.  Unlike CirclePoly::eval_at_point
+  // there is no reversal: the coefficients are stored bit-reversed, so the top split of the stored order is bit 0 of the ordered one (x).
+  // A reversal here is invisible while the last layer has at most two coefficients (log_last_layer_degree_bound <= 1).
   std::vector<QM31> d; for (uint32_t i = 0; i < log_size; ++i) { d.push_back(x); x = double_x(x); }
   std::function<QM31(const QM31*, size_t, const QM31*)> rec = [&](const QM31* v, size_t n, const QM31* f) -> QM31 {
     if (n == 1) return v[0];
     return rec(v, n / 2, f + 1) + rec(v + n / 2, n / 2, f + 1) * f[0];
   };
-  std::reverse(d.begin(), d.end());  // fold() consumes factors from the highest doubling first (as eval_at_point's `mappings.reverse()`)
   return rec(coeffs_bitrev.data(), coeffs_bitrev.size(), d.data());
 }
 

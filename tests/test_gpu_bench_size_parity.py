@@ -133,9 +133,9 @@ def test_commit_host_packed_bytes_at_bench_size(ctx):
 
 
 def test_proof_bytes_of_the_bench_machine(ctx):
-    """(c) AddMachine(n_lanes=21) — 3 / 339 / 1012 columns, the machine bench.py proves, with its shipped generated constraint and
-    logup kernels (jit_cache) — proof bytes equal the oracle's at 2^16 rows (the oracle needs ~30 s here; 2^20 takes minutes and is
-    bench.py's `--impl reference` leg)."""
+    """(c) AddMachine(n_lanes=21) — 3 / 339 / 1012 columns, the machine of `bench.py --machine add21`, with its shipped generated
+    constraint and logup kernels (jit_cache) — proof bytes equal the oracle's at 2^16 rows (the oracle needs ~30 s here).  bench.py's
+    default machine, NexusV1Machine, is compared on proof bytes in tests/test_gpu_opening_at_scale.py."""
     be = CudaBackend(ctx)
     m = M.AddMachine(log_size=16, n_lanes=21)
     cols, mult = m.fill_main_trace(seed=21, n_padding=1000)

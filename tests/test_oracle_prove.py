@@ -46,6 +46,16 @@ def test_tampered_proof_rejected(proved):
     assert rejected == 12
 
 
+@pytest.mark.parametrize("log_last", [0, 1, 2, 3])
+def test_proof_with_a_larger_last_fri_layer_verifies(log_last):
+    """The last FRI layer is sent as a LinePoly of 2^log_last coefficients.  From four coefficients on, its evaluation at a query depends on
+    which doubling of x multiplies which split of the coefficients; with one or two coefficients every order gives the same value."""
+    m = M.AddMachine(log_size=9, n_lanes=1)
+    cols, mult = m.fill_main_trace(seed=9)
+    proof, _claimed, aux = M.prove(m, OracleBackend(), cols, mult, config=dict(pow_bits=5, log_blowup=1, log_last=log_last, n_queries=10))
+    verify(m, proof, aux)
+
+
 def test_unsatisfied_constraint_is_reported():
     m = M.AddMachine(log_size=8, n_lanes=1)
     cols, mult = m.fill_main_trace(seed=4)
