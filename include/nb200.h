@@ -107,6 +107,12 @@ nb200_status nb200_merkle_decommit(nb200_ctx*, const nb200_tree*, const nb200_co
                                    uint32_t** queried_values, size_t* n_queried,
                                    uint8_t** hash_witness, size_t* n_hashes,
                                    uint32_t** column_witness, size_t* n_column_witness);
+/* The walk of nb200_merkle_decommit alone, on the host (no device needed): for a tree of 2^max_log leaves over columns of the given
+ * log sizes (the caller's order) and the same queries, the column values it names as n_values (column index, row, queried ? 1 : 0)
+ * triples and the hash witness as n_hashes (layer log, node) pairs, in proof order.  Outputs are malloc'ed; free with nb200_free. */
+nb200_status nb200_merkle_decommit_plan(uint32_t max_log, const uint32_t* col_log_sizes, size_t n_cols,
+                                        const uint32_t* q_log_sizes, const uint64_t* q_counts, const uint64_t* q_positions, size_t n_sizes,
+                                        uint64_t** values, size_t* n_values, uint64_t** hashes, size_t* n_hashes);
 void nb200_free(void*);
 /* Blake2sMerkleHasher::hash_node on the host: H(left || right || values) with the selected construction (0 or 1, see
  * nb200_set_flavor); left/right both NULL for leaves.  Used to combine the Merkle caps of row-sharded sub-trees that
@@ -183,6 +189,11 @@ void nb200_channel_mix_root(nb200_channel*, const uint8_t root[32]); /* Blake2sM
 void nb200_channel_draw_felt(nb200_channel*, uint32_t out[4]);
 void nb200_channel_draw_felts(nb200_channel*, size_t n, uint32_t* out);
 void nb200_channel_draw_random_bytes(nb200_channel*, uint8_t out[32]);
+/* The channel run by one device thread (what nb200_prove uses between FRI's inner layers), from the state (digest, n_sent): for each of
+ * n steps, mix the 32-byte roots[i] (skipped when roots is NULL) and draw one felt into felts_out[4 i .. 4 i + 3]; the final state is
+ * returned.  The draws honour nb200_set_flavor's draw_domain_sep. */
+nb200_status nb200_device_channel_draw(nb200_ctx*, const uint8_t digest[32], uint64_t n_sent, const uint8_t* roots, size_t n,
+                                       uint32_t* felts_out, uint8_t digest_out[32], uint64_t* n_sent_out);
 
 /* ---- AIR: FrameworkComponent<E> as data (SSA bytecode recorded from `add_constraints`, traits.rs:45-50) ---- */
 typedef struct nb200_air nb200_air;

@@ -1,6 +1,6 @@
 // C ABI of libnexus_b200.so (see include/nb200.h).  No CPU fallback anywhere: without a CUDA device
 // nb200_ctx_create fails with NB200_ERR_NO_DEVICE.
-#include "common.cuh"
+#include "pcs.h"
 #include "circle_host.h"
 #include "blake2s.cuh"
 #include <cstdlib>
@@ -12,7 +12,10 @@ void trace_mark(nb200_ctx* ctx, const char* stage) {
   if (!ctx || !ctx->trace) return;
   cudaStreamSynchronize(ctx->stream);
   double now = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-  if (stage) fprintf(stderr, "[nb200] %-28s %9.3f ms\n", stage, now - ctx->trace_t0);
+  // the wall-clock time of the mark (ns since the Unix epoch), the clock torch.profiler stamps its events with: tools/opening_timeline.py
+  // places the stage boundaries in a profile by it
+  const long long wall_ns = (long long)std::chrono::duration_cast<std::chrono::nanoseconds>(std::chrono::system_clock::now().time_since_epoch()).count();
+  if (stage) fprintf(stderr, "[nb200] %-28s %9.3f ms @%lld\n", stage, now - ctx->trace_t0, wall_ns);
   ctx->trace_t0 = now;
 }
 void fft_drop_tables(nb200_ctx* ctx);
@@ -256,6 +259,28 @@ nb200_status nb200_merkle_decommit(nb200_ctx* ctx, const nb200_tree* tree, const
   *queried_values = (uint32_t*)dup_bytes(qv.data(), qv.size() * 4); *n_queried = qv.size();
   *hash_witness = (uint8_t*)dup_bytes(hw.data(), hw.size()); *n_hashes = hw.size() / 32;
   *column_witness = (uint32_t*)dup_bytes(cw.data(), cw.size() * 4); *n_column_witness = cw.size();
+  return NB200_OK;
+}
+nb200_status nb200_merkle_decommit_plan(uint32_t max_log, const uint32_t* col_log_sizes, size_t n_cols,
+                                        const uint32_t* q_log_sizes, const uint64_t* q_counts, const uint64_t* q_positions, size_t n_sizes,
+                                        uint64_t** values, size_t* n_values, uint64_t** hashes, size_t* n_hashes) {
+  if ((n_cols && !col_log_sizes) || (n_sizes && (!q_log_sizes || !q_counts)) || !values || !n_values || !hashes || !n_hashes) return NB200_ERR_ARG;
+  std::vector<u32> logs(col_log_sizes, col_log_sizes + n_cols);
+  for (u32 l : logs) if (l > max_log) return NB200_ERR_ARG;
+  std::vector<std::pair<u32, std::vector<u64>>> queries;
+  size_t off = 0;
+  for (size_t k = 0; k < n_sizes; ++k) {
+    if (q_counts[k] && !q_positions) return NB200_ERR_ARG;
+    queries.push_back({q_log_sizes[k], std::vector<u64>(q_positions + off, q_positions + off + q_counts[k])});
+    off += q_counts[k];
+  }
+  DecommitPlan plan;
+  merkle_decommit_plan(max_log, logs, queries, plan);
+  std::vector<uint64_t> v, h;
+  for (size_t i = 0; i < plan.vals.size(); ++i) { v.push_back(plan.vals[i].first); v.push_back(plan.vals[i].second); v.push_back(plan.val_is_query[i]); }
+  for (auto& x : plan.hashes) { h.push_back(x.first); h.push_back(x.second); }
+  *values = (uint64_t*)dup_bytes(v.data(), v.size() * 8); *n_values = plan.vals.size();
+  *hashes = (uint64_t*)dup_bytes(h.data(), h.size() * 8); *n_hashes = plan.hashes.size();
   return NB200_OK;
 }
 void nb200_free(void* p) { free(p); }

@@ -185,7 +185,8 @@ nb200_status upload_transform_pipelined(nb200_ctx* ctx, const void* host, size_t
                                         u32* d_evals, u32* d_coeffs, u32* d_lde, u32* d_half_ext = nullptr, LeafSink* leaf = nullptr, u32 elem_bytes = 4);
 
 struct ColRef { const u32* d; u32 log_size; };
-nb200_status merkle_commit(nb200_ctx* ctx, const std::vector<ColRef>& cols, nb200_tree** out, nb200_tree* pre_leaf = nullptr);
+// root_to_host = false: the root stays on the device (tree->layer[0]; tree->root is not set) and nothing waits for the stream
+nb200_status merkle_commit(nb200_ctx* ctx, const std::vector<ColRef>& cols, nb200_tree** out, nb200_tree* pre_leaf = nullptr, bool root_to_host = true);
 // incremental leaf hashing while column chunks arrive from the host (merkle.cu)
 nb200_status merkle_tree_alloc(nb200_ctx* ctx, u32 max_log, nb200_tree** out);
 nb200_status merkle_leaf_absorb(nb200_ctx* ctx, nb200_tree* tree, const u32* d_cols, size_t stride, size_t n_cols, size_t cols_before, size_t total_cols, bool final);

@@ -1,7 +1,8 @@
 // Host-side Fiat-Shamir transcript: Blake2sChannel + Blake2sMerkleChannel::mix_root
 // (stwo core/channel/blake2s.rs, core/vcs/blake2_merkle.rs), as used by the reference at
 // nexus-zkvm prover/src/machine.rs:197-206,240,262 and inside stwo::prover::prove (machine.rs:286-290).
-// The channel serialises the protocol, it is not data-parallel work: it stays on the host (SURVEY.md §8 a6).
+// The channel serialises the protocol, it is not data-parallel work: it stays on the host (SURVEY.md §8 a6), except between FRI's
+// inner layers, where device_channel.cuh runs the same steps and this channel replays them.
 #pragma once
 #include "blake2s.cuh"
 #include <vector>

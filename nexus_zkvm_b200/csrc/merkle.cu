@@ -11,7 +11,7 @@
 // Kernel: one thread per node.  A warp reads 32 consecutive rows of each column (128-byte coalesced segments);
 // 16 column words form one 64-byte message block held in registers, so no transposition is ever materialised.
 // The work is integer-ALU bound (~1.2k ops per 64-byte block), not HBM bound.
-#include "common.cuh"
+#include "pcs.h"
 #include "blake2s.cuh"
 #include <algorithm>
 
@@ -174,7 +174,7 @@ __global__ void __launch_bounds__(256) merkle_tail_kernel(uint4* __restrict__ po
 
 // pre_leaf: a tree from merkle_tree_alloc whose leaf layer already holds the hashes of ALL the largest columns (merkle_leaf_absorb);
 // it is consumed (becomes *out, or is freed on failure)
-nb200_status merkle_commit(nb200_ctx* ctx, const std::vector<ColRef>& cols_in, nb200_tree** out, nb200_tree* pre_leaf) {
+nb200_status merkle_commit(nb200_ctx* ctx, const std::vector<ColRef>& cols_in, nb200_tree** out, nb200_tree* pre_leaf, bool root_to_host) {
   // stable sort by length, descending (MerkleProver::commit)
   std::vector<ColRef> cols = cols_in;
   std::stable_sort(cols.begin(), cols.end(), [](const ColRef& a, const ColRef& b) { return a.log_size > b.log_size; });
@@ -224,8 +224,13 @@ nb200_status merkle_commit(nb200_ctx* ctx, const std::vector<ColRef>& cols_in, n
     ctx->launches += 1;
   }
   e = cudaGetLastError();
-  if (e == cudaSuccess) e = cudaMemcpyAsync(tree->root, tree->layer[0], 32, cudaMemcpyDeviceToHost, ctx->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  // (without the sync, h_ptrs may go: a copy from pageable host memory has been staged by the time cudaMemcpyAsync returns)
+  if (root_to_host) {
+    if (e == cudaSuccess) e = cudaMemcpyAsync(tree->root, tree->layer[0], 32, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  } else {
+    memset(tree->root, 0, 32);
+  }
   if (d_ptrs) dfree(ctx, (void*)d_ptrs);
   if (e != cudaSuccess) { dfree(ctx, tree->d_pool); delete tree; return set_err(ctx, NB200_ERR_CUDA, std::string("merkle commit: ") + cudaGetErrorString(e)); }
   *out = tree;
@@ -269,23 +274,60 @@ nb200_status gather_hash(nb200_ctx* ctx, const std::vector<const uint8_t*>& addr
   return NB200_OK;
 }
 
-// MerkleProver::decommit (stwo prover/vcs/prover.rs): same walk as upstream; the hashes and column values it
-// names are fetched from the device with two gathers.
-nb200_status merkle_decommit(nb200_ctx* ctx, const nb200_tree* tree, const std::vector<ColRef>& cols_in,
-                             const std::vector<std::pair<u32, std::vector<u64>>>& queries,
-                             std::vector<u32>& queried_values, std::vector<uint8_t>& hash_witness, std::vector<u32>& column_witness) {
-  std::vector<ColRef> cols = cols_in;
-  std::stable_sort(cols.begin(), cols.end(), [](const ColRef& a, const ColRef& b) { return a.log_size > b.log_size; });
-  std::vector<const u32*> val_addrs;       // in visit order
-  std::vector<uint8_t> val_is_query;       // 1 -> queried_values, 0 -> column_witness
-  std::vector<const uint8_t*> hash_addrs;
+// Hashes and words from anywhere in device memory in ONE round trip: one upload of the address list, one launch, one copy back, one sync.
+// Thread i < n_hash copies the 32-byte node at hash_addrs[i]; the threads after it copy one word each.
+__global__ void gather_batch_kernel(const void* const* __restrict__ addrs, size_t n_hash, size_t n_val, uint4* __restrict__ hashes_out, u32* __restrict__ vals_out) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n_hash) {
+    const uint4* a = (const uint4*)addrs[i];
+    hashes_out[2 * i] = a[0]; hashes_out[2 * i + 1] = a[1];
+  } else if (i < n_hash + n_val) {
+    vals_out[i - n_hash] = *(const u32*)addrs[i];
+  }
+}
+
+nb200_status gather_batch(nb200_ctx* ctx, const std::vector<const uint8_t*>& hash_addrs, const std::vector<const u32*>& val_addrs, uint8_t* hashes_out, u32* vals_out) {
+  const size_t nh = hash_addrs.size(), nv = val_addrs.size(), n = nh + nv;
+  if (n == 0) return NB200_OK;
+  std::vector<const void*> addrs(n);
+  std::copy(hash_addrs.begin(), hash_addrs.end(), addrs.begin());
+  std::copy(val_addrs.begin(), val_addrs.end(), addrs.begin() + nh);
+  // one device buffer: the hashes (32 bytes each, 16-byte aligned for the vector stores), the words, then the addresses (8-byte aligned)
+  const size_t out_bytes = nh * 32 + nv * 4, a_off = (out_bytes + 7) & ~(size_t)7;
+  uint8_t* d = nullptr;
+  NB_CUDA(ctx, dmalloc(ctx, (void**)&d, a_off + n * sizeof(void*)));
+  uint8_t* d_o = d;
+  const void** d_a = (const void**)(d + a_off);
+  std::vector<uint8_t> host(out_bytes);
+  cudaError_t e = cudaMemcpyAsync(d_a, addrs.data(), n * sizeof(void*), cudaMemcpyHostToDevice, ctx->stream);
+  if (e == cudaSuccess) {
+    gather_batch_kernel<<<(u32)((n + 255) / 256), 256, 0, ctx->stream>>>(d_a, nh, nv, (uint4*)d_o, (u32*)(d_o + nh * 32));
+    ctx->launches += 1;
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(host.data(), d_o, out_bytes, cudaMemcpyDeviceToHost, ctx->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+  dfree(ctx, d);
+  if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("gather: ") + cudaGetErrorString(e));
+  if (nh) memcpy(hashes_out, host.data(), nh * 32);
+  if (nv) memcpy(vals_out, host.data() + nh * 32, nv * 4);
+  return NB200_OK;
+}
+
+// MerkleProver::decommit (stwo prover/vcs/prover.rs), the walk alone: which column values (in walk order, each marked queried or
+// witness) and which nodes of the layers below each layer (the hash witness, in order) the decommitment names.
+void merkle_decommit_plan(u32 max_log, const std::vector<u32>& col_logs, const std::vector<std::pair<u32, std::vector<u64>>>& queries, DecommitPlan& plan) {
+  plan = DecommitPlan();
+  std::vector<u32> order(col_logs.size());   // stable length-descending order of the columns, as committed
+  for (size_t i = 0; i < order.size(); ++i) order[i] = (u32)i;
+  std::stable_sort(order.begin(), order.end(), [&](u32 a, u32 b) { return col_logs[a] > col_logs[b]; });
   size_t ci = 0;
   std::vector<u64> last_layer_queries;
-  for (int l = (int)tree->max_log; l >= 0; --l) {
+  for (int l = (int)max_log; l >= 0; --l) {
     std::vector<u64> layer_total;
     size_t first = ci;
-    while (ci < cols.size() && cols[ci].log_size == (u32)l) ++ci;
-    const uint8_t* prev_hashes = ((u32)l < tree->max_log) ? tree->layer[l + 1] : nullptr;
+    while (ci < order.size() && col_logs[order[ci]] == (u32)l) ++ci;
+    const bool has_prev = (u32)l < max_log;
     const std::vector<u64>* lq = nullptr;
     for (auto& q : queries) if (q.first == (u32)l) lq = &q.second;
     size_t pq = 0, cq = 0;
@@ -297,25 +339,51 @@ nb200_status merkle_decommit(nb200_ctx* ctx, const nb200_tree* tree, const std::
       if (has_p && has_c) node = std::min(last_layer_queries[pq] / 2, (*lq)[cq]);
       else if (has_p) node = last_layer_queries[pq] / 2;
       else node = (*lq)[cq];
-      if (prev_hashes) {
+      if (has_prev) {
         if (pq < last_layer_queries.size() && last_layer_queries[pq] == 2 * node) ++pq;
-        else hash_addrs.push_back(prev_hashes + 32 * (2 * node));
+        else plan.hashes.push_back({(u32)l + 1, 2 * node});
         if (pq < last_layer_queries.size() && last_layer_queries[pq] == 2 * node + 1) ++pq;
-        else hash_addrs.push_back(prev_hashes + 32 * (2 * node + 1));
+        else plan.hashes.push_back({(u32)l + 1, 2 * node + 1});
       }
       bool queried = cq < nlq && (*lq)[cq] == node;
       if (queried) ++cq;
-      for (size_t c = first; c < ci; ++c) { val_addrs.push_back(cols[c].d + node); val_is_query.push_back(queried ? 1 : 0); }
+      for (size_t c = first; c < ci; ++c) { plan.vals.push_back({order[c], node}); plan.val_is_query.push_back(queried ? 1 : 0); }
       layer_total.push_back(node);
     }
     last_layer_queries.swap(layer_total);
   }
-  std::vector<u32> vals(val_addrs.size());
-  NB_TRY(gather_u32(ctx, val_addrs, vals.data()));
-  hash_witness.resize(hash_addrs.size() * 32);
-  NB_TRY(gather_hash(ctx, hash_addrs, hash_witness.data()));
+}
+
+// the device addresses a plan names in `tree` and `cols` (the caller's column order), appended to the two lists
+void merkle_decommit_addrs(const DecommitPlan& plan, const nb200_tree* tree, const std::vector<ColRef>& cols,
+                           std::vector<const uint8_t*>& hash_addrs, std::vector<const u32*>& val_addrs) {
+  for (auto& h : plan.hashes) hash_addrs.push_back(tree->layer[h.first] + 32 * h.second);
+  for (auto& v : plan.vals) val_addrs.push_back(cols[v.first].d + v.second);
+}
+
+// the gathered hashes and words of one plan, in its order, sorted into the decommitment's three lists
+void merkle_decommit_fill(const DecommitPlan& plan, const uint8_t* hashes, const u32* vals,
+                          std::vector<u32>& queried_values, std::vector<uint8_t>& hash_witness, std::vector<u32>& column_witness) {
+  hash_witness.assign(hashes, hashes + plan.hashes.size() * 32);
   queried_values.clear(); column_witness.clear();
-  for (size_t i = 0; i < vals.size(); ++i) (val_is_query[i] ? queried_values : column_witness).push_back(vals[i]);
+  for (size_t i = 0; i < plan.vals.size(); ++i) (plan.val_is_query[i] ? queried_values : column_witness).push_back(vals[i]);
+}
+
+// MerkleProver::decommit of one tree: plan, one gather, fill
+nb200_status merkle_decommit(nb200_ctx* ctx, const nb200_tree* tree, const std::vector<ColRef>& cols,
+                             const std::vector<std::pair<u32, std::vector<u64>>>& queries,
+                             std::vector<u32>& queried_values, std::vector<uint8_t>& hash_witness, std::vector<u32>& column_witness) {
+  std::vector<u32> logs(cols.size());
+  for (size_t i = 0; i < cols.size(); ++i) logs[i] = cols[i].log_size;
+  DecommitPlan plan;
+  merkle_decommit_plan(tree->max_log, logs, queries, plan);
+  std::vector<const uint8_t*> ha;
+  std::vector<const u32*> va;
+  merkle_decommit_addrs(plan, tree, cols, ha, va);
+  std::vector<uint8_t> hashes(ha.size() * 32);
+  std::vector<u32> vals(va.size());
+  NB_TRY(gather_batch(ctx, ha, va, hashes.data(), vals.data()));
+  merkle_decommit_fill(plan, hashes.data(), vals.data(), queried_values, hash_witness, column_witness);
   return NB200_OK;
 }
 

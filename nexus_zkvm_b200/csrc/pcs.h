@@ -3,6 +3,7 @@
 #include "common.cuh"
 #include "air.h"
 #include "jit.h"
+#include "device_channel.cuh"
 #include <utility>
 
 namespace nb {
@@ -21,6 +22,9 @@ nb200_status quotients_launch(nb200_ctx* ctx, const QBatchDev* h_batches, size_t
                               const u32* dom_x, const u32* dom_y, u32 log_size, u32* out /* 4 columns */, u32 row0 = 0, size_t n_rows = 0);
 nb200_status fold_circle_into_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, qm31 alpha);
 nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, qm31 alpha);
+nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, const u32* d_alpha);   // alpha: 4 words in device memory
+// the device channel (device_channel.cuh): mix the 32-byte root at d_root (skipped when null), draw a felt; d_rec = root words, then alpha
+nb200_status channel_mix_draw(nb200_ctx* ctx, DevChannel* d_ch, const uint8_t* d_root, u32* d_rec, int domain_sep);
 nb200_status add_inplace(nb200_ctx* ctx, u32* a, const u32* b, size_t n);
 nb200_status grind(nb200_ctx* ctx, const uint8_t digest[32], u32 pow_bits, uint64_t* nonce_out);
 
@@ -38,9 +42,27 @@ nb200_status logup_generate(nb200_ctx* ctx, const AirComponent& c, const std::ve
 nb200_status logup_rows(nb200_ctx* ctx, const AirComponent& c, const std::vector<const u32*>& mask_cols, const u32* d_params, u32* d_out, u32 rows_log, const JitKernel* jk);
 nb200_status logup_finalize_last(nb200_ctx* ctx, u32 log_size, u32* last4, qm31* claimed);
 nb200_status eval_at_points(nb200_ctx* ctx, const u32* coeffs, size_t n_cols, u32 log_size, const u32* points_xy, size_t n_points, u32* out_qm31);
+// f(points[point]) of the 2^log_size coefficients at `coeffs`
+struct EvalJob { const u32* coeffs; u32 log_size; u32 point; };
+// every job in one launch and one round trip: out_qm31[i] = job i's value; points_xy = n_points x {x[4], y[4]}
+nb200_status eval_at_points_multi(nb200_ctx* ctx, const std::vector<EvalJob>& jobs, const u32* points_xy, size_t n_points, u32* out_qm31);
 nb200_status merkle_decommit(nb200_ctx* ctx, const nb200_tree* tree, const std::vector<ColRef>& cols_in,
                              const std::vector<std::pair<u32, std::vector<u64>>>& queries,
                              std::vector<u32>& queried_values, std::vector<uint8_t>& hash_witness, std::vector<u32>& column_witness);
 nb200_status gather_u32(nb200_ctx* ctx, const std::vector<const u32*>& addrs, u32* host_out);
+// the hashes (32 bytes each) and words at the given device addresses, fetched with one launch and one sync
+nb200_status gather_batch(nb200_ctx* ctx, const std::vector<const uint8_t*>& hash_addrs, const std::vector<const u32*>& val_addrs, uint8_t* hashes_out, u32* vals_out);
+// MerkleProver::decommit split in two: the host-only walk (plan), and the sorting of the gathered results into the decommitment (fill),
+// so that many decommitments can share one gather
+struct DecommitPlan {
+  std::vector<std::pair<u32, u64>> vals;     // (column index in the caller's order, row), walk order
+  std::vector<uint8_t> val_is_query;         // 1 -> queried_values, 0 -> column_witness
+  std::vector<std::pair<u32, u64>> hashes;   // (layer, node): the hash witness, in order
+};
+void merkle_decommit_plan(u32 max_log, const std::vector<u32>& col_logs, const std::vector<std::pair<u32, std::vector<u64>>>& queries, DecommitPlan& plan);
+void merkle_decommit_addrs(const DecommitPlan& plan, const nb200_tree* tree, const std::vector<ColRef>& cols,
+                           std::vector<const uint8_t*>& hash_addrs, std::vector<const u32*>& val_addrs);
+void merkle_decommit_fill(const DecommitPlan& plan, const uint8_t* hashes, const u32* vals,
+                          std::vector<u32>& queried_values, std::vector<uint8_t>& hash_witness, std::vector<u32>& column_witness);
 
 }  // namespace nb

@@ -9,6 +9,7 @@
 // of sums used here (per-batch sum of line terms hoisted to the host) is bit-exact with the reference formula.
 #include "pcs.h"
 #include "blake2s.cuh"
+#include "device_channel.cuh"
 #include "circle_host.h"
 
 namespace nb {
@@ -212,7 +213,8 @@ nb200_status quotients_launch(nb200_ctx* ctx, const QBatchDev* h_batches, size_t
                                                                           out, out + n, out + 2 * n, out + 3 * n, row0, row_end);
   }
   NB_LAUNCH_CHECK(ctx);
-  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  // no sync: the host tables may go once the copies above have returned (a copy from pageable host memory is staged by then), and the
+  // frees are ordered after the kernel on the stream
   dfree(ctx, d_b); dfree(ctx, d_e);
   return NB200_OK;
 }
@@ -244,11 +246,13 @@ __global__ void fold_circle_kernel(u32* __restrict__ dst, const u32* __restrict_
   qm31 cur = ld_q(dst, m, i);
   st_q(dst, m, i, qm31_add(qm31_mul(cur, alpha_sq), fp));
 }
-// dst[i] = f0' + alpha f1',  (f0', f1') = ibutterfly(src[2i], src[2i+1], 1/x_i)
-__global__ void fold_line_kernel(u32* __restrict__ dst, const u32* __restrict__ src, u32 src_log, const u32* __restrict__ itw, u32 tw_len, qm31 alpha) {
+// dst[i] = f0' + alpha f1',  (f0', f1') = ibutterfly(src[2i], src[2i+1], 1/x_i); alpha is read from d_alpha (device memory) when it is set
+__global__ void fold_line_kernel(u32* __restrict__ dst, const u32* __restrict__ src, u32 src_log, const u32* __restrict__ itw, u32 tw_len, qm31 alpha,
+                                 const u32* __restrict__ d_alpha) {
   const size_t n = (size_t)1 << src_log, m = n >> 1;
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= m) return;
+  if (d_alpha) alpha = qm31_make(__ldg(d_alpha), __ldg(d_alpha + 1), __ldg(d_alpha + 2), __ldg(d_alpha + 3));
   u32 t = __ldg(itw + (tw_len - (1u << src_log)) + i);
   qm31 f0 = ld_q(src, n, 2 * i), f1 = ld_q(src, n, 2 * i + 1);
   qm31 s = qm31_add(f0, f1), d = qm31_mul_m31(qm31_sub(f0, f1), t);
@@ -263,12 +267,36 @@ nb200_status fold_circle_into_line(nb200_ctx* ctx, u32* dst, const u32* src, u32
   NB_LAUNCH_CHECK(ctx);
   return NB200_OK;
 }
-nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, qm31 alpha) {
+static nb200_status fold_line_launch(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, qm31 alpha, const u32* d_alpha) {
   NB_ARG(ctx, src_log >= 1, "fold_line: domain too small");
   NB_ARG(ctx, ctx->tw.d_itw && ctx->tw.half_log >= src_log, "fold_line: twiddles");
   size_t m = (size_t)1 << (src_log - 1);
   u32 thr = 256;
-  fold_line_kernel<<<(u32)((m + thr - 1) / thr), thr, 0, ctx->stream>>>(dst, src, src_log, ctx->tw.d_itw, 1u << ctx->tw.half_log, alpha);
+  fold_line_kernel<<<(u32)((m + thr - 1) / thr), thr, 0, ctx->stream>>>(dst, src, src_log, ctx->tw.d_itw, 1u << ctx->tw.half_log, alpha, d_alpha);
+  NB_LAUNCH_CHECK(ctx);
+  return NB200_OK;
+}
+nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, qm31 alpha) { return fold_line_launch(ctx, dst, src, src_log, alpha, nullptr); }
+nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, const u32* d_alpha) {
+  return fold_line_launch(ctx, dst, src, src_log, qm31_zero(), d_alpha);
+}
+
+// ---- the channel between FRI's inner layers (device_channel.cuh): one thread mixes the root a Merkle commit just wrote (unless root is
+// null) and draws the next alpha; rec receives the root's 8 words (zeros without a root) and the alpha's 4
+__global__ void channel_mix_draw_kernel(DevChannel* __restrict__ ch, const u32* __restrict__ root, u32* __restrict__ rec, int domain_sep) {
+  DevChannel c = *ch;
+  u32 r[8];
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { r[i] = root ? root[i] : 0u; rec[i] = r[i]; }
+  if (root) dev_mix_root(c, r);
+  u32 a[4];
+  dev_draw_felt(c, domain_sep != 0, a);
+#pragma unroll
+  for (int i = 0; i < 4; ++i) rec[8 + i] = a[i];
+  *ch = c;
+}
+nb200_status channel_mix_draw(nb200_ctx* ctx, DevChannel* d_ch, const uint8_t* d_root, u32* d_rec, int domain_sep) {
+  channel_mix_draw_kernel<<<1, 1, 0, ctx->stream>>>(d_ch, (const u32*)d_root, d_rec, domain_sep);
   NB_LAUNCH_CHECK(ctx);
   return NB200_OK;
 }

@@ -4,7 +4,8 @@
 //   CommitmentSchemeProver::<SimdBackend, Blake2sMerkleChannel>::new / tree_builder / commit   prover/src/machine.rs:202-263
 //   stwo::prover::prove::<SimdBackend, Blake2sMerkleChannel>(components, channel, scheme)         prover/src/machine.rs:286-290
 // (stwo @0790eba prover/mod.rs, prover/pcs/mod.rs, prover/fri.rs, prover/air/accumulation.rs, core/proof.rs).
-// The transcript (channel) is host-side by nature; every data-parallel step is a kernel launch on ctx->stream.
+// The transcript (channel) is host-side, except between FRI's inner layers (device_channel.cuh); every data-parallel step is a kernel
+// launch on ctx->stream.
 #include "pcs.h"
 #include "host_channel.h"
 #include "circle_host.h"
@@ -515,9 +516,9 @@ struct Queries {
   }
 };
 
-// decommitment positions + witness evaluations of one FRI layer column (compute_decommitment_positions_and_witness_evals)
-static nb200_status positions_and_witness(nb200_ctx* ctx, const nb200_cols* col4, const std::vector<u64>& queries, std::vector<u64>& positions, std::vector<qm31>& witness) {
-  std::vector<u64> need;
+// decommitment positions of one FRI layer column (compute_decommitment_positions_and_witness_evals), and the positions whose values
+// are its witness: the sibling of every query whose sibling is not queried itself
+static void positions_and_witness_plan(const std::vector<u64>& queries, std::vector<u64>& positions, std::vector<u64>& need) {
   size_t i = 0;
   while (i < queries.size()) {
     size_t j = i; u64 key = queries[i] >> 1;
@@ -530,12 +531,6 @@ static nb200_status positions_and_witness(nb200_ctx* ctx, const nb200_cols* col4
     }
     i = j;
   }
-  std::vector<const u32*> addrs;
-  for (u64 p : need) for (int k = 0; k < 4; ++k) addrs.push_back(col4->col(k) + p);
-  std::vector<u32> vals(addrs.size());
-  NB_TRY(gather_u32(ctx, addrs, vals.data()));
-  for (size_t w = 0; w < need.size(); ++w) witness.push_back(qm31_make(vals[4 * w], vals[4 * w + 1], vals[4 * w + 2], vals[4 * w + 3]));
-  return NB200_OK;
 }
 
 static qm31 load_param(const u32* p) { return qm31_make(p[0], p[1], p[2], p[3]); }
@@ -851,33 +846,48 @@ static nb200_status sample_oods(nb200_scheme* s, const AirProgram& air, HostChan
   auto& sampled = o.sampled;
   points.resize(4); sampled.resize(4);
   std::vector<std::vector<qm31>*> sharded_samples;   // (multi-GPU) sampled-value lists of column-sharded columns, one entry per pushed value
+  // every (column, point) pair of every tree is evaluated in one launch; a column-sharded column that this rank does not hold has no job
+  // (its value stays zero until the all-reduce below)
+  std::vector<EvalJob> jobs;
+  std::vector<u32> pts;                                  // one point per distinct (tree, column offsets): 8 words each
+  std::vector<std::vector<std::vector<long>>> job_of(4); // per tree / column / sample: its job, or -1
   for (int t = 0; t < 4; ++t) {
     const SchemeTree& tr = s->trees[t];
-    points[t].resize(tr.cols.size()); sampled[t].resize(tr.cols.size());
+    points[t].resize(tr.cols.size()); sampled[t].resize(tr.cols.size()); job_of[t].resize(tr.cols.size());
     for (size_t g = 0; g < tr.cols.size(); ++g)
       for (int32_t off : offs[t][g]) points[t][g].push_back(mask_point(tr.cols[g].log, off));
-    // groups of consecutive columns of one batch with the same offsets -> one eval_at_points launch
+    // groups of consecutive columns of one batch with the same offsets share their points
     size_t g = 0;
     while (g < tr.cols.size()) {
       size_t h = g + 1;
       while (h < tr.cols.size() && tr.cols[h].batch == tr.cols[g].batch && offs[t][h] == offs[t][g]) ++h;
-      size_t np = offs[t][g].size();
-      if (np > 0) {
-        std::vector<u32> pts(np * 8);
-        for (size_t k = 0; k < np; ++k) { memcpy(&pts[8 * k], points[t][g][k].x.c, 16); memcpy(&pts[8 * k + 4], points[t][g][k].y.c, 16); }
-        std::vector<u32> out((h - g) * np * 4, 0u);
-        if (tr.sharded && tr.cols[g].batch == SchemeTree::BIG) {
-          // column-sharded: this rank evaluates the columns whose coefficients it holds; the others stay zero until the all-reduce below
-          const size_t a = std::max<size_t>(g, tr.own_first), b2 = std::min<size_t>(h, tr.own_first + tr.own_count);
-          if (a < b2) NB_TRY(eval_at_points(ctx, tr.big_coeffs->col(a - tr.own_first), b2 - a, tr.cols[g].log, pts.data(), np, out.data() + (a - g) * np * 4));
-          for (size_t c = g; c < h; ++c) for (size_t k = 0; k < np; ++k) { sampled[t][c].push_back(load_param(&out[((c - g) * np + k) * 4])); sharded_samples.push_back(&sampled[t][c]); }
-        } else {
-          NB_TRY(eval_at_points(ctx, tr.coeff_ptr(g), h - g, tr.cols[g].log, pts.data(), np, out.data()));
-          for (size_t c = g; c < h; ++c) for (size_t k = 0; k < np; ++k) sampled[t][c].push_back(load_param(&out[((c - g) * np + k) * 4]));
+      const size_t np = offs[t][g].size(), p0 = pts.size() / 8;
+      for (size_t k = 0; k < np; ++k) {
+        pts.insert(pts.end(), points[t][g][k].x.c, points[t][g][k].x.c + 4);
+        pts.insert(pts.end(), points[t][g][k].y.c, points[t][g][k].y.c + 4);
+      }
+      const bool big = tr.sharded && tr.cols[g].batch == SchemeTree::BIG;
+      for (size_t c = g; c < h; ++c) {
+        const u32* co = nullptr;
+        if (!big) co = tr.coeff_ptr(c);
+        else if (c >= tr.own_first && c < tr.own_first + tr.own_count) co = tr.big_coeffs->col(c - tr.own_first);
+        for (size_t k = 0; k < np; ++k) {
+          job_of[t][c].push_back(co ? (long)jobs.size() : -1);
+          if (co) jobs.push_back(EvalJob{co, tr.cols[c].log, (u32)(p0 + k)});
         }
       }
       g = h;
     }
+  }
+  std::vector<u32> out(jobs.size() * 4);
+  NB_TRY(eval_at_points_multi(ctx, jobs, pts.data(), pts.size() / 8, out.data()));
+  for (int t = 0; t < 4; ++t) {
+    const SchemeTree& tr = s->trees[t];
+    for (size_t c = 0; c < tr.cols.size(); ++c)
+      for (long j : job_of[t][c]) {
+        sampled[t][c].push_back(j >= 0 ? load_param(&out[4 * j]) : qm31_zero());
+        if (tr.sharded && tr.cols[c].batch == SchemeTree::BIG) sharded_samples.push_back(&sampled[t][c]);
+      }
   }
   if (!sharded_samples.empty()) {
     // every sampled value of a sharded column was computed by exactly one rank (zero elsewhere): one all-reduce completes them.  The list holds one
@@ -963,31 +973,54 @@ static nb200_status fri_commit(nb200_scheme* s, HostChannel& ch, FriState& f, st
   qm31 circle_alpha = ch.draw_felt();
   const size_t last_domain = (size_t)1 << (s->log_last + s->log_blowup);
   u32 L = f.qlogs[0] - 1;
+  u32 n_inner = 0;
+  for (u32 l = L; ((size_t)1 << l) > last_domain && l > 0; --l) ++n_inner;
+  // The inner layers run on the device channel (device_channel.cuh), seeded from the host channel's state: each layer's Merkle root is
+  // mixed and the next alpha drawn by one device thread, so the layers are queued without waiting for the host.  chan = the channel
+  // state (16 words), then per layer its root (8 words) and alpha (4 words).
+  DevBuf chan;
+  NB_TRY(alloc(ctx, chan, 16 + 12 * (size_t)n_inner));
+  DevChannel seed{};
+  for (int i = 0; i < 8; ++i) seed.digest[i] = (u32)ch.digest[4 * i] | ((u32)ch.digest[4 * i + 1] << 8) | ((u32)ch.digest[4 * i + 2] << 16) | ((u32)ch.digest[4 * i + 3] << 24);
+  seed.n_sent[0] = (u32)ch.n_sent; seed.n_sent[1] = (u32)(ch.n_sent >> 32);
+  NB_CUDA(ctx, cudaMemcpyAsync(chan.p, &seed, sizeof(seed), cudaMemcpyHostToDevice, ctx->stream));
+  u32* rec = chan.p + 16;
   ColsPtr layer;
   NB_TRY(alloc(ctx, layer, 4, L));
   NB_CUDA(ctx, cudaMemsetAsync(layer->d, 0, (size_t)16 << L, ctx->stream));
   size_t ci = 0;
   while (((size_t)1 << L) > last_domain) {
+    const size_t k = f.inner.size();
+    if (k >= n_inner) return set_err(ctx, NB200_ERR_STATE, "fri: layer count");
     for (; ci < f.quotients.size() && f.qlogs[ci] - 1 == L; ++ci) NB_TRY(fold_circle_into_line(ctx, layer->d, f.quotients[ci]->d, f.qlogs[ci], circle_alpha));
-    std::vector<ColRef> refs; for (int k = 0; k < 4; ++k) refs.push_back(ColRef{layer->col(k), L});
+    std::vector<ColRef> refs; for (int c = 0; c < 4; ++c) refs.push_back(ColRef{layer->col(c), L});
     const u32* folded = layer->d;
     f.inner.push_back(FriLayer{std::move(layer), nullptr, L});
     nb200_tree* tree = nullptr;
-    NB_TRY(merkle_commit(ctx, refs, &tree));
+    NB_TRY(merkle_commit(ctx, refs, &tree, nullptr, false));
     f.inner.back().tree.reset(tree);
-    ch.mix_root(tree->root);
-    qm31 alpha = ch.draw_felt();
+    NB_TRY(channel_mix_draw(ctx, (DevChannel*)chan.p, tree->layer[0], rec + 12 * k, ch.draw_domain_sep));
     NB_TRY(alloc(ctx, layer, 4, L - 1));
-    NB_TRY(fold_line(ctx, layer->d, folded, L, alpha));
+    NB_TRY(fold_line(ctx, layer->d, folded, L, rec + 12 * k + 8));
     L -= 1;
   }
   // circle columns that fold exactly into the last layer's size would be an upstream assertion failure
   if (ci != f.quotients.size()) return set_err(ctx, NB200_ERR_STATE, "fri: not all columns consumed");
   if (((size_t)1 << L) != last_domain) return set_err(ctx, NB200_ERR_STATE, "fri: last layer size");
+  // one round trip for the whole FRI commit: every root and device-drawn alpha, and the last layer
+  std::vector<u32> recs(12 * (size_t)n_inner);
   std::vector<u32> host((size_t)4 << L);
+  if (!recs.empty()) NB_CUDA(ctx, cudaMemcpyAsync(recs.data(), rec, recs.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
   NB_CUDA(ctx, cudaMemcpyAsync(host.data(), layer->d, host.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
   NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   layer.reset();
+  // the host channel replays the layers: the same state as a channel that mixed each root and drew each alpha itself
+  for (size_t k = 0; k < f.inner.size(); ++k) {
+    memcpy(f.inner[k].tree->root, &recs[12 * k], 32);
+    ch.mix_root(f.inner[k].tree->root);
+    const qm31 alpha = ch.draw_felt();
+    if (memcmp(alpha.c, &recs[12 * k + 8], 16) != 0) return set_err(ctx, NB200_ERR_STATE, "fri: the device channel drew a different alpha than the host channel");
+  }
   // LineEvaluation::interpolate on the host (the last layer has 2^(log_last + blowup) points)
   size_t n = (size_t)1 << L;
   std::vector<qm31> v(n);
@@ -1037,17 +1070,40 @@ static nb200_status decommit(nb200_scheme* s, HostChannel& ch, const FriState& f
   std::vector<std::pair<u32, std::vector<u64>>> by_log;
   for (u32 lg : f.qlogs) by_log.push_back({lg, queries.fold(max_log - lg).positions});
 
+  // Every position is known now: the walks of all the decommitments (first FRI layer, inner layers, trace trees) are planned on the host,
+  // everything they name is fetched with ONE gather, and the results are sorted into the proof in the same order as a walk per tree.
+  std::vector<const uint8_t*> ha;
+  std::vector<const u32*> va;
+  struct Wit { std::vector<qm31>* out; size_t v0, n; };                            // FRI witness values: n QM31s from va[v0]
+  struct Part { DecommitPlan plan; size_t h0, v0; Decommitment* dec; std::vector<u32>* qv; };
+  std::vector<Wit> wits;
+  std::vector<Part> parts;
+  auto plan_witness = [&](const nb200_cols* col4, const std::vector<u64>& q, std::vector<u64>& pos, std::vector<qm31>& w) {
+    std::vector<u64> need;
+    positions_and_witness_plan(q, pos, need);
+    wits.push_back(Wit{&w, va.size(), need.size()});
+    for (u64 p : need) for (int k = 0; k < 4; ++k) va.push_back(col4->col(k) + p);
+  };
+  auto plan_tree = [&](const nb200_tree* tree, const std::vector<ColRef>& refs, const std::vector<std::pair<u32, std::vector<u64>>>& q,
+                       Decommitment& dec, std::vector<u32>* qv) {
+    Part p;
+    std::vector<u32> logs(refs.size());
+    for (size_t i = 0; i < refs.size(); ++i) logs[i] = refs[i].log_size;
+    merkle_decommit_plan(tree->max_log, logs, q, p.plan);
+    p.h0 = ha.size(); p.v0 = va.size(); p.dec = &dec; p.qv = qv;
+    merkle_decommit_addrs(p.plan, tree, refs, ha, va);
+    parts.push_back(std::move(p));
+  };
   {
     std::vector<std::pair<u32, std::vector<u64>>> dpos;
     for (size_t g = 0; g < f.quotients.size(); ++g) {
       std::vector<u64> pos;
-      NB_TRY(positions_and_witness(ctx, f.quotients[g].get(), queries.fold(max_log - f.qlogs[g]).positions, pos, out.first_layer.fri_witness));
+      plan_witness(f.quotients[g].get(), queries.fold(max_log - f.qlogs[g]).positions, pos, out.first_layer.fri_witness);
       dpos.push_back({f.qlogs[g], pos});
     }
     std::vector<ColRef> refs;
     for (size_t g = 0; g < f.quotients.size(); ++g) for (int k = 0; k < 4; ++k) refs.push_back(ColRef{f.quotients[g]->col(k), f.qlogs[g]});
-    std::vector<u32> qv;
-    NB_TRY(merkle_decommit(ctx, f.first_tree.get(), refs, dpos, qv, out.first_layer.decommitment.hash_witness, out.first_layer.decommitment.column_witness));
+    plan_tree(f.first_tree.get(), refs, dpos, out.first_layer.decommitment, nullptr);
     memcpy(out.first_layer.commitment, f.first_tree->root, 32);
   }
   out.inner_layers.resize(f.inner.size());
@@ -1057,11 +1113,10 @@ static nb200_status decommit(nb200_scheme* s, HostChannel& ch, const FriState& f
       const FriLayer& ly = f.inner[k];
       FriLayerProof& lp = out.inner_layers[k];
       std::vector<u64> pos;
-      NB_TRY(positions_and_witness(ctx, ly.cols.get(), lq.positions, pos, lp.fri_witness));
+      plan_witness(ly.cols.get(), lq.positions, pos, lp.fri_witness);
       std::vector<std::pair<u32, std::vector<u64>>> dpos{{ly.log, pos}};
       std::vector<ColRef> refs; for (int c = 0; c < 4; ++c) refs.push_back(ColRef{ly.cols->col(c), ly.log});
-      std::vector<u32> qv;
-      NB_TRY(merkle_decommit(ctx, ly.tree.get(), refs, dpos, qv, lp.decommitment.hash_witness, lp.decommitment.column_witness));
+      plan_tree(ly.tree.get(), refs, dpos, lp.decommitment, nullptr);
       memcpy(lp.commitment, ly.tree->root, 32);
       lq = lq.fold(1);
     }
@@ -1069,12 +1124,23 @@ static nb200_status decommit(nb200_scheme* s, HostChannel& ch, const FriState& f
   out.queried_values.resize(4); out.trees.resize(4);
   for (int t = 0; t < 4; ++t) {
     const SchemeTree& tr = s->trees[t];
+    if (tr.sharded) continue;   // below, with its own gathers and all-reduce
+    std::vector<ColRef> refs;
+    for (size_t g = 0; g < tr.cols.size(); ++g) refs.push_back(ColRef{tr.lde_ptr(g), tr.cols[g].log + blow});
+    plan_tree(tr.merkle.get(), refs, by_log, out.trees[t], &out.queried_values[t]);
+  }
+  std::vector<uint8_t> hashes(ha.size() * 32);
+  std::vector<u32> vals(va.size());
+  NB_TRY(gather_batch(ctx, ha, va, hashes.data(), vals.data()));
+  for (const Wit& w : wits)
+    for (size_t i = 0; i < w.n; ++i) { const u32* v = &vals[w.v0 + 4 * i]; w.out->push_back(qm31_make(v[0], v[1], v[2], v[3])); }
+  for (const Part& p : parts) {
+    std::vector<u32> unused;   // a FRI layer's queried values are not part of the proof
+    merkle_decommit_fill(p.plan, hashes.data() + 32 * p.h0, vals.data() + p.v0, p.qv ? *p.qv : unused, p.dec->hash_witness, p.dec->column_witness);
+  }
+  for (int t = 0; t < 4; ++t) {
+    const SchemeTree& tr = s->trees[t];
     if (tr.sharded) NB_TRY(merkle_decommit_sharded(ctx, tr, blow, by_log, out.queried_values[t], out.trees[t].hash_witness, out.trees[t].column_witness));
-    else {
-      std::vector<ColRef> refs;
-      for (size_t g = 0; g < tr.cols.size(); ++g) refs.push_back(ColRef{tr.lde_ptr(g), tr.cols[g].log + blow});
-      NB_TRY(merkle_decommit(ctx, tr.merkle.get(), refs, by_log, out.queried_values[t], out.trees[t].hash_witness, out.trees[t].column_witness));
-    }
   }
   return NB200_OK;
 }
@@ -1331,6 +1397,29 @@ void nb200_channel_mix_root(nb200_channel* c, const uint8_t root[32]) { c->ch.mi
 void nb200_channel_draw_felt(nb200_channel* c, uint32_t out[4]) { qm31 q = c->ch.draw_felt(); memcpy(out, q.c, 16); }
 void nb200_channel_draw_felts(nb200_channel* c, size_t n, uint32_t* out) { std::vector<qm31> v(n); c->ch.draw_felts(n, v.data()); if (n) memcpy(out, v.data(), n * 16); }
 void nb200_channel_draw_random_bytes(nb200_channel* c, uint8_t out[32]) { c->ch.draw_random_bytes(out); }
+nb200_status nb200_device_channel_draw(nb200_ctx* ctx, const uint8_t digest[32], uint64_t n_sent, const uint8_t* roots, size_t n,
+                                       uint32_t* felts_out, uint8_t digest_out[32], uint64_t* n_sent_out) {
+  if (!ctx || !digest || n == 0 || !felts_out || !digest_out || !n_sent_out) return NB200_ERR_ARG;
+  DevChannel st{};
+  for (int i = 0; i < 8; ++i) st.digest[i] = (u32)digest[4 * i] | ((u32)digest[4 * i + 1] << 8) | ((u32)digest[4 * i + 2] << 16) | ((u32)digest[4 * i + 3] << 24);
+  st.n_sent[0] = (u32)n_sent; st.n_sent[1] = (u32)(n_sent >> 32);
+  DevBuf d;   // the state (16 words), the roots (8 words each), the records (12 words each)
+  NB_TRY(alloc(ctx, d, 16 + 8 * n + 12 * n));
+  u32* d_roots = d.p + 16;
+  u32* d_rec = d_roots + 8 * n;
+  NB_CUDA(ctx, cudaMemcpyAsync(d.p, &st, sizeof(st), cudaMemcpyHostToDevice, ctx->stream));
+  if (roots) NB_CUDA(ctx, cudaMemcpyAsync(d_roots, roots, 32 * n, cudaMemcpyHostToDevice, ctx->stream));
+  for (size_t i = 0; i < n; ++i)
+    NB_TRY(channel_mix_draw(ctx, (DevChannel*)d.p, roots ? (const uint8_t*)(d_roots + 8 * i) : nullptr, d_rec + 12 * i, ctx->draw_domain_sep));
+  std::vector<u32> rec(12 * n);
+  NB_CUDA(ctx, cudaMemcpyAsync(rec.data(), d_rec, rec.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  NB_CUDA(ctx, cudaMemcpyAsync(&st, d.p, sizeof(st), cudaMemcpyDeviceToHost, ctx->stream));
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  for (size_t i = 0; i < n; ++i) memcpy(felts_out + 4 * i, &rec[12 * i + 8], 16);
+  for (int i = 0; i < 8; ++i) for (int b = 0; b < 4; ++b) digest_out[4 * i + b] = (uint8_t)(st.digest[i] >> (8 * b));
+  *n_sent_out = (uint64_t)st.n_sent[0] | ((uint64_t)st.n_sent[1] << 32);
+  return NB200_OK;
+}
 
 // ---- AIR ----
 nb200_status nb200_air_load(nb200_ctx* ctx, const uint32_t* words, size_t n_words, nb200_air** out) {

@@ -56,6 +56,9 @@ extern "C" {
                                  q_log_sizes: *const u32, q_counts: *const u64, q_positions: *const u64, n_sizes: usize,
                                  queried_values: *mut *mut u32, n_queried: *mut usize, hash_witness: *mut *mut u8, n_hashes: *mut usize,
                                  column_witness: *mut *mut u32, n_column_witness: *mut usize) -> c_int;
+    pub fn nb200_merkle_decommit_plan(max_log: u32, col_log_sizes: *const u32, n_cols: usize,
+                                      q_log_sizes: *const u32, q_counts: *const u64, q_positions: *const u64, n_sizes: usize,
+                                      values: *mut *mut u64, n_values: *mut usize, hashes: *mut *mut u64, n_hashes: *mut usize) -> c_int;
     pub fn nb200_free(p: *mut c_void);
     pub fn nb200_hash_node(merkle_hash: c_int, left: *const u8, right: *const u8, values: *const u32, n_values: usize, out: *mut u8) -> c_int;
     // ---- fused commitment
@@ -97,6 +100,8 @@ extern "C" {
     pub fn nb200_channel_draw_felt(ch: *mut nb200_channel, out: *mut u32);
     pub fn nb200_channel_draw_felts(ch: *mut nb200_channel, n: usize, out: *mut u32);
     pub fn nb200_channel_draw_random_bytes(ch: *mut nb200_channel, out: *mut u8);
+    pub fn nb200_device_channel_draw(ctx: *mut nb200_ctx, digest: *const u8, n_sent: u64, roots: *const u8, n: usize,
+                                     felts_out: *mut u32, digest_out: *mut u8, n_sent_out: *mut u64) -> c_int;
     // ---- AIR
     pub fn nb200_air_load(ctx: *mut nb200_ctx, words: *const u32, n_words: usize, out: *mut *mut nb200_air) -> c_int;
     pub fn nb200_air_free(air: *mut nb200_air);
