@@ -81,6 +81,9 @@ SHIPPED_MACHINES = [(20, 21, False), (22, 21, False), (16, 21, False), (8, 1, Fa
 SHIPPED_MULTI = [list(range(4, 12)), list(range(4, 18)), list(range(4, 22))]
 # the reference's v1 main component as data (nexus_v1.NexusV1Machine): log sizes of the tests, bench.py (16 = CPU sample, 20, 22) and smoke()
 SHIPPED_NEXUS_V1 = [8, 9, 12, 16, 18, 20, 22, 24]   # 18 / 24: the sharded large-proof test (default size / configs[3])
+# the keccak precompile extension (keccak.KeccakMachine): log2 of the permutation count of tests/test_gpu_keccak.py (KeccakRound 0 at 2^10 and 2^12
+# rows; 2^18 rows) and of tools/keccak_prove.py
+SHIPPED_KECCAK = [6, 8, 14]
 
 
 def kernel_sources(words, short_checks=False):
@@ -126,6 +129,8 @@ def precompile_kernels(machines=SHIPPED_MACHINES, verbose=False):
     ms += [M.MultiMachine(sizes) for sizes in SHIPPED_MULTI]
     from .nexus_v1 import NexusV1Machine
     ms += [NexusV1Machine(ls) for ls in SHIPPED_NEXUS_V1]
+    from .keccak import KeccakMachine
+    ms += [KeccakMachine(lp) for lp in SHIPPED_KECCAK]
     for m in ms:
         for key, src in kernel_sources(m.words, short_checks=True):
             path = os.path.join(JIT_CACHE, f"{key:016x}.cubin")
