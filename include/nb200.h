@@ -148,6 +148,26 @@ nb200_status nb200_commit_host_packed(nb200_ctx*, const void* const* host_batche
                                       const uint32_t* log_sizes, size_t n_batches, int coset_order, uint32_t log_blowup,
                                       nb200_cols** evals_io, nb200_cols** coeffs_io, nb200_cols** lde_io, nb200_tree** tree_out, uint8_t root[32]);
 
+/* ---- the keccak precompile extension's main trace, filled on the device from its side note ------------------------------------
+ * The reference fills tree 1 of keccak_extensions() (prover/src/extensions/keccak/mod.rs:12-33) on the host from KeccakSideNote
+ * (prover/src/trace/sidenote/keccak.rs:16-25) and hands over its BaseColumns; here only the side note crosses PCIe:
+ *   inputs     = n_perms x 25 input lanes (lane x + 5 y),
+ *   addresses  = n_perms base addresses (state byte k is at address + k),
+ *   timestamps = n_perms x 200 previous timestamps, one per state byte.
+ * Out: five new device batches (owned by the caller, nb200_cols_free) in commitment order and finalized order, ready for
+ * nb200_scheme_commit:
+ *   out[0] PermutationMemoryCheck, 2001 columns  (memory_check/trace.rs:32-123)
+ *   out[1] KeccakRound 0 (rounds 0..15), 1705    (round/trace.rs:297-366)
+ *   out[2] KeccakRound 1 (rounds 16..23), 1705
+ *   out[3] the XorTable then BitNotAndTable multiplicities, 32 columns of 2^12 rows (bitwise_table/constraints.rs:46-68)
+ *   out[4] the BitRotateTable multiplicity, 1 column of 2^11 rows (bit_rotate/mod.rs:69-91)
+ * Log sizes: memory check max(log2ceil(n_perms), 4), KeccakRound 0 / 1 max(log2ceil(16 / 8 n_perms), 4) (compute_log_size).  Padding
+ * rows of a round component hold the zero state and their lookups are counted; multiplicities are stored mod P.
+ * NB200_ERR_ARG: n_perms == 0 or above 2^18 (the multiplicity counters are 32-bit), an address above 2^32 - 200, a timestamp of
+ * 2^32 - 1.  Scratch memory (the side note on the device, the histograms) is released in stream order before the call returns. */
+nb200_status nb200_keccak_main_trace(nb200_ctx*, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
+                                     nb200_cols** out);
+
 /* ---- one commitment over N GPUs (SURVEY §8e; one process per GPU, NCCL over NVLink inside the library) ------------------------
  * The reference has no multi-device path (SURVEY App. C); these entry points are what a multi-GPU `CudaBackend` would drive from
  * TreeBuilder::commit (machine.rs:208-263).  Rank 0 creates the id and hands it to the other ranks out of band (MPI, a file,

@@ -236,6 +236,19 @@ class Context:
             ldes = [Columns(self, C.c_void_p(ld[i])) for i in range(n)]
         return evals, coeffs, ldes, MerkleTree(self, t, bytes(root), ldes)
 
+    def keccak_main_trace(self, inputs, addresses, timestamps):
+        """nb200_keccak_main_trace: tree 1 of the keccak extension filled on the device from its side note (inputs: (n_perms, 25) uint64
+        lanes, addresses: (n_perms,) uint32, timestamps: (n_perms, 200) uint32).  Returns its five device batches in commitment order."""
+        inp = np.ascontiguousarray(inputs, dtype=np.uint64)
+        addr = np.ascontiguousarray(addresses, dtype=np.uint32)
+        ts = np.ascontiguousarray(timestamps, dtype=np.uint32)
+        n = inp.shape[0] if inp.ndim == 2 else 0
+        assert inp.shape == (n, 25) and addr.shape == (n,) and ts.shape == (n, 200), "side note shapes"
+        out = (C.c_void_p * 5)()
+        self._chk(lib().nb200_keccak_main_trace(self._h, C.c_size_t(n), inp.ctypes.data_as(u64p), addr.ctypes.data_as(u32p),
+                                                ts.ctypes.data_as(u32p), out))
+        return [Columns(self, C.c_void_p(out[i])) for i in range(5)]
+
     # ---- multi-GPU (one process per GPU): NCCL communicator inside the library
     @staticmethod
     def comm_unique_id():

@@ -24,6 +24,8 @@ nb200_status merkle_decommit(nb200_ctx* ctx, const nb200_tree* tree, const std::
                              const std::vector<std::pair<u32, std::vector<u64>>>& queries,
                              std::vector<u32>& queried_values, std::vector<uint8_t>& hash_witness, std::vector<u32>& column_witness);
 nb200_status eval_at_points(nb200_ctx* ctx, const u32* coeffs, size_t n_cols, u32 log_size, const u32* points_xy, size_t n_points, u32* out_qm31);
+nb200_status keccak_main_trace(nb200_ctx* ctx, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
+                               nb200_cols** out);
 }  // namespace nb
 using namespace nb;
 
@@ -453,6 +455,13 @@ nb200_status nb200_commit_evals(nb200_ctx* ctx, const nb200_cols* const* eval_ba
   NB_TRY(merkle_commit(ctx, cols, tree_out));
   if (root) memcpy(root, (*tree_out)->root, 32);
   return NB200_OK;
+}
+
+// ---- the keccak precompile extension's main trace from its side note (csrc/keccak_trace.cu) ----
+nb200_status nb200_keccak_main_trace(nb200_ctx* ctx, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
+                                     nb200_cols** out) {
+  if (!ctx) return NB200_ERR_ARG;
+  return keccak_main_trace(ctx, n_perms, inputs, addresses, timestamps, out);
 }
 
 }  // extern "C"

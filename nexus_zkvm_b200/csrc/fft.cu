@@ -18,6 +18,7 @@
 //   `fft_tile_kernel<INV,T,W>` is the compile-time specialised fast path; `fft_pass_kernel` is the generic
 //   fallback for shapes outside the specialised set.
 #include "fft_common.cuh"
+#include "finalize_order.cuh"
 #include "circle_host.h"
 #include <map>
 #include <mutex>
@@ -370,12 +371,7 @@ __global__ void reorder_kernel(const void* __restrict__ src, u32* __restrict__ d
   size_t n = (size_t)1 << log_size;
   size_t c = e >> log_size;
   u32 i = (u32)(e & (n - 1));
-  size_t s = i;
-  if (coset_order) {
-    u32 j = log_size ? (__brev(i) >> (32 - log_size)) : 0;
-    size_t half = n >> 1;
-    s = j < half ? ((size_t)j << 1) : (n - 1 - (((size_t)j - half) << 1));
-  }
+  const size_t s = coset_order ? finalized_src_row(i, log_size) : i;
   u32 v;
   if (EB == 1) v = reinterpret_cast<const uint8_t*>(src)[c * n + s];
   else if (EB == 2) v = reinterpret_cast<const uint16_t*>(src)[c * n + s];

@@ -228,9 +228,22 @@ class KeccakMachine:
     prove_keccak test takes (1 << log_n_instances) - 1 inputs: every component then has padding rows).  Sizes (compute_log_size):
     memory check 2^max(log2ceil(n_perms), 4) rows, KeccakRound 0 / 1 16 / 8 rows per permutation rounded up to a power of two, the tables
     fixed.  Same interface as the other machines: `air`, `words`, `relations`, `log_sizes`, `preprocessed_columns()`, `fill_main_trace()`
-    (tree 1 in commitment order, the table multiplicities last: `multiplicity_columns()`), `column_log_sizes()`."""
+    (tree 1 in commitment order, the table multiplicities last: `multiplicity_columns()`), `column_log_sizes()`.
 
-    def __init__(self, log_n_perms, seed=0, n_perms=None):
+    An explicit side note (the layout of KeccakSideNote, prover/src/trace/sidenote/keccak.rs:16-25) proves given permutations instead of
+    seeded random ones: `inputs` (n_perms, 25) lanes x + 5 y, `addresses` (n_perms,) base addresses, `timestamps` (n_perms, 200) previous
+    timestamps; `log_n_perms`, `seed` and `n_perms` are then ignored.  An address range must not wrap 2^32 and no timestamp may be 2^32 - 1.
+    `device_trees(ctx)` fills tree 1 on the device from the side note (nb200_keccak_main_trace) for machine.prove(..., resident=...)."""
+
+    def __init__(self, log_n_perms=None, seed=0, n_perms=None, inputs=None, addresses=None, timestamps=None):
+        if inputs is not None:
+            inputs = np.array(inputs, dtype=np.uint64)
+            n_perms = inputs.shape[0]
+            addresses = np.array(addresses, dtype=np.uint64)
+            timestamps = np.array(timestamps, dtype=np.uint64)
+            assert inputs.shape == (n_perms, 25) and addresses.shape == (n_perms,) and timestamps.shape == (n_perms, STATE_SIZE)
+            assert int(addresses.max(initial=0)) <= (1 << 32) - STATE_SIZE, "an address range of 200 bytes wraps 2^32"
+            assert int(timestamps.max(initial=0)) < (1 << 32) - 1, "a timestamp of 2^32 - 1 has no successor"
         self.n_perms = (1 << log_n_perms) - 1 if n_perms is None else int(n_perms)
         assert self.n_perms >= 1
         self.seed = seed
@@ -253,6 +266,10 @@ class KeccakMachine:
         self.log_sizes = [self.mem_log_size] + self.round_log_sizes + [BITWISE_LOG_SIZE, BITWISE_LOG_SIZE, ROTATE_LOG_SIZE]
         self.log_size = max(self.log_sizes)
         self.words = air.serialize()
+        self._main = None
+        if inputs is not None:
+            self.inputs, self.addresses, self.timestamps = np.ascontiguousarray(inputs.T), addresses, timestamps
+            return
         rng = np.random.default_rng(seed)
         self.inputs = rng.integers(0, 1 << 64, (25, self.n_perms), dtype=np.uint64, endpoint=False)
         # memory side note: one base address per permutation, one previous timestamp per state byte; low 16 bits near 0xffff on
@@ -261,7 +278,24 @@ class KeccakMachine:
         self.addresses = (rng.integers(0, 1 << 14, self.n_perms).astype(np.uint64) << np.uint64(16)) | lo.astype(np.uint64)
         ts_lo = np.where(rng.integers(0, 8, (self.n_perms, STATE_SIZE)) == 0, 0xFFFF, rng.integers(0, 0x10000, (self.n_perms, STATE_SIZE)))
         self.timestamps = (rng.integers(0, 1 << 14, (self.n_perms, STATE_SIZE)).astype(np.uint64) << np.uint64(16)) | ts_lo.astype(np.uint64)
-        self._main = None
+
+    def side_note(self):
+        """(inputs (n_perms, 25) uint64, addresses (n_perms,) uint32, timestamps (n_perms, 200) uint32): the arguments of
+        nb200_keccak_main_trace."""
+        return (np.ascontiguousarray(self.inputs.T), self.addresses.astype(np.uint32), np.ascontiguousarray(self.timestamps, dtype=np.uint32))
+
+    def device_trees(self, ctx):
+        """(tree-0 device batches, tree-1 device batches), finalized order, for machine.prove / check_constraints(..., resident=...): tree 0
+        uploaded from preprocessed_columns() (27 small columns), tree 1 filled on the device from the side note (nb200_keccak_main_trace:
+        the memory check, the two round components, the 32 bitwise and the rotate multiplicity columns, batched as the host columns are)."""
+        cols, tree0, i = self.preprocessed_columns(), [], 0
+        while i < len(cols):
+            j = i
+            while j < len(cols) and len(cols[j]) == len(cols[i]):
+                j += 1
+            tree0.append(ctx.upload(np.stack(cols[i:j]), coset_order=True))
+            i = j
+        return tree0, ctx.keccak_main_trace(*self.side_note())
 
     # ---- tree 0
     def preprocessed_columns(self):

@@ -153,11 +153,12 @@ def prove(machine, backend, main_cols, mult, config=None, associated_data=b"", r
     return proof, claimed, aux
 
 
-def check_constraints(machine, backend, main_cols, mult, associated_data=b""):
+def check_constraints(machine, backend, main_cols, mult, associated_data=b"", resident=None):
     """assert_constraints_on_polys for every component (the reference's `assert_chip` / `assert_component`) on the GPU: the trees are committed
     as `prove` commits them, then each component's constraints are evaluated on every row of its trace domain.  Returns
-    ({component: [(constraint, degree, failing rows, first failing row in trace order)]}, whether the claimed LogUp sums cancel)."""
-    _ch, prover, params, claimed, _roots, _ls = _commit_trees(machine, backend, main_cols, mult, None, associated_data, None)
+    ({component: [(constraint, degree, failing rows, first failing row in trace order)]}, whether the claimed LogUp sums cancel).
+    `resident` as in `prove`: trees 0 and 1 already on the device (e.g. a keccak trace filled there)."""
+    _ch, prover, params, claimed, _roots, _ls = _commit_trees(machine, backend, main_cols, mult, None, associated_data, resident)
     report = {k: prover.check_constraints(k, params) for k in range(len(machine.air.components))}
     return report, verify_claimed_sums(claimed)
 

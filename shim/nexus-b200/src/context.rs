@@ -81,6 +81,19 @@ impl Context {
         }
         Ok(out)
     }
+    /// Tree 1 of `keccak_extensions()` (prover/src/extensions/keccak/mod.rs:12-33) filled on the device from the extension's side note
+    /// (`KeccakSideNote`, prover/src/trace/sidenote/keccak.rs:16-25): `inputs[p]` the 25 input lanes, `addresses[p]` the base address,
+    /// `timestamps[p]` the 200 previous timestamps of permutation p.  Returns the five batches of `nb200_keccak_main_trace` (memory check,
+    /// KeccakRound 0, KeccakRound 1, bitwise multiplicities, rotate multiplicity), finalized, in commitment order.
+    pub fn keccak_main_trace(&self, inputs: &[[u64; 25]], addresses: &[u32], timestamps: &[Vec<u32>]) -> Result<Vec<Columns>> {
+        assert!(addresses.len() == inputs.len() && timestamps.len() == inputs.len());
+        let ts: Vec<u32> = timestamps.iter().flat_map(|t| { assert_eq!(t.len(), 200); t.iter().copied() }).collect();
+        let mut out = [ptr::null_mut(); 5];
+        self.check(unsafe {
+            nb200_keccak_main_trace(self.raw(), inputs.len(), inputs.as_ptr() as *const u64, addresses.as_ptr(), ts.as_ptr(), out.as_mut_ptr())
+        })?;
+        Ok(out.iter().map(|&h| Columns { ctx: self.clone(), h }).collect())
+    }
     /// NCCL communicator of this context (one process per GPU): rank 0 calls `comm_unique_id()`, ships the bytes to the other ranks, all call `comm_init`.
     pub fn comm_unique_id() -> Result<Vec<u8>> {
         let mut id = vec![0u8; unsafe { nb200_comm_unique_id_bytes() }];

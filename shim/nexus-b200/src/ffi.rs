@@ -72,6 +72,9 @@ extern "C" {
     pub fn nb200_commit_host_packed(ctx: *mut nb200_ctx, host_batches: *const *const c_void, elem_bytes: *const u32, n_cols: *const usize,
                                     log_sizes: *const u32, n_batches: usize, coset_order: c_int, log_blowup: u32, evals_io: *mut *mut nb200_cols,
                                     coeffs_io: *mut *mut nb200_cols, lde_io: *mut *mut nb200_cols, tree_out: *mut *mut nb200_tree, root: *mut u8) -> c_int;
+    // ---- the keccak extension's main trace filled on the device from its side note (out: 5 batches)
+    pub fn nb200_keccak_main_trace(ctx: *mut nb200_ctx, n_perms: usize, inputs: *const u64, addresses: *const u32, timestamps: *const u32,
+                                   out: *mut *mut nb200_cols) -> c_int;
     // ---- one commitment over N GPUs (NCCL inside the library)
     pub fn nb200_comm_unique_id_bytes() -> usize;
     pub fn nb200_comm_get_unique_id(id_out: *mut u8) -> c_int;
