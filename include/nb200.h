@@ -287,6 +287,28 @@ nb200_status nb200_check_constraints(nb200_ctx*, const nb200_air*, uint32_t comp
                                      const nb200_cols* const* tree2, size_t n2, const uint32_t* params, size_t n_params,
                                      uint64_t* n_failing, uint64_t* first_row, size_t n);
 
+/* ---- lookup-table multiplicities, counted on the GPU from the AIR's own lookups --------------------------------------------------
+ * Every fraction's denominator is Relation::combine, sum_i alpha_i v_i - z; its relation is named by the z parameter and its tuple is
+ * (v_0 .. v_n-1).  A table fraction has the numerator -m for one tree-1 column m (its multiplicity column) and a tuple of tree-0 columns
+ * and constants; a lookup is any other fraction into a relation that has a table fraction.  Relations without one are ignored.
+ * nb200_air_lookup_tables: per fraction of the component (declaration order; n = its fraction count): kind (0 ignored, 1 table, 2 lookup,
+ * 3 does not parse where it would be needed), relation (the z parameter index; UINT32_MAX when the denominator does not parse) and arg (a
+ * table: the index of its multiplicity column in tree 1; otherwise the tuple length).  No device needed.
+ * nb200_air_count_kernel_source: the CUDA C of the component's count kernel (NVRTC, sm_90a; its own cubin-cache key), malloc'ed, free with
+ * nb200_free; NB200_ERR_STATE when the component has neither a table nor a lookup, NB200_ERR_ARG when a fraction it needs does not parse.
+ * It is an entry of its own rather than a fifth `which` of nb200_air_kernel_source, which keeps answering NB200_ERR_ARG outside 0-3. */
+nb200_status nb200_air_lookup_tables(const nb200_air*, uint32_t component, uint32_t* kind, uint32_t* relation, uint32_t* arg, size_t n);
+nb200_status nb200_air_count_kernel_source(const nb200_air*, uint32_t component, char** out);
+/* The multiplicity column of every table fraction, written in place into the tree-1 batch that holds it (finalized order, mod P; whatever the
+ * column held is overwritten): the sum of the numerators of the lookups whose tuple equals that row's, over every row of every component.
+ * tree0 / tree1 = the evaluation batches of trees 0 and 1 in commitment and finalized order, before tree 1 is committed.  A lookup with a
+ * nonzero numerator whose tuple is in no table row is unmatched: n_unmatched counts them, first_unmatched = (component, fraction, row in
+ * trace order) of the smallest, or UINT32_MAX x 3.  Returns NB200_OK whether or not lookups were unmatched; NB200_ERR_ARG for a missing or
+ * wrongly sized column, a needed fraction that does not parse, a tuple listed twice in one relation, or more than 2^33 lookups (rows x
+ * lookup fractions); NB200_ERR_STATE with NB200_JIT=0 (the count has no interpreter).  Scratch is released in stream order. */
+nb200_status nb200_table_multiplicities(nb200_ctx*, const nb200_air*, const nb200_cols* const* tree0, size_t n0, nb200_cols* const* tree1, size_t n1,
+                                        uint64_t* n_unmatched, uint32_t first_unmatched[3]);
+
 /* ---- one PROOF over N GPUs ---------------------------------------------------------------------------------------------------
  * Every rank calls the same sequence (the Machine::prove order, machine.rs:197-290) with its own shard; transcript, roots and proof
  * bytes come out identical on all ranks and identical to the single-GPU proof.

@@ -249,6 +249,17 @@ class Context:
                                                 ts.ctypes.data_as(u32p), out))
         return [Columns(self, C.c_void_p(out[i])) for i in range(5)]
 
+    def table_multiplicities(self, air, tree0, tree1):
+        """nb200_table_multiplicities: every table fraction's multiplicity column of `tree1` (device batches, finalized order) is overwritten
+        with the count of the AIR's lookups into it.  `air` is a loaded AIR (prover.Air).  Returns (n_unmatched, first_unmatched), the latter
+        (component, fraction, row in trace order) of the smallest unmatched lookup, or None."""
+        t0 = (C.c_void_p * max(len(tree0), 1))(*[b._h for b in tree0])
+        t1 = (C.c_void_p * max(len(tree1), 1))(*[b._h for b in tree1])
+        n = C.c_uint64()
+        first = (C.c_uint32 * 3)()
+        self._chk(lib().nb200_table_multiplicities(self._h, air._h, t0, C.c_size_t(len(tree0)), t1, C.c_size_t(len(tree1)), C.byref(n), first))
+        return int(n.value), (None if n.value == 0 else tuple(int(x) for x in first))
+
     # ---- multi-GPU (one process per GPU): NCCL communicator inside the library
     @staticmethod
     def comm_unique_id():

@@ -134,6 +134,7 @@ class ComponentBuilder:
         self.mask_slot = {}
         self.constraints = []  # node ids
         self.fracs = []        # (num node id (E), den node id (E))
+        self.lookups = []      # per fraction: (relation, numerator Expr, values: Exprs or ints) — kept on the Python side only (not serialized)
         self.batching = None
         self.cumsum_shift_param = NO_PARAM
         self.interaction_col0 = None
@@ -228,6 +229,7 @@ class ComponentBuilder:
         assert len(values) <= relation.size
         if not isinstance(multiplicity, Expr):
             multiplicity = self.const(multiplicity)
+        self.lookups.append((relation, multiplicity, list(values)))
         self.fracs.append((self._to_e(multiplicity).id, self.combine(relation, values).id))
 
     def _frac_sum(self, ids):

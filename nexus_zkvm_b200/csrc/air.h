@@ -4,6 +4,7 @@
 #pragma once
 #include "m31.cuh"
 #include <string>
+#include <utility>
 #include <vector>
 #include <stdexcept>
 
@@ -163,6 +164,138 @@ inline std::vector<char> masks_read_by(const AirComponent& c, const std::vector<
     }
   }
   return used;
+}
+
+// register kind ('b' base, 'e' secure, 0 none) of operands a and b and of the destination
+inline void operand_kinds(u32 op, char& ka, char& kb, char& kd) {
+  ka = kb = kd = 0;
+  switch (op) {
+    case OP_LOADM: case OP_CONSTB: kd = 'b'; break;
+    case OP_ADDB: case OP_SUBB: case OP_MULB: ka = kb = kd = 'b'; break;
+    case OP_NEGB: ka = kd = 'b'; break;
+    case OP_PARAME: case OP_LOADME: kd = 'e'; break;
+    case OP_ADDE: case OP_SUBE: case OP_MULE: ka = kb = kd = 'e'; break;
+    case OP_NEGE: ka = kd = 'e'; break;
+    case OP_ADDEB: case OP_SUBEB: case OP_MULEB: ka = kd = 'e'; kb = 'b'; break;
+    case OP_BTOE: ka = 'b'; kd = 'e'; break;
+    case OP_CONSTRB: ka = 'b'; break;
+    case OP_CONSTRE: ka = 'e'; break;
+    case OP_FRAC: ka = kb = 'e'; break;
+    default: break;
+  }
+}
+
+// Reaching definitions: def_a / def_b[pc] = position of the instruction whose result operand a / b of prog[pc] reads (-1: none).  Registers
+// are reused, so a register number alone names nothing; a position does.
+inline void prog_defs(const std::vector<AirInstr>& prog, u32 nb, u32 ne, std::vector<int>& def_a, std::vector<int>& def_b) {
+  const int n = (int)prog.size();
+  def_a.assign(n, -1); def_b.assign(n, -1);
+  std::vector<int> cur_b(nb + 1, -1), cur_e(ne + 1, -1);
+  for (int pc = 0; pc < n; ++pc) {
+    const AirInstr& in = prog[pc];
+    char ka, kb, kd;
+    operand_kinds(in.op, ka, kb, kd);
+    if (ka) def_a[pc] = (ka == 'b' ? cur_b : cur_e)[in.a];
+    if (kb) def_b[pc] = (kb == 'b' ? cur_b : cur_e)[in.b];
+    if (kd) (kd == 'b' ? cur_b : cur_e)[in.dst] = pc;
+  }
+}
+
+// ---- lookup tables and their lookups, read off the logup programs (nb200_table_multiplicities)
+// Every fraction's denominator is Relation::combine (air.py ComponentBuilder.combine): sum_i alpha_i v_i - z, i.e.
+//   SUBE(ADDE(..ADDE(MULEB(PARAME alpha_0, v_0), MULEB(PARAME alpha_1, v_1)).., MULEB(PARAME alpha_n-1, v_n-1)), PARAME z).
+// The relation is named by its z parameter, the tuple is (v_0 .. v_n-1).  A table fraction has the numerator -m for one tree-1 mask m (its
+// multiplicity column) and a tuple that reads tree-0 masks and constants only; every other fraction into a relation that has a table
+// fraction is a lookup of that table, and must have a base-field numerator.  Relations without a table fraction are not counted.
+enum FracKind : u32 { FRAC_IGNORED = 0, FRAC_TABLE = 1, FRAC_LOOKUP = 2, FRAC_BAD = 3 };
+struct AirFrac {
+  u32 kind = FRAC_IGNORED;
+  u32 rel = 0xFFFFFFFFu;     // z parameter of the relation (0xFFFFFFFF: the denominator does not parse)
+  u32 mult_mask = 0;         // FRAC_TABLE: the mask of the multiplicity column
+  int num = -1;              // position of the base value whose BTOE is the numerator (-1: not a base value)
+  std::vector<int> tuple;    // positions of the instructions that compute v_0 .. v_n-1
+  std::string why;           // FRAC_BAD: what does not parse
+};
+inline std::vector<std::vector<AirFrac>> air_lookup_tables(const AirProgram& a) {
+  std::vector<std::vector<AirFrac>> out(a.comps.size());
+  std::vector<char> has_table(a.n_params, 0);
+  std::vector<std::vector<u32>> alphas(a.n_params);   // per z: the alpha parameter of each tuple position seen so far
+  for (size_t k = 0; k < a.comps.size(); ++k) {
+    const AirComponent& c = a.comps[k];
+    const std::vector<AirInstr>& prog = c.logup_prog;
+    std::vector<int> da, db;
+    prog_defs(prog, c.lg_base_regs, c.lg_ext_regs, da, db);
+    std::vector<signed char> t0(prog.size(), -1);     // memo: the base value reads tree-0 masks and constants only
+    auto only_tree0 = [&](int q, auto& self) -> bool {
+      if (q < 0) return false;
+      if (t0[q] >= 0) return t0[q] != 0;
+      const AirInstr& in = prog[q];
+      bool r = false;
+      switch (in.op) {
+        case OP_LOADM: r = c.masks[in.a].tree == 0; break;
+        case OP_CONSTB: r = true; break;
+        case OP_ADDB: case OP_SUBB: case OP_MULB: r = self(da[q], self) && self(db[q], self); break;
+        case OP_NEGB: r = self(da[q], self); break;
+        default: break;
+      }
+      t0[q] = r ? 1 : 0;
+      return r;
+    };
+    auto param = [&](int q) { return q >= 0 && prog[q].op == OP_PARAME; };
+    for (size_t pc = 0; pc < prog.size(); ++pc) {
+      if (prog[pc].op != OP_FRAC) continue;
+      AirFrac f;
+      const int d = db[pc];
+      if (d >= 0 && prog[d].op == OP_SUBE && param(db[d])) {
+        f.rel = prog[db[d]].a;
+        std::vector<std::pair<u32, int>> terms;   // (alpha parameter, value), last term first
+        auto term = [&](int t) {
+          if (t < 0 || prog[t].op != OP_MULEB || !param(da[t]) || db[t] < 0) return false;
+          terms.push_back({prog[da[t]].a, db[t]});
+          return true;
+        };
+        bool ok = true;
+        int x = da[d];
+        while (ok && x >= 0 && prog[x].op == OP_ADDE) { ok = term(db[x]); x = da[x]; }
+        ok = ok && term(x);
+        if (ok) {
+          std::vector<u32>& al = alphas[f.rel];
+          for (size_t i = 0; i < terms.size() && ok; ++i) {
+            const u32 alpha = terms[terms.size() - 1 - i].first;
+            if (i < al.size()) ok = al[i] == alpha;
+            else al.push_back(alpha);
+            f.tuple.push_back(terms[terms.size() - 1 - i].second);
+          }
+          if (!ok) f.why = "the tuple's alpha parameters differ from another fraction's of the same relation";
+        } else {
+          f.why = "the denominator is not sum_i alpha_i v_i - z with base-field v_i";
+        }
+        if (!ok) { f.kind = FRAC_BAD; f.tuple.clear(); }
+      } else {
+        f.kind = FRAC_BAD;
+        f.why = "the denominator is not a combination minus the relation's z parameter";
+      }
+      const int nq = da[pc];
+      if (nq >= 0 && prog[nq].op == OP_BTOE) f.num = da[nq];
+      if (f.kind != FRAC_BAD && f.num >= 0 && prog[f.num].op == OP_NEGB) {
+        const int m = da[f.num];
+        bool table = m >= 0 && prog[m].op == OP_LOADM && c.masks[prog[m].a].tree == 1 && c.masks[prog[m].a].off == 0;
+        for (int v : f.tuple) table = table && only_tree0(v, only_tree0);
+        if (table) { f.kind = FRAC_TABLE; f.mult_mask = prog[m].a; has_table[f.rel] = 1; }
+      }
+      out[k].push_back(std::move(f));
+    }
+  }
+  for (auto& comp : out)
+    for (AirFrac& f : comp) {
+      if (f.kind == FRAC_TABLE) continue;
+      const bool into_table = f.rel < a.n_params && has_table[f.rel];
+      if (f.kind == FRAC_BAD) { if (f.rel < a.n_params && !into_table) f.kind = FRAC_IGNORED; continue; }   // not needed
+      if (!into_table) continue;
+      if (f.num < 0) { f.kind = FRAC_BAD; f.why = "a lookup into a table has a numerator outside the base field"; continue; }
+      f.kind = FRAC_LOOKUP;
+    }
+  return out;
 }
 
 }  // namespace nb

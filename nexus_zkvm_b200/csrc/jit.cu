@@ -145,24 +145,6 @@ void emit_op(std::ostringstream& o, const AirInstr& in, Ld ld) {
 // boundaries cost more than the arithmetic (the synthetic ADD machine has 4 + 4 and never showed it).
 struct ChunkLive { std::vector<std::vector<u32>> in_b, in_e, out_b, out_e; };
 struct Regs { std::vector<u32> rb, re; int wb = -1, we = -1; };   // registers a statement reads and writes (base / secure)
-// register kind ('b' base, 'e' secure, 0 none) of operands a and b and of the destination
-static void operand_kinds(u32 op, char& ka, char& kb, char& kd) {
-  ka = kb = kd = 0;
-  switch (op) {
-    case OP_LOADM: case OP_CONSTB: kd = 'b'; break;
-    case OP_ADDB: case OP_SUBB: case OP_MULB: ka = kb = kd = 'b'; break;
-    case OP_NEGB: ka = kd = 'b'; break;
-    case OP_PARAME: case OP_LOADME: kd = 'e'; break;
-    case OP_ADDE: case OP_SUBE: case OP_MULE: ka = kb = kd = 'e'; break;
-    case OP_NEGE: ka = kd = 'e'; break;
-    case OP_ADDEB: case OP_SUBEB: case OP_MULEB: ka = kd = 'e'; kb = 'b'; break;
-    case OP_BTOE: ka = 'b'; kd = 'e'; break;
-    case OP_CONSTRB: ka = 'b'; break;
-    case OP_CONSTRE: ka = 'e'; break;
-    case OP_FRAC: ka = kb = 'e'; break;
-    default: break;
-  }
-}
 static Regs instr_regs(const AirInstr& in) {
   Regs r;
   char ka, kb, kd;
@@ -611,11 +593,170 @@ std::string gen_check_source(const AirComponent& c) {
   o << "}\n";
   return o.str();
 }
+
+// The table-multiplicity count (nb200_table_multiplicities) of one component, from its logup program as air_lookup_tables reads it.
+// mode 0 (build): every table fraction's tuple on every row goes into an open-addressing hash keyed by (relation, length, values), the
+//                 value being the row's bin: tbase[t] + the row's position (finalized order).  A tuple that is already there sets *err.
+// mode 1 (probe): every lookup with a nonzero numerator finds its tuple's bin and adds the numerator to its u64 counter (in shared memory
+//                 when the caller privatises the bins, nsh > 0).  A tuple without a bin is unmatched: um[0] counts them, um[1] keeps the
+//                 smallest (component << 48 | fraction << 28 | row in coset order).
+// Only base values are evaluated: each chunk recomputes, as SSA values, what its fractions read (mask loads and a few base operations), so
+// no register crosses a chunk.  Hash and bins are laid out by the caller; the source depends on this component alone.
+std::string gen_count_source(const AirComponent& c, const std::vector<AirFrac>& fr) {
+  std::ostringstream o;
+  o << "// table multiplicities: build (table tuples -> bins) and probe (lookups -> counters)\n";
+  o << kPrelude;
+  o << "#define NB_DL " << c.log_size << "u\n#define NB_N (1u << NB_DL)\n"
+    << "__device__ __forceinline__ u32 pos_to_row(u32 i) { const u32 j = __brev(i) >> (32 - NB_DL); return j < NB_N / 2 ? 2 * j : 2 * NB_N - 2 * j - 1; }\n"
+    << "__device__ __forceinline__ u32 canon(u32 v) { return v >= P31 ? v - P31 : v; }\n"
+    << "#define NB_EMPTY 0xffffffffu\n"
+    << "__device__ __forceinline__ u32 khash(u32 rel, u32 len, const u32* v) {\n"
+    << "  u64 h = ((u64)rel << 32 | len) * 0x9E3779B97F4A7C15ull;\n"
+    << "  for (u32 i = 0; i < len; ++i) { h = (h ^ v[i]) * 0x9E3779B97F4A7C15ull; h ^= h >> 31; }\n"
+    << "  return (u32)(h >> 32);\n}\n"
+    // a key is rel, len, values: kw words per bin
+    // the build reads keys other threads of the same launch wrote (through L2: __ldcg); the probe reads a finished table (__ldg)
+    << "__device__ __forceinline__ bool ksame_cg(const u32* k, u32 rel, u32 len, const u32* v) {\n"
+    << "  if (__ldcg(k) != rel || __ldcg(k + 1) != len) return false;\n"
+    << "  for (u32 i = 0; i < len; ++i) if (__ldcg(k + 2 + i) != v[i]) return false;\n  return true;\n}\n"
+    << "__device__ __forceinline__ bool ksame(const u32* k, u32 rel, u32 len, const u32* v) {\n"
+    << "  if (__ldg(k) != rel || __ldg(k + 1) != len) return false;\n"
+    << "  for (u32 i = 0; i < len; ++i) if (__ldg(k + 2 + i) != v[i]) return false;\n  return true;\n}\n"
+    << "__device__ __noinline__ void nb_insert(u32 rel, u32 len, const u32* v, u32 bin, u32* slots, u32* keys, u32 kw, u32 mask, u32* err) {\n"
+    << "  u32* k = keys + (u64)bin * kw;\n"
+    << "  k[0] = rel; k[1] = len; for (u32 i = 0; i < len; ++i) k[2 + i] = v[i];\n"
+    << "  __threadfence();   // the key is visible before the slot that names it\n"
+    << "  for (u32 s = khash(rel, len, v) & mask;; s = (s + 1) & mask) {\n"
+    << "    const u32 prev = atomicCAS(slots + s, NB_EMPTY, bin);\n"
+    << "    if (prev == NB_EMPTY) return;\n"
+    << "    if (ksame_cg(keys + (u64)prev * kw, rel, len, v)) { atomicOr(err, 1u); return; }   // the same tuple in two rows: ambiguous\n"
+    << "  }\n}\n"
+    << "__device__ __noinline__ void nb_lookup(u32 rel, u32 len, const u32* v, u32 num, u64 tag, u32 pos, const u32* __restrict__ slots,\n"
+    << "    const u32* __restrict__ keys, u32 kw, u32 mask, u64* cnt, u32* sh, u64* um) {\n"
+    << "  u32 bin = NB_EMPTY;\n"
+    << "  for (u32 s = khash(rel, len, v) & mask;; s = (s + 1) & mask) {\n"
+    << "    const u32 e = __ldg(slots + s);\n"
+    << "    if (e == NB_EMPTY) break;\n"
+    << "    if (ksame(keys + (u64)e * kw, rel, len, v)) { bin = e; break; }\n"
+    << "  }\n"
+    << "  const bool bad = bin == NB_EMPTY;\n"
+    // a private bin is two u32 words (low, high) in shared memory: a 64-bit shared add would be a CAS loop, a 32-bit one is one ATOMS.ADD;
+    // the thread whose add wraps the low word carries into the high one
+    << "  if (!bad) {\n"
+    << "    if (sh) { if (atomicAdd(sh + 2 * bin, num) + num < num) atomicAdd(sh + 2 * bin + 1, 1u); }\n"
+    << "    else atomicAdd(cnt + bin, (u64)num);\n  }\n"
+    // the check kernel's warp aggregation; the 64-bit minimum as two 32-bit ones (threads of other call sites may share the warp)
+    << "  const unsigned am = __activemask();\n"
+    << "  const unsigned m = __ballot_sync(am, bad);\n"
+    << "  if (m) {\n"
+    << "    const u64 key = bad ? (tag | pos_to_row(pos)) : ~0ull;\n"
+    << "    const u32 hi = __reduce_min_sync(am, (u32)(key >> 32));\n"
+    << "    const u32 lo = __reduce_min_sync(am, (u32)(key >> 32) == hi ? (u32)key : 0xffffffffu);\n"
+    << "    if ((threadIdx.x & 31u) == (u32)(__ffs(am) - 1)) { atomicAdd(um, (u64)__popc(m)); atomicMin(um + 1, (u64)hi << 32 | lo); }\n"
+    << "  }\n}\n";
+  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
+  const std::vector<AirInstr>& prog = c.logup_prog;
+  std::vector<int> da, db;
+  prog_defs(prog, c.lg_base_regs, c.lg_ext_regs, da, db);
+  auto x = [](int q) { return "x" + std::to_string(q); };
+  // the statements computing the base values at positions `roots`, with everything they read, in program order
+  auto emit_values = [&](std::ostringstream& s, const std::vector<int>& roots) {
+    std::vector<char> need(prog.size(), 0);
+    std::vector<int> st(roots.begin(), roots.end());
+    while (!st.empty()) {
+      const int q = st.back(); st.pop_back();
+      if (q < 0 || need[q]) continue;
+      need[q] = 1;
+      st.push_back(da[q]);
+      if (prog[q].op != OP_NEGB) st.push_back(db[q]);
+    }
+    for (size_t q = 0; q < prog.size(); ++q) {
+      if (!need[q]) continue;
+      const AirInstr& in = prog[q];
+      s << "  const u32 " << x((int)q) << " = ";
+      switch (in.op) {
+        case OP_LOADM: s << "__ldg(ccols[" << in.a << "] + pos)"; break;
+        case OP_CONSTB: s << in.a << "u"; break;
+        case OP_ADDB: s << "add(" << x(da[q]) << ", " << x(db[q]) << ")"; break;
+        case OP_SUBB: s << "sub(" << x(da[q]) << ", " << x(db[q]) << ")"; break;
+        case OP_MULB: s << "mul(" << x(da[q]) << ", " << x(db[q]) << ")"; break;
+        case OP_NEGB: s << "neg(" << x(da[q]) << ")"; break;
+        default: s << "0u"; break;   // unreachable: air_lookup_tables takes tuples and numerators from base values only
+      }
+      s << ";\n";
+    }
+  };
+  auto tuple = [&](const AirFrac& f) {
+    std::ostringstream s;
+    s << "const u32 v[" << f.tuple.size() << "] = {";
+    for (size_t i = 0; i < f.tuple.size(); ++i) s << (i ? ", " : "") << "canon(" << x(f.tuple[i]) << ")";
+    s << "};";
+    return s.str();
+  };
+  const size_t CH = 64;   // fractions per __noinline__ chunk: NVVM's time grows faster than the function
+  std::vector<size_t> tables, lookups;
+  for (size_t i = 0; i < fr.size(); ++i) {
+    if (fr[i].kind == FRAC_TABLE) tables.push_back(i);
+    if (fr[i].kind == FRAC_LOOKUP) lookups.push_back(i);
+  }
+  u32 t_index = 0;
+  std::map<size_t, u32> t_of;
+  for (size_t i : tables) t_of[i] = t_index++;
+  const size_t nbc = (tables.size() + CH - 1) / CH, npc = (lookups.size() + CH - 1) / CH;
+  for (size_t ci = 0; ci < nbc; ++ci) {
+    o << "__device__ __noinline__ void bchunk" << ci << "(u32 pos, const u32* __restrict__ tbase, u32* slots, u32* keys, u32 kw, u32 mask, u32* err) {\n";
+    std::vector<int> roots;
+    for (size_t j = ci * CH; j < std::min(tables.size(), (ci + 1) * CH); ++j) for (int v : fr[tables[j]].tuple) roots.push_back(v);
+    emit_values(o, roots);
+    for (size_t j = ci * CH; j < std::min(tables.size(), (ci + 1) * CH); ++j) {
+      const AirFrac& f = fr[tables[j]];
+      o << "  { " << tuple(f) << " nb_insert(" << f.rel << "u, " << f.tuple.size() << "u, v, __ldg(tbase + " << t_of[tables[j]] << ") + pos, slots, keys, kw, mask, err); }\n";
+    }
+    o << "}\n";
+  }
+  for (size_t ci = 0; ci < npc; ++ci) {
+    o << "__device__ __noinline__ void pchunk" << ci << "(u32 pos, u64 ctag, const u32* __restrict__ slots, const u32* __restrict__ keys, u32 kw, u32 mask, u64* cnt, u32* sh, u64* um) {\n";
+    std::vector<int> roots;
+    for (size_t j = ci * CH; j < std::min(lookups.size(), (ci + 1) * CH); ++j) {
+      for (int v : fr[lookups[j]].tuple) roots.push_back(v);
+      roots.push_back(fr[lookups[j]].num);
+    }
+    emit_values(o, roots);
+    for (size_t j = ci * CH; j < std::min(lookups.size(), (ci + 1) * CH); ++j) {
+      const AirFrac& f = fr[lookups[j]];
+      o << "  { const u32 n = canon(" << x(f.num) << "); if (n) { " << tuple(f) << " nb_lookup(" << f.rel << "u, " << f.tuple.size() << "u, v, n, ctag | "
+        << lookups[j] << "ull << 28, pos, slots, keys, kw, mask, cnt, sh, um); } }\n";
+    }
+    o << "}\n";
+  }
+  // one launch per mode; rows by a grid-stride loop (the probe's private bins are zeroed and flushed once per CTA)
+  o << "extern __shared__ u32 nbsh[];   // 2 words per private bin\n"
+    << "extern \"C\" __global__ void __launch_bounds__(256) nbjit(u32 mode, u32 comp, const u32* __restrict__ tbase, u32* slots, u32* keys, u32 kw, u32 mask,\n"
+    << "    u64* cnt, u32 nsh, u64* um, u32* err) {\n"
+    << "  const u32 stride = gridDim.x * blockDim.x;\n"
+    << "  if (mode == 0) {\n"
+    << "    for (u32 pos = blockIdx.x * blockDim.x + threadIdx.x; pos < NB_N; pos += stride) {\n";
+  for (size_t ci = 0; ci < nbc; ++ci) o << "      bchunk" << ci << "(pos, tbase, slots, keys, kw, mask, err);\n";
+  o << "    }\n    return;\n  }\n"
+    << "  u32* sh = nsh ? nbsh : nullptr;\n"
+    << "  for (u32 i = threadIdx.x; i < 2 * nsh; i += blockDim.x) nbsh[i] = 0u;\n"
+    << "  if (nsh) __syncthreads();\n"
+    << "  const u64 ctag = (u64)comp << 48;\n"
+    << "  for (u32 pos = blockIdx.x * blockDim.x + threadIdx.x; pos < NB_N; pos += stride) {\n";
+  for (size_t ci = 0; ci < npc; ++ci) o << "    pchunk" << ci << "(pos, ctag, slots, keys, kw, mask, cnt, sh, um);\n";
+  o << "  }\n"
+    << "  if (nsh) {\n    __syncthreads();\n"
+    << "    for (u32 i = threadIdx.x; i < nsh; i += blockDim.x) {\n"
+    << "      const u64 v = (u64)nbsh[2 * i + 1] << 32 | nbsh[2 * i];\n"
+    << "      if (v) atomicAdd(cnt + i, v);\n    }\n  }\n}\n";
+  return o.str();
+}
 }  // namespace
 
 std::string jit_source(const AirComponent& c, bool d2) { return gen_source(c, d2); }
 std::string jit_logup_source(const AirComponent& c) { return gen_logup_source(c); }
 std::string jit_check_source(const AirComponent& c) { return gen_check_source(c); }
+std::string jit_count_source(const AirComponent& c, const std::vector<AirFrac>& fr) { return gen_count_source(c, fr); }
 
 bool jit_enabled() {
   const char* e = getenv("NB200_JIT");
@@ -631,6 +772,9 @@ static nb200_status jit_compile_source(nb200_ctx* ctx, const AirComponent& c, co
 nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, bool d2, JitKernel* out) { return jit_compile_source(ctx, c, gen_source(c, d2), out); }
 nb200_status jit_compile_logup(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_logup_source(c), out); }
 nb200_status jit_compile_check(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_check_source(c), out); }
+nb200_status jit_compile_count(nb200_ctx* ctx, const AirComponent& c, const std::vector<AirFrac>& fr, JitKernel* out) {
+  return jit_compile_source(ctx, c, gen_count_source(c, fr), out);
+}
 // ---- cubin cache: <directory of this library>/jit_cache/<key>.cubin (or $NB200_JIT_CACHE).  `python -m nexus_zkvm_b200.build`
 // fills it for the shipped machines with nvcc, so a fresh box neither loads libnvrtc nor compiles; kernels compiled at run time are
 // added when the directory is writable.  The key covers the generated source and the target; the D2 variant of a constraint kernel
@@ -756,6 +900,21 @@ nb200_status jit_launch_check(nb200_ctx* ctx, const JitKernel& jk, const u32* co
   NB_TRY(jit_set_cols(ctx, jk, d_cols));
   void* args[] = {(void*)&d_params, (void*)&d_nfail, (void*)&d_first};
   cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)((rows + block - 1) / block)), dim3(block), args, 0, ctx->stream);
+  ctx->launches += 1;
+  if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
+  return NB200_OK;
+}
+
+nb200_status jit_launch_count(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const CountArgs& a) {
+  // rows by a grid-stride loop: at most 8 CTAs per SM, so that the probe's private bins are zeroed and flushed a bounded number of times
+  const size_t rows = (size_t)1 << jk.log_size;
+  const u32 block = (u32)std::min<size_t>(rows, 256);
+  const u32 grid = (u32)std::min<size_t>((rows + block - 1) / block, (size_t)ctx->sm_count * 8);
+  NB_TRY(jit_set_cols(ctx, jk, d_cols));
+  CountArgs v = a;
+  void* args[] = {(void*)&v.mode, (void*)&v.comp, (void*)&v.tbase, (void*)&v.slots, (void*)&v.keys, (void*)&v.kw, (void*)&v.mask,
+                  (void*)&v.cnt, (void*)&v.nsh, (void*)&v.um, (void*)&v.err};
+  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3(grid), dim3(block), args, a.mode ? (size_t)a.nsh * 8 : 0, ctx->stream);
   ctx->launches += 1;
   if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
   return NB200_OK;

@@ -40,6 +40,21 @@ std::string jit_logup_source(const AirComponent& c);
 std::string jit_check_source(const AirComponent& c);
 nb200_status jit_compile_check(nb200_ctx* ctx, const AirComponent& c, JitKernel* out);
 nb200_status jit_launch_check(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, u32* d_nfail, u32* d_first);
+// the table-multiplicity count (jit.cu gen_count_source): mode 0 builds the hash of the component's table tuples, mode 1 counts its lookups
+std::string jit_count_source(const AirComponent& c, const std::vector<AirFrac>& fr);
+nb200_status jit_compile_count(nb200_ctx* ctx, const AirComponent& c, const std::vector<AirFrac>& fr, JitKernel* out);
+struct CountArgs {
+  u32 mode = 0, comp = 0;
+  const u32* tbase = nullptr;           // bin of row 0 of each of the component's table fractions
+  u32* slots = nullptr;                 // hash slots (bin or 0xffffffff), mask + 1 of them
+  u32* keys = nullptr;                  // kw words per bin: relation, tuple length, values
+  u32 kw = 0, mask = 0;
+  unsigned long long* cnt = nullptr;    // u64 counter per bin
+  u32 nsh = 0;                          // > 0: the probe counts into nsh bins in shared memory (all bins), flushed once per CTA
+  unsigned long long* um = nullptr;     // unmatched: count, smallest (component << 48 | fraction << 28 | row)
+  u32* err = nullptr;                   // build: nonzero when a tuple is in two rows of one relation
+};
+nb200_status jit_launch_count(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const CountArgs& a);
 nb200_status jit_launch_constraints(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, const u32* d_coeff,
                                     const u32* d_dinv, u32* const acc[4], u32 rows_log, u32 dom_log, u32 row0 = 0, size_t n_rows = 0,
                                     u32* const acc_high[4] = nullptr);

@@ -313,6 +313,18 @@ nb200_status add_inplace(nb200_ctx* ctx, u32* a, const u32* b, size_t n) {
   return NB200_OK;
 }
 
+// ---- table multiplicities (nb200_table_multiplicities): a table fraction's column (finalized order) = its bins' u64 counters mod P ----
+__global__ void table_mult_store_kernel(u32* __restrict__ dst, const unsigned long long* __restrict__ cnt, size_t n) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dst[i] = (u32)(cnt[i] % P31);
+}
+nb200_status table_mult_store(nb200_ctx* ctx, u32* dst, const unsigned long long* cnt, size_t n) {
+  u32 thr = 256;
+  table_mult_store_kernel<<<(u32)((n + thr - 1) / thr), thr, 0, ctx->stream>>>(dst, cnt, n);
+  NB_LAUNCH_CHECK(ctx);
+  return NB200_OK;
+}
+
 // a[i] = (a[i] - b[i]) / t, t = the top-layer (line layer tw_log - 1) twiddle of CanonicCoset(tw_log)'s FFT on the first half of the domain.
 // Used to split a polynomial of 2^tw_log coefficients into its low and high halves from evaluations on two half-size domains (prove.cu).
 __global__ void sub_scale_kernel(u32* __restrict__ a, const u32* __restrict__ b, size_t n, const u32* __restrict__ itw_top) {

@@ -23,7 +23,9 @@ struct nb200_air {
   std::vector<nb::JitKernel> jit_d2;     // its constraints of degree above AIR_LOW_DEGREE (D2 of the half-domain route)
   std::vector<nb::JitKernel> jit_logup;  // logup (interaction trace) program
   std::vector<nb::JitKernel> jit_check;  // constraint check on the trace domain (nb200_check_constraints)
-  ~nb200_air() { for (auto* v : {&jit, &jit_d2, &jit_logup, &jit_check}) for (auto& j : *v) nb::jit_release(j); }
+  std::vector<nb::JitKernel> jit_count;  // table-multiplicity build / probe (nb200_table_multiplicities)
+  std::vector<std::vector<nb::AirFrac>> fracs;   // every component's fractions as tables, lookups or neither (air_lookup_tables)
+  ~nb200_air() { for (auto* v : {&jit, &jit_d2, &jit_logup, &jit_check, &jit_count}) for (auto& j : *v) nb::jit_release(j); }
 };
 
 namespace nb {
@@ -81,9 +83,10 @@ static nb200_status upload_params(nb200_ctx* ctx, const void* params, size_t n_p
 // `interp_fallback`: the caller can run the bytecode interpreter, so programs shorter than JIT_MIN_INSTR are not compiled and a failed
 // compile is only logged (NB200_TRACE).  The sharded row kernels and the constraint check have no interpreter: they try every program and
 // reject a nullptr.
-enum JitKind { JIT_CONSTRAINTS, JIT_D2, JIT_LOGUP, JIT_CHECK };
+enum JitKind { JIT_CONSTRAINTS, JIT_D2, JIT_LOGUP, JIT_CHECK, JIT_COUNT };
 static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp_idx, JitKind kind, bool interp_fallback) {
-  std::vector<JitKernel>& v = kind == JIT_CHECK ? air_h->jit_check : kind == JIT_LOGUP ? air_h->jit_logup : kind == JIT_D2 ? air_h->jit_d2 : air_h->jit;
+  std::vector<JitKernel>& v = kind == JIT_COUNT ? air_h->jit_count : kind == JIT_CHECK ? air_h->jit_check : kind == JIT_LOGUP ? air_h->jit_logup
+                            : kind == JIT_D2 ? air_h->jit_d2 : air_h->jit;
   if (v.size() != air_h->prog.comps.size()) v.resize(air_h->prog.comps.size());
   JitKernel& jk = v[comp_idx];
   if (!jk.tried) {
@@ -91,7 +94,8 @@ static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp
     const AirComponent& c = air_h->prog.comps[comp_idx];
     const bool worth_it = kind == JIT_LOGUP ? (c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0) : c.prog.size() >= JIT_MIN_INSTR;
     if ((worth_it || !interp_fallback) && jit_enabled()) {
-      nb200_status st = kind == JIT_CHECK ? jit_compile_check(ctx, c, &jk)
+      nb200_status st = kind == JIT_COUNT ? jit_compile_count(ctx, c, air_h->fracs[comp_idx], &jk)
+                      : kind == JIT_CHECK ? jit_compile_check(ctx, c, &jk)
                       : kind == JIT_LOGUP ? jit_compile_logup(ctx, c, &jk) : jit_compile_constraints(ctx, c, kind == JIT_D2, &jk);
       if (st != NB200_OK) jk.err = ctx->err;   // kept with the kernel: a later call that finds it missing reports why
       if (interp_fallback) {
@@ -1295,6 +1299,137 @@ nb200_status check_constraints(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, c
   return NB200_OK;
 }
 
+// Every table fraction's multiplicity column, counted on the GPU from the AIR's own lookups (air_lookup_tables, jit.cu gen_count_source).
+// Each row of each table fraction is a bin (tables in component then fraction order, rows in finalized order).  The build kernels hash
+// every table tuple to its bin, the probe kernels add every lookup's numerator to its tuple's bin, and the bins are written mod P into the
+// multiplicity columns of tree 1, in place.
+nb200_status table_multiplicities(nb200_ctx* ctx, nb200_air* air_h, const nb200_cols* const* const trees[2], const size_t n_trees[2],
+                                  uint64_t* n_unmatched, uint32_t first[3]) {
+  const AirProgram& air = air_h->prog;
+  const std::vector<std::vector<AirFrac>>& fr = air_h->fracs;
+  std::vector<std::vector<u32*>> flat(2);
+  std::vector<std::vector<u32>> flog(2);
+  for (int t = 0; t < 2; ++t)
+    for (size_t b = 0; b < n_trees[t]; ++b) {
+      NB_ARG(ctx, trees[t][b], "table_multiplicities: null batch");
+      for (size_t k = 0; k < trees[t][b]->n_cols; ++k) { flat[t].push_back(trees[t][b]->col(k)); flog[t].push_back(trees[t][b]->log_size); }
+    }
+  NB_ARG(ctx, air.comps.size() < (1u << 16), "table_multiplicities: at most 2^16 - 1 components");
+  std::vector<std::vector<u32>> tbase(air.comps.size());
+  std::vector<std::pair<u32*, u32>> mult;      // bin order: (multiplicity column, log size) per table fraction
+  std::set<const u32*> mult_seen;
+  std::vector<char> builds(air.comps.size(), 0), probes(air.comps.size(), 0);
+  uint64_t n_bins = 0, additions = 0;
+  u32 max_len = 0;
+  for (size_t k = 0; k < air.comps.size(); ++k) {
+    const AirComponent& c = air.comps[k];
+    for (size_t i = 0; i < fr[k].size(); ++i) {
+      const AirFrac& f = fr[k][i];
+      const std::string where = "table_multiplicities: component " + std::to_string(k) + ", fraction " + std::to_string(i) + ": ";
+      NB_ARG(ctx, f.kind != FRAC_BAD, where + f.why);
+      if (f.kind == FRAC_TABLE) {
+        const AirMask& mk = c.masks[f.mult_mask];
+        NB_ARG(ctx, mk.col < flat[1].size() && flog[1][mk.col] == c.log_size, where + "its multiplicity column is missing from tree 1 or has another size");
+        NB_ARG(ctx, mult_seen.insert(flat[1][mk.col]).second, where + "two table fractions share a multiplicity column");
+        tbase[k].push_back((u32)n_bins);
+        mult.push_back({flat[1][mk.col], c.log_size});
+        n_bins += (uint64_t)1 << c.log_size;
+        builds[k] = 1;
+      } else if (f.kind == FRAC_LOOKUP) {
+        NB_ARG(ctx, i < (1u << 20), where + "at most 2^20 fractions per component");
+        additions += (uint64_t)1 << c.log_size;
+        probes[k] = 1;
+      } else {
+        continue;
+      }
+      max_len = std::max<u32>(max_len, (u32)f.tuple.size());
+    }
+  }
+  *n_unmatched = 0;
+  first[0] = first[1] = first[2] = UINT32_MAX;
+  if (n_bins == 0) return NB200_OK;   // no table: nothing to count
+  NB_ARG(ctx, n_bins <= (1ull << 30), "table_multiplicities: at most 2^30 table rows");
+  // a numerator is below 2^31, so a u64 bin is exact for up to 2^33 additions: more lookups than that in one call could wrap it
+  NB_ARG(ctx, additions <= (1ull << 33), "table_multiplicities: more than 2^33 lookups (rows x lookup fractions) could overflow a 64-bit counter");
+  // the columns each component's count kernel reads (trees 0 and 1; the logup program reads nothing else)
+  std::vector<const u32*> cols_all;
+  std::vector<size_t> cols_at(air.comps.size(), 0);
+  for (size_t k = 0; k < air.comps.size(); ++k) {
+    const AirComponent& c = air.comps[k];
+    cols_at[k] = cols_all.size();
+    for (const AirMask& mk : c.masks) {
+      const u32* p = nullptr;
+      if ((builds[k] || probes[k]) && mk.tree < 2) {
+        NB_ARG(ctx, mk.col < flat[mk.tree].size(), "table_multiplicities: AIR references a missing trace column");
+        NB_ARG(ctx, flog[mk.tree][mk.col] == c.log_size, "table_multiplicities: column size differs from the component's log_size");
+        p = flat[mk.tree][mk.col];
+      }
+      cols_all.push_back(p);
+    }
+  }
+  std::vector<const JitKernel*> jk(air.comps.size(), nullptr);
+  for (size_t k = 0; k < air.comps.size(); ++k) {
+    if (!builds[k] && !probes[k]) continue;
+    jk[k] = ensure_jit(ctx, air_h, k, JIT_COUNT, false);
+    if (!jk[k])
+      return set_err(ctx, NB200_ERR_STATE, jit_enabled() ? "table_multiplicities: the count kernel could not be compiled: " + air_h->jit_count[k].err
+                                                         : std::string("table_multiplicities: the count runs only as a generated kernel (NB200_JIT=0)"));
+  }
+  // hash: at most half full; keys: relation, length, values per bin
+  uint64_t cap = 1024;   // <= 2^31: the slot index and its mask fit 32 bits
+  while (cap < 2 * n_bins) cap <<= 1;
+  const u32 kw = 2 + max_len;
+  std::vector<u32> tb;
+  std::vector<size_t> tb_at(air.comps.size(), 0);
+  for (size_t k = 0; k < air.comps.size(); ++k) { tb_at[k] = tb.size(); tb.insert(tb.end(), tbase[k].begin(), tbase[k].end()); }
+  DevBuf d_slots, d_keys, d_cnt, d_um, d_err, d_tb, d_cols;
+  NB_TRY(alloc(ctx, d_slots, cap));
+  NB_TRY(alloc(ctx, d_keys, n_bins * kw));
+  NB_TRY(alloc(ctx, d_cnt, 2 * n_bins));
+  NB_TRY(alloc(ctx, d_um, 4 + 1));
+  NB_TRY(alloc(ctx, d_tb, std::max<size_t>(tb.size(), 1)));
+  NB_TRY(alloc(ctx, d_cols, std::max<size_t>(cols_all.size(), 1) * 2));
+  NB_CUDA(ctx, cudaMemsetAsync(d_slots.p, 0xff, (size_t)cap * 4, ctx->stream));
+  NB_CUDA(ctx, cudaMemsetAsync(d_cnt.p, 0, n_bins * 8, ctx->stream));
+  const uint64_t um_init[2] = {0, UINT64_MAX};
+  NB_CUDA(ctx, cudaMemcpyAsync(d_um.p, um_init, 16, cudaMemcpyHostToDevice, ctx->stream));
+  NB_CUDA(ctx, cudaMemsetAsync(d_um.p + 4, 0, 4, ctx->stream));
+  if (!tb.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_tb.p, tb.data(), tb.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+  if (!cols_all.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_cols.p, cols_all.data(), cols_all.size() * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream));
+  CountArgs a;
+  a.slots = d_slots.p; a.keys = d_keys.p; a.kw = kw; a.mask = (u32)(cap - 1);
+  a.cnt = (unsigned long long*)d_cnt.p; a.um = (unsigned long long*)d_um.p; a.err = d_um.p + 4;
+  trace_mark(ctx, nullptr);
+  for (size_t k = 0; k < air.comps.size(); ++k) {
+    if (!builds[k]) continue;
+    a.mode = 0; a.comp = (u32)k; a.tbase = d_tb.p + tb_at[k]; a.nsh = 0;
+    NB_TRY(jit_launch_count(ctx, *jk[k], (const u32* const*)d_cols.p + cols_at[k], a));
+  }
+  u32 dup = 0;
+  NB_CUDA(ctx, cudaMemcpyAsync(&dup, d_um.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // also: the host tables above have been consumed
+  if (dup) return set_err(ctx, NB200_ERR_ARG, "table_multiplicities: a table lists the same tuple in two rows of one relation");
+  // bins privatised per CTA when they fit in 32 KB of shared memory (the v1 machine's Range256 + Range32: 288 bins)
+  const u32 nsh = n_bins * 8 <= 32768 ? (u32)n_bins : 0u;
+  for (size_t k = 0; k < air.comps.size(); ++k) {
+    if (!probes[k]) continue;
+    a.mode = 1; a.comp = (u32)k; a.tbase = d_tb.p; a.nsh = nsh;
+    NB_TRY(jit_launch_count(ctx, *jk[k], (const u32* const*)d_cols.p + cols_at[k], a));
+  }
+  uint64_t bin = 0;
+  for (auto& m : mult) {
+    NB_TRY(table_mult_store(ctx, m.first, (const unsigned long long*)d_cnt.p + bin, (size_t)1 << m.second));
+    bin += (uint64_t)1 << m.second;
+  }
+  uint64_t um[2];
+  NB_CUDA(ctx, cudaMemcpyAsync(um, d_um.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  trace_mark(ctx, "table multiplicities");
+  *n_unmatched = um[0];
+  if (um[0]) { first[0] = (uint32_t)(um[1] >> 48); first[1] = (uint32_t)((um[1] >> 28) & 0xFFFFF); first[2] = (uint32_t)(um[1] & 0xFFFFFFF); }
+  return NB200_OK;
+}
+
 // LogupTraceGenerator of the sharded (main) component: this rank runs the row kernel on ITS trace rows (all columns: the row slices kept by
 // nb200_scheme_commit_sharded), the last secure column is all-gathered for the global claimed sum / coset-order prefix sum (finalize_last),
 // and one rows -> columns exchange hands every rank its COLUMN shard of the 4 * n_logup interaction columns, ready for the next sharded commit.
@@ -1424,8 +1559,9 @@ nb200_status nb200_device_channel_draw(nb200_ctx* ctx, const uint8_t digest[32],
 // ---- AIR ----
 nb200_status nb200_air_load(nb200_ctx* ctx, const uint32_t* words, size_t n_words, nb200_air** out) {
   if (!out) return NB200_ERR_ARG;
-  try { nb200_air* a = new nb200_air(); a->prog = air_parse(words, n_words); *out = a; return NB200_OK; }
-  catch (std::exception& e) { return set_err(ctx, NB200_ERR_ARG, e.what()); }
+  nb200_air* a = new nb200_air();
+  try { a->prog = air_parse(words, n_words); a->fracs = air_lookup_tables(a->prog); *out = a; return NB200_OK; }
+  catch (std::exception& e) { delete a; return set_err(ctx, NB200_ERR_ARG, e.what()); }
 }
 void nb200_air_free(nb200_air* a) { delete a; }
 uint32_t nb200_air_n_params(const nb200_air* a) { return a ? a->prog.n_params : 0; }
@@ -1535,6 +1671,41 @@ nb200_status nb200_check_constraints(nb200_ctx* ctx, const nb200_air* air, uint3
   const nb200_cols* const* trees[3] = {tree0, tree1, tree2};
   const size_t n_trees[3] = {n0, n1, n2};
   return check_constraints(ctx, const_cast<nb200_air*>(air), component, trees, n_trees, params, n_params, n_failing, first_row, n);
+}
+nb200_status nb200_table_multiplicities(nb200_ctx* ctx, const nb200_air* air, const nb200_cols* const* tree0, size_t n0, nb200_cols* const* tree1, size_t n1,
+                                        uint64_t* n_unmatched, uint32_t first_unmatched[3]) {
+  if (!ctx || !air || (n0 && !tree0) || (n1 && !tree1) || !n_unmatched || !first_unmatched) return NB200_ERR_ARG;
+  const nb200_cols* const* trees[2] = {tree0, (const nb200_cols* const*)tree1};
+  const size_t n_trees[2] = {n0, n1};
+  return table_multiplicities(ctx, const_cast<nb200_air*>(air), trees, n_trees, n_unmatched, first_unmatched);
+}
+nb200_status nb200_air_lookup_tables(const nb200_air* a, uint32_t component, uint32_t* kind, uint32_t* relation, uint32_t* arg, size_t n) {
+  if (!a || component >= a->prog.comps.size()) return NB200_ERR_ARG;
+  const std::vector<AirFrac>& fr = a->fracs[component];
+  if (n != fr.size() || (n && (!kind || !relation || !arg))) return NB200_ERR_ARG;
+  const AirComponent& c = a->prog.comps[component];
+  for (size_t i = 0; i < n; ++i) {
+    kind[i] = fr[i].kind;
+    relation[i] = fr[i].rel;
+    arg[i] = fr[i].kind == FRAC_TABLE ? c.masks[fr[i].mult_mask].col : (u32)fr[i].tuple.size();
+  }
+  return NB200_OK;
+}
+nb200_status nb200_air_count_kernel_source(const nb200_air* a, uint32_t component, char** out) {
+  if (!a || !out || component >= a->prog.comps.size()) return NB200_ERR_ARG;
+  *out = nullptr;
+  bool any = false;
+  for (const AirFrac& f : a->fracs[component]) {
+    if (f.kind == FRAC_BAD) return NB200_ERR_ARG;
+    any = any || f.kind == FRAC_TABLE || f.kind == FRAC_LOOKUP;
+  }
+  if (!any) return NB200_ERR_STATE;   // neither a table nor a lookup: nothing to count
+  const std::string src = jit_count_source(a->prog.comps[component], a->fracs[component]);
+  char* o = (char*)malloc(src.size() + 1);
+  if (!o) return NB200_ERR_OOM;
+  memcpy(o, src.c_str(), src.size() + 1);
+  *out = o;
+  return NB200_OK;
 }
 
 // ---- backend-trait level operations (the per-trait surface a `CudaBackend` shim binds; the coarse nb200_prove runs the same code) ----

@@ -148,6 +148,15 @@ impl Context {
                                                     t[2].as_ptr(), t[2].len(), p.as_ptr(), params.len(), failing.as_mut_ptr(), first.as_mut_ptr(), n) })?;
         Ok((0..n).filter(|&k| failing[k] != 0).map(|k| (k, failing[k], first[k])).collect())
     }
+    /// Overwrite every lookup table's multiplicity column in `tree1` (before tree 1 is committed) with the count of the AIR's lookups into
+    /// it, on the device.  Returns the number of lookups that match no table row and `(component, fraction, row in trace order)` of the first.
+    pub fn table_multiplicities(&self, air: &Air, tree0: &[&Columns], tree1: &mut [&mut Columns]) -> Result<(u64, Option<(u32, u32, u32)>)> {
+        let t0: Vec<*const nb200_cols> = tree0.iter().map(|c| c.h as *const _).collect();
+        let t1: Vec<*mut nb200_cols> = tree1.iter().map(|c| c.h).collect();
+        let (mut n, mut first) = (0u64, [u32::MAX; 3]);
+        self.check(unsafe { nb200_table_multiplicities(self.raw(), air.h, t0.as_ptr(), t0.len(), t1.as_ptr(), t1.len(), &mut n, first.as_mut_ptr()) })?;
+        Ok((n, if n == 0 { None } else { Some((first[0], first[1], first[2])) }))
+    }
 }
 
 /// `PcsConfig { pow_bits, fri_config: FriConfig { log_blowup_factor, log_last_layer_degree_bound, n_queries } }`
