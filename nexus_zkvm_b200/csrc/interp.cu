@@ -247,10 +247,10 @@ static nb200_status inclusive_scan(nb200_ctx* ctx, u32* d, size_t n) {
 }
 
 // ---- host drivers ----
-static nb200_status upload_prog(nb200_ctx* ctx, const std::vector<AirInstr>& prog, uint4** d_prog) {
-  static_assert(sizeof(AirInstr) == sizeof(uint4), "instr layout");
-  NB_CUDA(ctx, dmalloc(ctx, (void**)d_prog, prog.size() * sizeof(uint4)));
-  NB_CUDA(ctx, cudaMemcpyAsync(*d_prog, prog.data(), prog.size() * sizeof(uint4), cudaMemcpyHostToDevice, ctx->stream));
+// a host array in a new device buffer
+static nb200_status upload(nb200_ctx* ctx, const void* src, size_t bytes, DevBuf& out) {
+  NB_TRY(alloc(ctx, out, (bytes + 3) / 4));
+  NB_CUDA(ctx, cudaMemcpyAsync(out.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
   return NB200_OK;
 }
 
@@ -313,46 +313,62 @@ nb200_status constraint_eval(nb200_ctx* ctx, const AirComponent& c, const std::v
   }
   std::vector<MaskDev> hm(c.masks.size());
   for (size_t m = 0; m < hm.size(); ++m) { hm[m].ptr = mask_cols[m]; hm[m].off = c.masks[m].off; hm[m].pad = 0; }
-  uint4* d_prog = nullptr; MaskDev* d_masks = nullptr; u32 *d_coeff = nullptr, *d_dinv = nullptr;
-  NB_TRY(upload_prog(ctx, c.prog, &d_prog));
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_masks, hm.size() * sizeof(MaskDev)));
-  NB_CUDA(ctx, cudaMemcpyAsync(d_masks, hm.data(), hm.size() * sizeof(MaskDev), cudaMemcpyHostToDevice, ctx->stream));
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_coeff, coeffs.size() * 16));
-  NB_CUDA(ctx, cudaMemcpyAsync(d_coeff, coeffs.data(), coeffs.size() * 16, cudaMemcpyHostToDevice, ctx->stream));
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_dinv, dinv.size() * 4));
-  NB_CUDA(ctx, cudaMemcpyAsync(d_dinv, dinv.data(), dinv.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+  static_assert(sizeof(AirInstr) == sizeof(uint4), "instr layout");
+  DevBuf d_prog, d_masks, d_coeff, d_dinv;
+  NB_TRY(upload(ctx, c.prog.data(), c.prog.size() * sizeof(uint4), d_prog));
+  NB_TRY(upload(ctx, hm.data(), hm.size() * sizeof(MaskDev), d_masks));
+  NB_TRY(upload(ctx, coeffs.data(), coeffs.size() * 16, d_coeff));
+  NB_TRY(upload(ctx, dinv.data(), dinv.size() * 4, d_dinv));
   nb200_status st;
   const bool use_jit = jit_usable(jk, c, rows_log);
   if (row0 != 0 || n_rows != 0) NB_ARG(ctx, use_jit, "constraint_eval: a row range needs the specialised kernel");
   NB_ARG(ctx, !acc_high || use_jit, "constraint_eval: the high-degree accumulators need the specialised kernel");
   if (use_jit) {
     // NVRTC-specialised kernel (jit.cu): same arithmetic, registers instead of the shared-memory register file
-    const u32** d_cols = nullptr;
-    NB_CUDA(ctx, dmalloc(ctx, (void**)&d_cols, mask_cols.size() * sizeof(u32*)));
-    NB_CUDA(ctx, cudaMemcpyAsync(d_cols, mask_cols.data(), mask_cols.size() * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream));
     std::vector<u32> tab;
     jit_coeff_table(coeffs, tab);
-    u32* d_tab = nullptr;
-    NB_CUDA(ctx, dmalloc(ctx, (void**)&d_tab, tab.size() * 4 + 16));
-    NB_CUDA(ctx, cudaMemcpyAsync(d_tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-    st = jit_launch_constraints(ctx, *jk, d_cols, d_params, d_tab, d_dinv, acc, rows_log, dom_log, row0, n_rows, acc_high);
+    DevBuf d_tab;
+    NB_TRY(alloc(ctx, d_tab, tab.size() + 4));
+    NB_CUDA(ctx, cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    const size_t rows = n_rows ? n_rows : (size_t)1 << rows_log;
+    const u32** no_cols = nullptr;   // the generated code reads its columns from the kernel's column table
+    u32 el = dom_log;
+    u32* h[4] = {nullptr, nullptr, nullptr, nullptr};
+    if (acc_high) for (int k = 0; k < 4; ++k) h[k] = acc_high[k];
+    void* args[] = {(void*)&no_cols, (void*)&d_params, (void*)&d_tab.p, (void*)&d_dinv.p, (void*)&acc[0], (void*)&acc[1], (void*)&acc[2], (void*)&acc[3],
+                    (void*)&el, (void*)&row0, (void*)&h[0], (void*)&h[1], (void*)&h[2], (void*)&h[3]};
+    st = rows < JIT_BLOCK || rows % JIT_BLOCK != 0 ? set_err(ctx, NB200_ERR_STATE, "jit: row range too small")
+       : jit_launch(ctx, *jk, mask_cols.data(), mask_cols.size(), dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args);
     cudaStreamSynchronize(ctx->stream);
-    dfree(ctx, (void*)d_cols); dfree(ctx, d_tab);
   } else {
     InterpArgs a{};
-    a.prog = d_prog; a.n_instr = (u32)c.prog.size(); a.masks = d_masks; a.params = d_params;
+    a.prog = (const uint4*)d_prog.p; a.n_instr = (u32)c.prog.size(); a.masks = (const MaskDev*)d_masks.p; a.params = d_params;
     a.nb = c.n_base_regs; a.ne = c.n_ext_regs; a.log_size = c.log_size; a.eval_log = elog;
-    a.coeff = d_coeff; a.dinv = d_dinv;
+    a.coeff = d_coeff.p; a.dinv = d_dinv.p;
     for (int k = 0; k < 4; ++k) a.acc[k] = acc[k];
     st = launch_interp<false>(ctx, a, rows_log);
   }
   // host vectors were consumed by async copies: make sure they are done before the vectors die
   cudaStreamSynchronize(ctx->stream);
-  dfree(ctx, d_prog); dfree(ctx, d_masks); dfree(ctx, d_coeff); dfree(ctx, d_dinv);
   return st;
 }
 
 nb200_status logup_finalize_last(nb200_ctx* ctx, u32 log_size, u32* last4, qm31* claimed);
+
+// the row kernel alone on 2^rows_log rows (a rank's slice of the trace domain): out = 4 * n_logup_cols columns of 2^rows_log rows
+nb200_status logup_rows(nb200_ctx* ctx, const AirComponent& c, const std::vector<const u32*>& mask_cols, const u32* d_params, u32* d_out, u32 rows_log, const JitKernel* jk) {
+  NB_ARG(ctx, mask_cols.size() == c.masks.size() && jk && jk->kernel && jk->log_size == c.log_size, "logup_rows: needs the specialised kernel");
+  std::vector<const u32*> ptrs(c.masks.size());
+  for (size_t m = 0; m < ptrs.size(); ++m) ptrs[m] = (c.masks[m].off == 0 && c.masks[m].tree != 2) ? mask_cols[m] : nullptr;
+  // the kernel is row-local: its rows are the whole trace domain or a rank's slice of it
+  const size_t rows = (size_t)1 << rows_log;
+  const u32** no_cols = nullptr;   // the generated code reads its columns from the kernel's column table
+  void* args[] = {(void*)&no_cols, (void*)&d_params, (void*)&d_out, (void*)&rows_log};
+  nb200_status js = rows < JIT_BLOCK ? set_err(ctx, NB200_ERR_STATE, "jit: domain too small")
+                  : jit_launch(ctx, *jk, ptrs.data(), ptrs.size(), dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args);
+  cudaStreamSynchronize(ctx->stream);
+  return js;
+}
 
 // LogupTraceGenerator: fills 4 * n_logup_cols columns (bit-reversed circle-domain order) and returns the claimed sum.
 // mask_cols[m]: device pointer of mask m's trace column on the trace domain (nullptr for masks the program never reads).
@@ -364,46 +380,21 @@ nb200_status logup_generate(nb200_ctx* ctx, const AirComponent& c, const std::ve
   NB_ARG(ctx, mask_cols.size() == c.masks.size(), "logup_generate: shape");
   std::vector<MaskDev> hm(c.masks.size());
   for (size_t m = 0; m < hm.size(); ++m) { hm[m].ptr = (c.masks[m].off == 0 && c.masks[m].tree != 2) ? mask_cols[m] : nullptr; hm[m].off = 0; hm[m].pad = 0; }
-  uint4* d_prog = nullptr; MaskDev* d_masks = nullptr; u32* d_batch = nullptr;
-  NB_TRY(upload_prog(ctx, c.logup_prog, &d_prog));
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_masks, hm.size() * sizeof(MaskDev)));
-  NB_CUDA(ctx, cudaMemcpyAsync(d_masks, hm.data(), hm.size() * sizeof(MaskDev), cudaMemcpyHostToDevice, ctx->stream));
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_batch, c.batching.size() * 4));
-  NB_CUDA(ctx, cudaMemcpyAsync(d_batch, c.batching.data(), c.batching.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+  DevBuf d_prog, d_masks, d_batch;
+  NB_TRY(upload(ctx, c.logup_prog.data(), c.logup_prog.size() * sizeof(uint4), d_prog));
+  NB_TRY(upload(ctx, hm.data(), hm.size() * sizeof(MaskDev), d_masks));
+  NB_TRY(upload(ctx, c.batching.data(), c.batching.size() * 4, d_batch));
   InterpArgs a{};
-  a.prog = d_prog; a.n_instr = (u32)c.logup_prog.size(); a.masks = d_masks; a.params = d_params;
+  a.prog = (const uint4*)d_prog.p; a.n_instr = (u32)c.logup_prog.size(); a.masks = (const MaskDev*)d_masks.p; a.params = d_params;
   a.nb = c.lg_base_regs; a.ne = c.lg_ext_regs; a.log_size = c.log_size; a.eval_log = c.log_size;
-  a.batching = d_batch; a.out = d_out; a.n_batches = ncols;
-  if (jk && jk->kernel && jk->log_size == c.log_size && ((size_t)1 << c.log_size) >= JIT_BLOCK) {
+  a.batching = d_batch.p; a.out = d_out; a.n_batches = ncols;
+  if (jit_usable(jk, c, c.log_size)) {
     // NVRTC-specialised kernel (jit.cu gen_logup_source): same arithmetic as the bytecode loop below
-    std::vector<const u32*> ptrs(hm.size());
-    for (size_t m = 0; m < hm.size(); ++m) ptrs[m] = hm[m].ptr;
-    const u32** d_cols = nullptr;
-    NB_CUDA(ctx, dmalloc(ctx, (void**)&d_cols, std::max<size_t>(ptrs.size(), 1) * sizeof(u32*)));
-    NB_CUDA(ctx, cudaMemcpyAsync(d_cols, ptrs.data(), ptrs.size() * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream));
-    nb200_status js = jit_launch_logup(ctx, *jk, d_cols, d_params, d_out, c.log_size);
-    cudaStreamSynchronize(ctx->stream);
-    dfree(ctx, (void*)d_cols);
-    NB_TRY(js);
+    NB_TRY(logup_rows(ctx, c, mask_cols, d_params, d_out, c.log_size, jk));
   } else {
     NB_TRY(launch_interp<true>(ctx, a, c.log_size));
   }
-  dfree(ctx, d_prog); dfree(ctx, d_masks); dfree(ctx, d_batch);
   return logup_finalize_last(ctx, c.log_size, d_out + ((size_t)(4 * (ncols - 1)) << c.log_size), claimed);
-}
-
-// the row kernel alone on 2^rows_log rows (a rank's slice of the trace domain): out = 4 * n_logup_cols columns of 2^rows_log rows
-nb200_status logup_rows(nb200_ctx* ctx, const AirComponent& c, const std::vector<const u32*>& mask_cols, const u32* d_params, u32* d_out, u32 rows_log, const JitKernel* jk) {
-  NB_ARG(ctx, mask_cols.size() == c.masks.size() && jk && jk->kernel && jk->log_size == c.log_size, "logup_rows: needs the specialised kernel");
-  std::vector<const u32*> ptrs(c.masks.size());
-  for (size_t m = 0; m < ptrs.size(); ++m) ptrs[m] = (c.masks[m].off == 0 && c.masks[m].tree != 2) ? mask_cols[m] : nullptr;
-  const u32** d_cols = nullptr;
-  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_cols, std::max<size_t>(ptrs.size(), 1) * sizeof(u32*)));
-  NB_CUDA(ctx, cudaMemcpyAsync(d_cols, ptrs.data(), ptrs.size() * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream));
-  nb200_status js = jit_launch_logup(ctx, *jk, d_cols, d_params, d_out, rows_log);
-  cudaStreamSynchronize(ctx->stream);
-  dfree(ctx, (void*)d_cols);
-  return js;
 }
 
 // finalize_last on the FULL last secure column (4 coordinate columns of 2^log_size rows): claimed sum, shift by claimed / 2^n, prefix sum in coset order

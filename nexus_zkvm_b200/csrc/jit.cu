@@ -16,6 +16,7 @@
 #include <cstdio>
 #include <nvrtc.h>
 #include <sstream>
+#include <algorithm>
 #include <functional>
 #include <map>
 #include <cstdlib>
@@ -139,11 +140,6 @@ void emit_op(std::ostringstream& o, const AirInstr& in, Ld ld) {
   }
 }
 
-// Which virtual registers cross a chunk boundary?  live_in[ci] = registers read in chunk ci or later before they are rewritten.  A chunk loads only
-// those from the state struct and stores only the ones it wrote that a later chunk still reads: the real v1 AIR keeps 26 base + 15 secure
-// registers alive somewhere (shared selectors such as IsTypeR), and copying all 90 words in and out of local memory at each of its 19 chunk
-// boundaries cost more than the arithmetic (the synthetic ADD machine has 4 + 4 and never showed it).
-struct ChunkLive { std::vector<std::vector<u32>> in_b, in_e, out_b, out_e; };
 struct Regs { std::vector<u32> rb, re; int wb = -1, we = -1; };   // registers a statement reads and writes (base / secure)
 static Regs instr_regs(const AirInstr& in) {
   Regs r;
@@ -154,43 +150,108 @@ static Regs instr_regs(const AirInstr& in) {
   if (kd) (kd == 'b' ? r.wb : r.we) = (int)in.dst;
   return r;
 }
-// stmts[begin[ci] .. begin[ci + 1]) make up chunk ci
-static ChunkLive chunk_liveness(const std::vector<Regs>& stmts, const std::vector<size_t>& begin, u32 nb, u32 ne) {
-  const size_t n_chunks = begin.size() - 1;
+struct Stmt { std::string code; Regs r; bool effect = false; int constr = -1; };   // effect: adds constraint `constr` to rr (never removed as dead)
+template <class Ld>
+static Stmt op_stmt(const AirInstr& in, Ld ld) {
+  std::ostringstream o;
+  emit_op(o, in, ld);
+  return Stmt{o.str(), instr_regs(in)};
+}
+
+// Which virtual registers cross a chunk boundary?  in[ci] = registers read in chunk ci or later before they are rewritten.  A chunk loads only
+// those from the state struct and stores only the ones it wrote that a later chunk still reads: the real v1 AIR keeps 26 base + 15 secure
+// registers alive somewhere (shared selectors such as IsTypeR), and copying all 90 words in and out of local memory at each of its 19 chunk
+// boundaries cost more than the arithmetic (the synthetic ADD machine has 4 + 4 and never showed it).
+struct ChunkLive { std::vector<std::vector<u32>> in_b, in_e, out_b, out_e; };
+// chunk ci is the statements of program positions [ci * ch, (ci + 1) * ch)
+static ChunkLive chunk_liveness(const std::vector<std::vector<Stmt>>& at, size_t ch, u32 nb, u32 ne) {
+  const size_t n_chunks = (at.size() + ch - 1) / ch;
+  auto end = [&](size_t ci) { return std::min(at.size(), (ci + 1) * ch); };
   ChunkLive L; L.in_b.resize(n_chunks); L.in_e.resize(n_chunks); L.out_b.resize(n_chunks); L.out_e.resize(n_chunks);
   std::vector<char> lb(nb + 1, 0), le(ne + 1, 0);
   std::vector<std::vector<char>> after_b(n_chunks), after_e(n_chunks);   // live sets at the END of each chunk
   for (size_t ci = n_chunks; ci-- > 0;) {
     after_b[ci] = lb; after_e[ci] = le;
-    for (size_t pc = begin[ci + 1]; pc-- > begin[ci];) {
-      const Regs& r = stmts[pc];
-      if (r.wb >= 0) lb[r.wb] = 0;
-      if (r.we >= 0) le[r.we] = 0;
-      for (u32 x : r.rb) lb[x] = 1;
-      for (u32 x : r.re) le[x] = 1;
-    }
+    for (size_t pc = end(ci); pc-- > ci * ch;)
+      for (size_t i = at[pc].size(); i-- > 0;) {
+        const Regs& r = at[pc][i].r;
+        if (r.wb >= 0) lb[r.wb] = 0;
+        if (r.we >= 0) le[r.we] = 0;
+        for (u32 x : r.rb) lb[x] = 1;
+        for (u32 x : r.re) le[x] = 1;
+      }
     for (u32 r = 0; r < nb; ++r) if (lb[r]) L.in_b[ci].push_back(r);
     for (u32 r = 0; r < ne; ++r) if (le[r]) L.in_e[ci].push_back(r);
   }
   for (size_t ci = 0; ci < n_chunks; ++ci) {
     std::vector<char> wrb(nb + 1, 0), wre(ne + 1, 0);
-    for (size_t pc = begin[ci]; pc < begin[ci + 1]; ++pc) {
-      if (stmts[pc].wb >= 0) wrb[stmts[pc].wb] = 1;
-      if (stmts[pc].we >= 0) wre[stmts[pc].we] = 1;
-    }
+    for (size_t pc = ci * ch; pc < end(ci); ++pc)
+      for (const Stmt& st : at[pc]) {
+        if (st.r.wb >= 0) wrb[st.r.wb] = 1;
+        if (st.r.we >= 0) wre[st.r.we] = 1;
+      }
     for (u32 r = 0; r < nb; ++r) if (wrb[r] && after_b[ci][r]) L.out_b[ci].push_back(r);
     for (u32 r = 0; r < ne; ++r) if (wre[r] && after_e[ci][r]) L.out_e[ci].push_back(r);
   }
   return L;
 }
-// one statement per instruction, chunks of CH instructions
-static ChunkLive prog_liveness(const std::vector<AirInstr>& prog, size_t CH, u32 nb, u32 ne) {
-  std::vector<Regs> regs;
-  for (const AirInstr& in : prog) regs.push_back(instr_regs(in));
-  std::vector<size_t> begin;
-  for (size_t pc = 0; pc < prog.size(); pc += CH) begin.push_back(pc);
-  begin.push_back(prog.size());
-  return chunk_liveness(regs, begin, nb, ne);
+
+// column base pointers live in constant memory (filled before every launch, jit_launch): an access costs no pointer load from global memory
+// (the real AIR reads 2765 mask values per row: one dependent global load less per value)
+static std::string ccols_decl(const AirComponent& c) {
+  return "#define NB_NMASKS " + std::to_string(c.masks.size()) + "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
+}
+
+// The kernel the constraint (D1 and D2), LogUp and check programs are generated as.  at[pc] holds the statements of program position pc; the
+// positions are cut into __noinline__ chunks of `ch`, each of which loads the registers it reads from the state struct St and stores the ones
+// a later chunk reads (chunk_liveness).  A chunk without code is left out.  The strings are the parts that differ between the programs.
+struct ChunkedKernel {
+  size_t ch = 0;
+  u32 nb = 0, ne = 0;      // base / secure registers
+  std::string state;       // St's fields after the registers
+  std::string decls;       // between the column table and the first chunk
+  std::string params;      // a chunk's parameters after St& s
+  std::string enter;       // the end of a chunk's first line: its state fields loaded from s
+  std::string leave;       // a chunk's last lines: its state fields stored back
+  std::string last;        // lines at the end of the last chunk, before its stores
+  std::string sig;         // nbjit's parameters
+  std::string prologue;    // nbjit's lines before St s
+  std::string init;        // nbjit's lines after the registers are zeroed
+  std::string args;        // a chunk call's arguments after s
+  std::string epilogue;    // nbjit's lines after the last chunk
+};
+static void emit_chunked(std::ostringstream& o, const AirComponent& c, const std::vector<std::vector<Stmt>>& at, const ChunkedKernel& k) {
+  const size_t n_chunks = (at.size() + k.ch - 1) / k.ch;
+  const ChunkLive live = chunk_liveness(at, k.ch, k.nb, k.ne);
+  o << "struct St { u32 b[" << k.nb << "]; Q e[" << k.ne << "];" << k.state << " };\n" << ccols_decl(c) << k.decls;
+  std::vector<char> has_code(n_chunks, 0);   // the D2 kernel leaves out most statements
+  for (size_t pc = 0; pc < at.size(); ++pc)
+    for (const Stmt& st : at[pc]) if (!st.code.empty()) has_code[pc / k.ch] = 1;
+  for (size_t ci = 0; ci < n_chunks; ++ci) {
+    if (!has_code[ci]) continue;
+    o << "__device__ __noinline__ void chunk" << ci << "(St& s, " << k.params << ") {\n";
+    o << "  u32 b[" << k.nb << "]; Q e[" << k.ne << "];" << k.enter << "\n";
+    for (u32 r : live.in_b[ci]) o << "  b[" << r << "] = s.b[" << r << "];";
+    for (u32 r : live.in_e[ci]) o << "  e[" << r << "] = s.e[" << r << "];";
+    o << "\n";
+    for (size_t pc = ci * k.ch; pc < std::min(at.size(), (ci + 1) * k.ch); ++pc) {
+      o << "  ";
+      for (size_t i = 0; i < at[pc].size(); ++i) o << (i ? " " : "") << at[pc][i].code;
+      o << "\n";
+    }
+    if (ci + 1 == n_chunks) o << k.last;
+    for (u32 r : live.out_b[ci]) o << "  s.b[" << r << "] = b[" << r << "];";
+    for (u32 r : live.out_e[ci]) o << "  s.e[" << r << "] = e[" << r << "];";
+    o << "\n" << k.leave << "}\n";
+  }
+  // The CTAs re-converge (__syncthreads) after every chunk: the warps of a CTA then execute the same few tens of KB of straight-line
+  // code at a time and the instruction cache serves them from one fetch.  Without the barriers the warps drift apart over the ~0.7 MB
+  // program and the kernel becomes instruction-fetch bound.
+  o << "extern \"C\" __global__ void __launch_bounds__(" << JIT_BLOCK << ", 1) nbjit(" << k.sig << ") {\n" << k.prologue << "  St s;\n"
+    << "  for (int i = 0; i < " << k.nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << k.ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n" << k.init;
+  for (size_t ci = 0; ci < n_chunks; ++ci)
+    if (has_code[ci]) o << "  chunk" << ci << "(s, " << k.args << ");\n  __syncthreads();\n";
+  o << k.epilogue << "}\n";
 }
 
 // ---- folding the random coefficient into LogUp denominators
@@ -206,7 +267,6 @@ static ChunkLive prog_liveness(const std::vector<AirInstr>& prog, size_t CH, u32
 // The den's own terms and partial sums may be shared with other constraints (air.py merges equal nodes), so they are not scaled in
 // place: coeff * den is summed afresh at the MULE from the base values the den read, and a base value whose register is rewritten
 // before that point is first copied to a register of its own.  Whatever only the folded dens read is then dropped as dead code.
-struct Stmt { std::string code; Regs r; bool effect = false; int constr = -1; };   // effect: adds constraint `constr` to rr (never removed as dead)
 struct ConstraintPlan {
   std::vector<std::vector<Stmt>> at;               // the statements emitted at each program position
   u32 nb = 0;                                      // base registers, the copies of folded base values included
@@ -365,79 +425,50 @@ std::string gen_source(const AirComponent& c, bool d2) {
   };
   const std::vector<char> high = high_constraints(c);
   ConstraintPlan pl = plan_constraints(c, ld, c.n_base_regs ? c.n_base_regs : 1, ne, d2 ? high : std::vector<char>(c.n_constraints, 1));
-  const u32 nb = pl.nb;
   // rh: the high constraints' part of rr, taken as the change of rr across their statements (no products of its own)
   const bool track_high = !d2 && count_high(high) > 0;
   if (track_high)
     for (auto& at : pl.at)
       for (Stmt& st : at)
         if (st.effect && high[st.constr]) st.code = "{ const Q r0 = rr; " + st.code + " rh = qadd(rh, qsub(rr, r0)); }";
-  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; Q rr;" << (track_high ? " Q rh;" : "") << " };\n";
-  // column base pointers live in constant memory (filled before every launch): an access costs no pointer load from global memory
-  // (the real AIR reads 2765 mask values per row: one dependent global load less per value)
-  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
+  ChunkedKernel kk;
+  kk.ch = 250; kk.nb = pl.nb; kk.ne = ne;
+  kk.state = track_high ? " Q rr; Q rh;" : " Q rr;";
   if (!pl.slots.empty()) {
     // the folded products coeff_k * params[p]: (k, p) per slot, and their values, computed by each CTA before the first chunk
-    o << "#ifndef __CUDACC__\n#define __shared__\n#endif\n#define NB_NFOLD " << pl.slots.size() << "\n__constant__ const uint2 nbfold_src[NB_NFOLD] = {";
-    for (size_t i = 0; i < pl.slots.size(); ++i) o << (i ? ", " : "") << "{" << pl.slots[i].first << "u, " << pl.slots[i].second << "u}";
-    o << "};\n__shared__ uint4 nbfold[NB_NFOLD];\n"
+    std::ostringstream d;
+    d << "#ifndef __CUDACC__\n#define __shared__\n#endif\n#define NB_NFOLD " << pl.slots.size() << "\n__constant__ const uint2 nbfold_src[NB_NFOLD] = {";
+    for (size_t i = 0; i < pl.slots.size(); ++i) d << (i ? ", " : "") << "{" << pl.slots[i].first << "u, " << pl.slots[i].second << "u}";
+    d << "};\n__shared__ uint4 nbfold[NB_NFOLD];\n"
       << "__device__ __forceinline__ Q ldf(u32 i) { const uint4 v = nbfold[i]; return Q{v.x, v.y, v.z, v.w}; }\n"
       << "__device__ __forceinline__ Q qmacq(Q acc, Q x, Q y) {\n"
       << "  u32 gp = add(add(y.c3, y.c3), y.c2), g = sub(add(y.c2, y.c2), y.c3);\n"
       << "  return qmac(acc, x, y.c0, y.c1, y.c2, y.c3, P31 - y.c1, P31 - y.c3, g, gp, P31 - gp);\n}\n";
+    kk.decls = d.str();
   }
-  const size_t CH = 250;
-  const size_t n_chunks = (c.prog.size() + CH - 1) / CH;
-  std::vector<Regs> regs;
-  std::vector<size_t> begin;
-  for (size_t pc = 0; pc < c.prog.size(); ++pc) {
-    if (pc % CH == 0) begin.push_back(regs.size());
-    for (const Stmt& st : pl.at[pc]) regs.push_back(st.r);
-  }
-  begin.push_back(regs.size());
-  const ChunkLive live = chunk_liveness(regs, begin, nb, ne);
-  std::vector<char> has_code(n_chunks, 0);   // the D2 kernel leaves out most statements: chunks left empty are not emitted
-  for (size_t pc = 0; pc < c.prog.size(); ++pc)
-    for (const Stmt& st : pl.at[pc]) if (!st.code.empty()) has_code[pc / CH] = 1;
-  for (size_t ci = 0; ci < n_chunks; ++ci) {
-    if (!has_code[ci]) continue;
-    o << "__device__ __noinline__ void chunk" << ci << "(St& s, const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff, u32 row, u32 EL) {\n";
-    o << "  u32 b[" << nb << "]; Q e[" << ne << "]; Q rr = s.rr;" << (track_high ? " Q rh = s.rh;" : "") << "\n";
-    for (u32 r : live.in_b[ci]) o << "  b[" << r << "] = s.b[" << r << "];";
-    for (u32 r : live.in_e[ci]) o << "  e[" << r << "] = s.e[" << r << "];";
-    o << "\n";
-    for (size_t pc = ci * CH; pc < std::min(c.prog.size(), (ci + 1) * CH); ++pc) {
-      o << "  ";
-      for (size_t i = 0; i < pl.at[pc].size(); ++i) o << (i ? " " : "") << pl.at[pc][i].code;
-      o << "\n";
-    }
-    for (u32 r : live.out_b[ci]) o << "  s.b[" << r << "] = b[" << r << "];";
-    for (u32 r : live.out_e[ci]) o << "  s.e[" << r << "] = e[" << r << "];";
-    o << "\n  s.rr = rr;" << (track_high ? " s.rh = rh;" : "") << "\n}\n";
-  }
-  // The CTAs re-converge (__syncthreads) after every chunk: the warps of a CTA then execute the same few tens of KB of straight-line
-  // code at a time and the instruction cache serves them from one fetch.  Without the barriers the warps drift apart over the ~0.7 MB
-  // program and the kernel becomes instruction-fetch bound.
-  o << "extern \"C\" __global__ void __launch_bounds__(" << JIT_BLOCK << ", 1) nbjit(const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff,\n"
-    << "    const u32* __restrict__ dinv, u32* __restrict__ a0, u32* __restrict__ a1, u32* __restrict__ a2, u32* __restrict__ a3, u32 EL, u32 row0,\n"
-    << "    u32* __restrict__ h0 = nullptr, u32* __restrict__ h1 = nullptr, u32* __restrict__ h2 = nullptr, u32* __restrict__ h3 = nullptr) {\n"
-    << "  const u32 row = row0 + blockIdx.x * blockDim.x + threadIdx.x;   // row0: a rank of a multi-GPU proof evaluates its slice of the domain's rows\n  St s;\n"
-    << "  for (int i = 0; i < " << nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n  s.rr = Q{0u, 0u, 0u, 0u};\n";
-  if (track_high) o << "  s.rh = Q{0u, 0u, 0u, 0u};\n";
+  kk.params = "const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff, u32 row, u32 EL";
+  kk.enter = track_high ? " Q rr = s.rr; Q rh = s.rh;" : " Q rr = s.rr;";
+  kk.leave = track_high ? "  s.rr = rr; s.rh = rh;\n" : "  s.rr = rr;\n";
+  kk.sig = "const u32* const* __restrict__ cols, const u32* __restrict__ params, const u32* __restrict__ coeff,\n"
+          "    const u32* __restrict__ dinv, u32* __restrict__ a0, u32* __restrict__ a1, u32* __restrict__ a2, u32* __restrict__ a3, u32 EL, u32 row0,\n"
+          "    u32* __restrict__ h0 = nullptr, u32* __restrict__ h1 = nullptr, u32* __restrict__ h2 = nullptr, u32* __restrict__ h3 = nullptr";
+  kk.prologue = "  const u32 row = row0 + blockIdx.x * blockDim.x + threadIdx.x;   // row0: a rank of a multi-GPU proof evaluates its slice of the domain's rows\n";
+  kk.init = track_high ? "  s.rr = Q{0u, 0u, 0u, 0u};\n  s.rh = Q{0u, 0u, 0u, 0u};\n" : "  s.rr = Q{0u, 0u, 0u, 0u};\n";
   if (!pl.slots.empty())
-    o << "  for (u32 i = threadIdx.x; i < NB_NFOLD; i += blockDim.x) {\n"
-      << "    const Q f = qmac_tab(Q{0u, 0u, 0u, 0u}, ldq(params + 4 * nbfold_src[i].y), coeff + " << JIT_COEFF_WORDS << " * nbfold_src[i].x);\n"
-      << "    nbfold[i] = uint4{f.c0, f.c1, f.c2, f.c3};\n  }\n  __syncthreads();\n";
-  for (size_t ci = 0; ci < n_chunks; ++ci)
-    if (has_code[ci]) o << "  chunk" << ci << "(s, cols, params, coeff, row, EL);\n  __syncthreads();\n";
-  o << "  const u32 di = __ldg(dinv + (row >> " << DL << "));\n"
+    kk.init += "  for (u32 i = threadIdx.x; i < NB_NFOLD; i += blockDim.x) {\n"
+              "    const Q f = qmac_tab(Q{0u, 0u, 0u, 0u}, ldq(params + 4 * nbfold_src[i].y), coeff + " + std::to_string(JIT_COEFF_WORDS) + " * nbfold_src[i].x);\n"
+              "    nbfold[i] = uint4{f.c0, f.c1, f.c2, f.c3};\n  }\n  __syncthreads();\n";
+  kk.args = "cols, params, coeff, row, EL";
+  std::ostringstream e;
+  e << "  const u32 di = __ldg(dinv + (row >> " << DL << "));\n"
     << "  a0[row] = add(a0[row], mul(s.rr.c0, di)); a1[row] = add(a1[row], mul(s.rr.c1, di));\n"
     << "  a2[row] = add(a2[row], mul(s.rr.c2, di)); a3[row] = add(a3[row], mul(s.rr.c3, di));\n";
   if (track_high)
-    o << "  if (h0) {\n"
+    e << "  if (h0) {\n"
       << "    h0[row] = add(h0[row], mul(s.rh.c0, di)); h1[row] = add(h1[row], mul(s.rh.c1, di));\n"
       << "    h2[row] = add(h2[row], mul(s.rh.c2, di)); h3[row] = add(h3[row], mul(s.rh.c3, di));\n  }\n";
-  o << "}\n";
+  kk.epilogue = e.str();
+  emit_chunked(o, c, pl.at, kk);
   return o.str();
 }
 
@@ -447,9 +478,6 @@ std::string gen_source(const AirComponent& c, bool d2) {
 std::string gen_logup_source(const AirComponent& c) {
   std::ostringstream o;
   o << kPrelude;
-  const u32 nb = c.lg_base_regs ? c.lg_base_regs : 1, ne = c.lg_ext_regs ? c.lg_ext_regs : 1;
-  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; Q fn, fd, run; };\n";
-  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
   auto ld = [&](u32 m) {
     std::ostringstream s;
     // next-row masks and interaction-trace masks are not inputs of the logup program (they read as zero, as in the interpreter)
@@ -457,9 +485,6 @@ std::string gen_logup_source(const AirComponent& c) {
     else s << "0u";
     return s.str();
   };
-  size_t CH = 150;
-  size_t n_chunks = (c.logup_prog.size() + CH - 1) / CH;
-  const ChunkLive live = prog_liveness(c.logup_prog, CH, nb, ne);
   // The QM31 inverse (one per batch of fractions; 38 M31 products for x^(P-2) alone) is batched over G consecutive batches of the same
   // row: prefix products, ONE inverse, back-substitution (3 products per extra batch).  The inverse is unique, so the values are the
   // interpreter's.  `pending` batches wait in pfn/pfd until the group is full; the running row sum is then advanced batch by batch.
@@ -487,41 +512,50 @@ std::string gen_logup_source(const AirComponent& c) {
     pending.push_back(cur_batch);
     if ((int)pending.size() == G) flush(o2);
   };
-  o << "struct Pend { Q n[" << G << "], d[" << G << "]; };\n";
-  for (size_t ci = 0; ci < n_chunks; ++ci) {
-    o << "__device__ __noinline__ void chunk" << ci << "(St& s, Pend& pe, const u32* const* __restrict__ cols, const u32* __restrict__ params, u32* __restrict__ out, u32 row, u32 LS) {\n";
-    o << "  u32 b[" << nb << "]; Q e[" << ne << "]; Q fn = s.fn, fd = s.fd, run = s.run;\n";
-    for (int g = 0; g < G; ++g) o << "  Q pfn" << g << " = pe.n[" << g << "], pfd" << g << " = pe.d[" << g << "];\n";
-    for (u32 r : live.in_b[ci]) o << "  b[" << r << "] = s.b[" << r << "];";
-    for (u32 r : live.in_e[ci]) o << "  e[" << r << "] = s.e[" << r << "];";
-    o << "\n";
-    for (size_t pc = ci * CH; pc < std::min(c.logup_prog.size(), (ci + 1) * CH); ++pc) {
-      const AirInstr& in = c.logup_prog[pc];
-      if (in.op == OP_FRAC) {
-        u32 bt = c.batching[k];
-        if (have && bt != cur_batch) { finalize(o); have = false; }
-        if (!have) o << "  fn = e[" << in.a << "]; fd = e[" << in.b << "];\n";                      // first fraction of the batch: 0/1 + n/d
-        else o << "  fn = qadd(qmul(fn, e[" << in.b << "]), qmul(e[" << in.a << "], fd)); fd = qmul(fd, e[" << in.b << "]);\n";
-        cur_batch = bt; have = true; ++k;
-      } else {
-        o << "  "; emit_op(o, in, ld); o << "\n";
-      }
-    }
-    if (ci + 1 == n_chunks) { if (have) finalize(o); flush(o); }
-    for (u32 r : live.out_b[ci]) o << "  s.b[" << r << "] = b[" << r << "];";
-    for (u32 r : live.out_e[ci]) o << "  s.e[" << r << "] = e[" << r << "];";
-    o << "\n  s.fn = fn; s.fd = fd; s.run = run;\n";
-    for (int g = 0; g < G; ++g) o << "  pe.n[" << g << "] = pfn" << g << "; pe.d[" << g << "] = pfd" << g << ";\n";
-    o << "}\n";
+  std::vector<std::vector<Stmt>> at(c.logup_prog.size());
+  for (size_t pc = 0; pc < c.logup_prog.size(); ++pc) {
+    const AirInstr& in = c.logup_prog[pc];
+    if (in.op != OP_FRAC) { at[pc].push_back(op_stmt(in, ld)); continue; }
+    std::ostringstream s;   // whole lines, the previous batch's completion first (the emitter writes the first indent and the last newline)
+    u32 bt = c.batching[k];
+    if (have && bt != cur_batch) { finalize(s); have = false; }
+    if (!have) s << "  fn = e[" << in.a << "]; fd = e[" << in.b << "];";                      // first fraction of the batch: 0/1 + n/d
+    else s << "  fn = qadd(qmul(fn, e[" << in.b << "]), qmul(e[" << in.a << "], fd)); fd = qmul(fd, e[" << in.b << "]);";
+    cur_batch = bt; have = true; ++k;
+    at[pc].push_back(Stmt{s.str().substr(2), instr_regs(in)});
   }
-  o << "extern \"C\" __global__ void __launch_bounds__(" << JIT_BLOCK << ", 1) nbjit(const u32* const* __restrict__ cols, const u32* __restrict__ params, u32* __restrict__ out, u32 LS) {\n"
-    << "  const u32 row = blockIdx.x * blockDim.x + threadIdx.x;\n  St s;\n"
-    << "  for (int i = 0; i < " << nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n"
-    << "  s.fn = Q{0u, 0u, 0u, 0u}; s.fd = Q{1u, 0u, 0u, 0u}; s.run = Q{0u, 0u, 0u, 0u};\n"
-    << "  Pend pe; for (int i = 0; i < " << 4 << "; ++i) { pe.n[i] = Q{0u, 0u, 0u, 0u}; pe.d[i] = Q{1u, 0u, 0u, 0u}; }\n";
-  for (size_t ci = 0; ci < n_chunks; ++ci) o << "  chunk" << ci << "(s, pe, cols, params, out, row, LS);\n  __syncthreads();\n";
-  o << "}\n";
+  std::ostringstream last;
+  if (have) finalize(last);
+  flush(last);
+  ChunkedKernel kk;
+  kk.ch = 150; kk.nb = c.lg_base_regs ? c.lg_base_regs : 1; kk.ne = c.lg_ext_regs ? c.lg_ext_regs : 1;
+  kk.state = " Q fn, fd, run;";
+  kk.decls = "struct Pend { Q n[" + std::to_string(G) + "], d[" + std::to_string(G) + "]; };\n";
+  kk.params = "Pend& pe, const u32* const* __restrict__ cols, const u32* __restrict__ params, u32* __restrict__ out, u32 row, u32 LS";
+  std::ostringstream enter, leave;
+  enter << " Q fn = s.fn, fd = s.fd, run = s.run;";
+  leave << "  s.fn = fn; s.fd = fd; s.run = run;\n";
+  for (int g = 0; g < G; ++g) {
+    enter << "\n  Q pfn" << g << " = pe.n[" << g << "], pfd" << g << " = pe.d[" << g << "];";
+    leave << "  pe.n[" << g << "] = pfn" << g << "; pe.d[" << g << "] = pfd" << g << ";\n";
+  }
+  kk.enter = enter.str();
+  kk.leave = leave.str();
+  kk.last = last.str();
+  kk.sig = "const u32* const* __restrict__ cols, const u32* __restrict__ params, u32* __restrict__ out, u32 LS";
+  kk.prologue = "  const u32 row = blockIdx.x * blockDim.x + threadIdx.x;\n";
+  kk.init = "  s.fn = Q{0u, 0u, 0u, 0u}; s.fd = Q{1u, 0u, 0u, 0u}; s.run = Q{0u, 0u, 0u, 0u};\n"
+            "  Pend pe; for (int i = 0; i < 4; ++i) { pe.n[i] = Q{0u, 0u, 0u, 0u}; pe.d[i] = Q{1u, 0u, 0u, 0u}; }\n";
+  kk.args = "pe, cols, params, out, row, LS";
+  emit_chunked(o, c, at, kk);
   return o.str();
+}
+
+// Columns are in bit-reversed circle-domain order.  Position i holds circle-domain index brev(i), which is coset (trace) row 2j for circle
+// index j < N/2 and 2N - 2j - 1 above (the inverse of coset_index_to_circle_domain_index).
+static std::string coset_rows(const AirComponent& c) {
+  return "#define NB_DL " + std::to_string(c.log_size) + "u\n#define NB_N (1u << NB_DL)\n"
+         "__device__ __forceinline__ u32 pos_to_row(u32 i) { const u32 j = __brev(i) >> (32 - NB_DL); return j < NB_N / 2 ? 2 * j : 2 * NB_N - 2 * j - 1; }\n";
 }
 
 // The constraint check (the GPU counterpart of stwo's assert_constraints_on_polys): the plain constraint program on the trace domain
@@ -532,12 +566,8 @@ std::string gen_check_source(const AirComponent& c) {
   std::ostringstream o;
   o << "// constraint check on the trace domain: each constraint tested for zero on every row\n";
   o << kPrelude;
-  const u32 DL = c.log_size;
-  // Columns are in bit-reversed circle-domain order.  Position i holds circle-domain index brev(i), which is coset (trace) row
-  // 2j for circle index j < N/2 and 2N - 2j - 1 above (the inverse of coset_index_to_circle_domain_index); a mask at offset `off`
-  // reads coset row (r + off) mod N, wrapping at both ends as assert_constraints_on_polys does.
-  o << "#define NB_DL " << DL << "u\n#define NB_N (1u << NB_DL)\n"
-    << "__device__ __forceinline__ u32 pos_to_row(u32 i) { const u32 j = __brev(i) >> (32 - NB_DL); return j < NB_N / 2 ? 2 * j : 2 * NB_N - 2 * j - 1; }\n"
+  // a mask at offset `off` reads coset row (r + off) mod N, wrapping at both ends as assert_constraints_on_polys does
+  o << coset_rows(c)
     << "__device__ __forceinline__ u32 row_to_pos(u32 r) { const u32 j = (r & 1) ? NB_N - (r + 1) / 2 : r / 2; return __brev(j) >> (32 - NB_DL); }\n"
     << "__device__ __forceinline__ u32 offrow(u32 r, int off) { return row_to_pos((r + (u32)off) & (NB_N - 1)); }   // N divides 2^32\n"
     // every prelude operation returns a canonical residue; P is also taken as zero for a constraint that is a raw (unreduced) cell
@@ -551,46 +581,32 @@ std::string gen_check_source(const AirComponent& c) {
     << "    const u32 lo = __reduce_min_sync(am, bad ? r : 0xffffffffu);\n"
     << "    if ((threadIdx.x & 31u) == (u32)(__ffs(am) - 1)) { atomicAdd(nfail + k, (u32)__popc(m)); atomicMin(first + k, lo); }\n"
     << "  }\n}\n";
-  const u32 nb = c.n_base_regs ? c.n_base_regs : 1, ne = c.n_ext_regs ? c.n_ext_regs : 1;
-  o << "struct St { u32 b[" << nb << "]; Q e[" << ne << "]; };\n";
-  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
   auto ld = [&](u32 m) {
     std::ostringstream s;
     if (c.masks[m].off == 0) s << "__ldg(ccols[" << m << "] + pos)";
     else s << "__ldg(ccols[" << m << "] + offrow(r, " << c.masks[m].off << "))";
     return s.str();
   };
-  const size_t CH = 250;
-  const size_t n_chunks = (c.prog.size() + CH - 1) / CH;
-  const ChunkLive live = prog_liveness(c.prog, CH, nb, ne);
+  std::vector<std::vector<Stmt>> at(c.prog.size());
   u32 k = 0;
-  for (size_t ci = 0; ci < n_chunks; ++ci) {
-    o << "__device__ __noinline__ void chunk" << ci << "(St& s, const u32* __restrict__ params, u32* __restrict__ nfail, u32* __restrict__ first, u32 pos, u32 r, bool live) {\n";
-    o << "  u32 b[" << nb << "]; Q e[" << ne << "];\n";
-    for (u32 x : live.in_b[ci]) o << "  b[" << x << "] = s.b[" << x << "];";
-    for (u32 x : live.in_e[ci]) o << "  e[" << x << "] = s.e[" << x << "];";
-    o << "\n";
-    for (size_t pc = ci * CH; pc < std::min(c.prog.size(), (ci + 1) * CH); ++pc) {
-      const AirInstr& in = c.prog[pc];
-      o << "  ";
-      if (in.op == OP_CONSTRB) o << "check(" << k++ << "u, live && nzb(b[" << in.a << "]), r, nfail, first);";
-      else if (in.op == OP_CONSTRE) o << "check(" << k++ << "u, live && nze(e[" << in.a << "]), r, nfail, first);";
-      else emit_op(o, in, ld);
-      o << "\n";
-    }
-    for (u32 x : live.out_b[ci]) o << "  s.b[" << x << "] = b[" << x << "];";
-    for (u32 x : live.out_e[ci]) o << "  s.e[" << x << "] = e[" << x << "];";
-    o << "\n}\n";
+  for (size_t pc = 0; pc < c.prog.size(); ++pc) {
+    const AirInstr& in = c.prog[pc];
+    Stmt st = op_stmt(in, ld);
+    if (in.op == OP_CONSTRB) st.code = "check(" + std::to_string(k++) + "u, live && nzb(b[" + std::to_string(in.a) + "]), r, nfail, first);";
+    if (in.op == OP_CONSTRE) st.code = "check(" + std::to_string(k++) + "u, live && nze(e[" + std::to_string(in.a) + "]), r, nfail, first);";
+    at[pc].push_back(st);
   }
+  ChunkedKernel kk;
+  kk.ch = 250; kk.nb = c.n_base_regs ? c.n_base_regs : 1; kk.ne = c.n_ext_regs ? c.n_ext_regs : 1;
+  kk.params = "const u32* __restrict__ params, u32* __restrict__ nfail, u32* __restrict__ first, u32 pos, u32 r, bool live";
   // nfail[k] / first[k]: rows on which constraint k is non-zero and the first of them in coset order (0xffffffff: none)
-  o << "extern \"C\" __global__ void __launch_bounds__(" << JIT_BLOCK << ", 1) nbjit(const u32* __restrict__ params, u32* __restrict__ nfail, u32* __restrict__ first) {\n"
-    << "  const u32 gid = blockIdx.x * blockDim.x + threadIdx.x;\n"
-    << "  const bool live = gid < NB_N;\n"
-    << "  const u32 pos = live ? gid : 0u;   // a thread past the domain runs row 0 with its results masked: every thread reaches the barriers\n"
-    << "  const u32 r = pos_to_row(pos);\n  St s;\n"
-    << "  for (int i = 0; i < " << nb << "; ++i) s.b[i] = 0u;\n  for (int i = 0; i < " << ne << "; ++i) s.e[i] = Q{0u, 0u, 0u, 0u};\n";
-  for (size_t ci = 0; ci < n_chunks; ++ci) o << "  chunk" << ci << "(s, params, nfail, first, pos, r, live);\n  __syncthreads();\n";
-  o << "}\n";
+  kk.sig = "const u32* __restrict__ params, u32* __restrict__ nfail, u32* __restrict__ first";
+  kk.prologue = "  const u32 gid = blockIdx.x * blockDim.x + threadIdx.x;\n"
+                "  const bool live = gid < NB_N;\n"
+                "  const u32 pos = live ? gid : 0u;   // a thread past the domain runs row 0 with its results masked: every thread reaches the barriers\n"
+                "  const u32 r = pos_to_row(pos);\n";
+  kk.args = "params, nfail, first, pos, r, live";
+  emit_chunked(o, c, at, kk);
   return o.str();
 }
 
@@ -606,8 +622,7 @@ std::string gen_count_source(const AirComponent& c, const std::vector<AirFrac>& 
   std::ostringstream o;
   o << "// table multiplicities: build (table tuples -> bins) and probe (lookups -> counters)\n";
   o << kPrelude;
-  o << "#define NB_DL " << c.log_size << "u\n#define NB_N (1u << NB_DL)\n"
-    << "__device__ __forceinline__ u32 pos_to_row(u32 i) { const u32 j = __brev(i) >> (32 - NB_DL); return j < NB_N / 2 ? 2 * j : 2 * NB_N - 2 * j - 1; }\n"
+  o << coset_rows(c)
     << "__device__ __forceinline__ u32 canon(u32 v) { return v >= P31 ? v - P31 : v; }\n"
     << "#define NB_EMPTY 0xffffffffu\n"
     << "__device__ __forceinline__ u32 khash(u32 rel, u32 len, const u32* v) {\n"
@@ -654,7 +669,7 @@ std::string gen_count_source(const AirComponent& c, const std::vector<AirFrac>& 
     << "    const u32 lo = __reduce_min_sync(am, (u32)(key >> 32) == hi ? (u32)key : 0xffffffffu);\n"
     << "    if ((threadIdx.x & 31u) == (u32)(__ffs(am) - 1)) { atomicAdd(um, (u64)__popc(m)); atomicMin(um + 1, (u64)hi << 32 | lo); }\n"
     << "  }\n}\n";
-  o << "#define NB_NMASKS " << c.masks.size() << "\n__constant__ const u32* ccols[NB_NMASKS > 0 ? NB_NMASKS : 1];\n";
+  o << ccols_decl(c);
   const std::vector<AirInstr>& prog = c.logup_prog;
   std::vector<int> da, db;
   prog_defs(prog, c.lg_base_regs, c.lg_ext_regs, da, db);
@@ -753,10 +768,25 @@ std::string gen_count_source(const AirComponent& c, const std::vector<AirFrac>& 
 }
 }  // namespace
 
-std::string jit_source(const AirComponent& c, bool d2) { return gen_source(c, d2); }
-std::string jit_logup_source(const AirComponent& c) { return gen_logup_source(c); }
-std::string jit_check_source(const AirComponent& c) { return gen_check_source(c); }
-std::string jit_count_source(const AirComponent& c, const std::vector<AirFrac>& fr) { return gen_count_source(c, fr); }
+bool jit_specialised(JitKind kind, const AirComponent& c, const std::vector<AirFrac>& fr) {
+  switch (kind) {
+    case JIT_CONSTRAINTS: return c.prog.size() >= JIT_MIN_INSTR;
+    case JIT_LOGUP: return c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0;
+    case JIT_D2: return c.prog.size() >= JIT_MIN_INSTR && count_high(high_constraints(c)) > 0;
+    case JIT_CHECK: return c.n_constraints > 0;
+    case JIT_COUNT: return std::any_of(fr.begin(), fr.end(), [](const AirFrac& f) { return f.kind == FRAC_TABLE || f.kind == FRAC_LOOKUP; });
+    default: return false;
+  }
+}
+
+std::string jit_kernel_source(JitKind kind, const AirComponent& c, const std::vector<AirFrac>& fr) {
+  switch (kind) {
+    case JIT_LOGUP: return gen_logup_source(c);
+    case JIT_CHECK: return gen_check_source(c);
+    case JIT_COUNT: return gen_count_source(c, fr);
+    default: return gen_source(c, kind == JIT_D2);
+  }
+}
 
 bool jit_enabled() {
   const char* e = getenv("NB200_JIT");
@@ -768,13 +798,6 @@ void jit_release(JitKernel& jk) {
   jk = JitKernel();
 }
 
-static nb200_status jit_compile_source(nb200_ctx* ctx, const AirComponent& c, const std::string& src, JitKernel* out);
-nb200_status jit_compile_constraints(nb200_ctx* ctx, const AirComponent& c, bool d2, JitKernel* out) { return jit_compile_source(ctx, c, gen_source(c, d2), out); }
-nb200_status jit_compile_logup(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_logup_source(c), out); }
-nb200_status jit_compile_check(nb200_ctx* ctx, const AirComponent& c, JitKernel* out) { return jit_compile_source(ctx, c, gen_check_source(c), out); }
-nb200_status jit_compile_count(nb200_ctx* ctx, const AirComponent& c, const std::vector<AirFrac>& fr, JitKernel* out) {
-  return jit_compile_source(ctx, c, gen_count_source(c, fr), out);
-}
 // ---- cubin cache: <directory of this library>/jit_cache/<key>.cubin (or $NB200_JIT_CACHE).  `python -m nexus_zkvm_b200.build`
 // fills it for the shipped machines with nvcc, so a fresh box neither loads libnvrtc nor compiles; kernels compiled at run time are
 // added when the directory is writable.  The key covers the generated source and the target; the D2 variant of a constraint kernel
@@ -831,8 +854,9 @@ static nb200_status jit_load_cubin(nb200_ctx* ctx, const AirComponent& c, const 
   return NB200_OK;
 }
 
-static nb200_status jit_compile_source(nb200_ctx* ctx, const AirComponent& c, const std::string& src, JitKernel* out) {
+nb200_status jit_compile(nb200_ctx* ctx, JitKind kind, const AirComponent& c, const std::vector<AirFrac>& fr, JitKernel* out) {
   out->lib = nullptr; out->kernel = nullptr; out->tried = true;
+  const std::string src = jit_kernel_source(kind, c, fr);
   const std::string cache = jit_cache_path(src);
   if (!cache.empty()) {
     std::vector<char> cubin;
@@ -871,67 +895,16 @@ void jit_coeff_table(const std::vector<qm31>& coeffs, std::vector<u32>& out) {
   }
 }
 
-// the kernel's column pointers: device array -> the module's __constant__ table, in stream order
-static nb200_status jit_set_cols(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols) {
+// the kernel's column pointers (a host array, one per mask) into the module's __constant__ table, then the kernel, both in stream order
+nb200_status jit_launch(nb200_ctx* ctx, const JitKernel& jk, const u32* const* cols, size_t n_cols, dim3 grid, dim3 block, void** args, size_t smem) {
   void* dptr = nullptr; size_t bytes = 0;
   cudaError_t e = cudaLibraryGetGlobal(&dptr, &bytes, (cudaLibrary_t)jk.lib, "ccols");
   if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit: cudaLibraryGetGlobal(ccols): ") + cudaGetErrorString(e));
-  e = cudaMemcpyAsync(dptr, d_cols, bytes, cudaMemcpyDeviceToDevice, ctx->stream);
-  if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit: ccols copy: ") + cudaGetErrorString(e));
-  return NB200_OK;
-}
-
-nb200_status jit_launch_logup(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, u32* d_out, u32 log_size) {
-  // log_size = log2 of the rows of THIS launch (the whole trace domain, or a rank's slice of it: the kernel is row-local)
-  size_t rows = (size_t)1 << log_size;
-  if (rows < JIT_BLOCK) return set_err(ctx, NB200_ERR_STATE, "jit: domain too small");
-  NB_TRY(jit_set_cols(ctx, jk, d_cols));
-  void* args[] = {(void*)&d_cols, (void*)&d_params, (void*)&d_out, (void*)&log_size};
-  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args, 0, ctx->stream);
-  ctx->launches += 1;
-  if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
-  return NB200_OK;
-}
-
-nb200_status jit_launch_check(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, u32* d_nfail, u32* d_first) {
-  // one thread per trace row; a domain smaller than a CTA (MultiMachine has 2^4-row components) runs as one CTA of exactly its rows
-  const size_t rows = (size_t)1 << jk.log_size;
-  const u32 block = (u32)std::min<size_t>(rows, JIT_LAUNCH_BLOCK);
-  NB_TRY(jit_set_cols(ctx, jk, d_cols));
-  void* args[] = {(void*)&d_params, (void*)&d_nfail, (void*)&d_first};
-  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)((rows + block - 1) / block)), dim3(block), args, 0, ctx->stream);
-  ctx->launches += 1;
-  if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
-  return NB200_OK;
-}
-
-nb200_status jit_launch_count(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const CountArgs& a) {
-  // rows by a grid-stride loop: at most 8 CTAs per SM, so that the probe's private bins are zeroed and flushed a bounded number of times
-  const size_t rows = (size_t)1 << jk.log_size;
-  const u32 block = (u32)std::min<size_t>(rows, 256);
-  const u32 grid = (u32)std::min<size_t>((rows + block - 1) / block, (size_t)ctx->sm_count * 8);
-  NB_TRY(jit_set_cols(ctx, jk, d_cols));
-  CountArgs v = a;
-  void* args[] = {(void*)&v.mode, (void*)&v.comp, (void*)&v.tbase, (void*)&v.slots, (void*)&v.keys, (void*)&v.kw, (void*)&v.mask,
-                  (void*)&v.cnt, (void*)&v.nsh, (void*)&v.um, (void*)&v.err};
-  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3(grid), dim3(block), args, a.mode ? (size_t)a.nsh * 8 : 0, ctx->stream);
-  ctx->launches += 1;
-  if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
-  return NB200_OK;
-}
-
-nb200_status jit_launch_constraints(nb200_ctx* ctx, const JitKernel& jk, const u32* const* d_cols, const u32* d_params, const u32* d_coeff, const u32* d_dinv, u32* const acc[4],
-                                    u32 rows_log, u32 dom_log, u32 row0, size_t n_rows, u32* const acc_high[4]) {
-  size_t rows = n_rows ? n_rows : (size_t)1 << rows_log;
-  if (rows < JIT_BLOCK || rows % JIT_BLOCK != 0) return set_err(ctx, NB200_ERR_STATE, "jit: row range too small");
-  NB_TRY(jit_set_cols(ctx, jk, d_cols));
-  u32 el = dom_log;
-  u32* a0 = acc[0]; u32* a1 = acc[1]; u32* a2 = acc[2]; u32* a3 = acc[3];
-  u32* h[4] = {nullptr, nullptr, nullptr, nullptr};
-  if (acc_high) for (int k = 0; k < 4; ++k) h[k] = acc_high[k];
-  void* args[] = {(void*)&d_cols, (void*)&d_params, (void*)&d_coeff, (void*)&d_dinv, (void*)&a0, (void*)&a1, (void*)&a2, (void*)&a3, (void*)&el, (void*)&row0,
-                  (void*)&h[0], (void*)&h[1], (void*)&h[2], (void*)&h[3]};
-  cudaError_t e = cudaLaunchKernel((const void*)jk.kernel, dim3((u32)(rows / JIT_LAUNCH_BLOCK)), dim3(JIT_LAUNCH_BLOCK), args, 0, ctx->stream);
+  if (n_cols) {
+    e = cudaMemcpyAsync(dptr, cols, n_cols * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream);
+    if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit: ccols copy: ") + cudaGetErrorString(e));
+  }
+  e = cudaLaunchKernel((const void*)jk.kernel, grid, block, args, smem, ctx->stream);
   ctx->launches += 1;
   if (e != cudaSuccess) return set_err(ctx, NB200_ERR_CUDA, std::string("jit launch: ") + cudaGetErrorString(e));
   return NB200_OK;

@@ -18,14 +18,10 @@
 struct nb200_channel { nb::HostChannel ch; };
 struct nb200_air {
   nb::AirProgram prog;
-  // per component, compiled on first use (NVRTC); empty kernel = bytecode interpreter
-  std::vector<nb::JitKernel> jit;        // constraint program (D1 and whole domains)
-  std::vector<nb::JitKernel> jit_d2;     // its constraints of degree above AIR_LOW_DEGREE (D2 of the half-domain route)
-  std::vector<nb::JitKernel> jit_logup;  // logup (interaction trace) program
-  std::vector<nb::JitKernel> jit_check;  // constraint check on the trace domain (nb200_check_constraints)
-  std::vector<nb::JitKernel> jit_count;  // table-multiplicity build / probe (nb200_table_multiplicities)
+  // per kind and component, compiled on first use (NVRTC); empty kernel = bytecode interpreter
+  std::vector<nb::JitKernel> jit[nb::JIT_KINDS];
   std::vector<std::vector<nb::AirFrac>> fracs;   // every component's fractions as tables, lookups or neither (air_lookup_tables)
-  ~nb200_air() { for (auto* v : {&jit, &jit_d2, &jit_logup, &jit_check, &jit_count}) for (auto& j : *v) nb::jit_release(j); }
+  ~nb200_air() { for (auto& v : jit) for (auto& j : v) nb::jit_release(j); }
 };
 
 namespace nb {
@@ -80,26 +76,21 @@ static nb200_status upload_params(nb200_ctx* ctx, const void* params, size_t n_p
 }
 
 // The component's specialised kernel, compiled on first use; nullptr = none.
-// `interp_fallback`: the caller can run the bytecode interpreter, so programs shorter than JIT_MIN_INSTR are not compiled and a failed
-// compile is only logged (NB200_TRACE).  The sharded row kernels and the constraint check have no interpreter: they try every program and
-// reject a nullptr.
-enum JitKind { JIT_CONSTRAINTS, JIT_D2, JIT_LOGUP, JIT_CHECK, JIT_COUNT };
+// `interp_fallback`: the caller can run the bytecode interpreter, so only the kinds jit_specialised names are compiled and a failed
+// compile is only logged (NB200_TRACE).  The sharded row kernels, the constraint check and the count have no interpreter: they try every
+// program and reject a nullptr.
 static const JitKernel* ensure_jit(nb200_ctx* ctx, nb200_air* air_h, size_t comp_idx, JitKind kind, bool interp_fallback) {
-  std::vector<JitKernel>& v = kind == JIT_COUNT ? air_h->jit_count : kind == JIT_CHECK ? air_h->jit_check : kind == JIT_LOGUP ? air_h->jit_logup
-                            : kind == JIT_D2 ? air_h->jit_d2 : air_h->jit;
+  std::vector<JitKernel>& v = air_h->jit[kind];
   if (v.size() != air_h->prog.comps.size()) v.resize(air_h->prog.comps.size());
   JitKernel& jk = v[comp_idx];
   if (!jk.tried) {
     jk.tried = true;
     const AirComponent& c = air_h->prog.comps[comp_idx];
-    const bool worth_it = kind == JIT_LOGUP ? (c.logup_prog.size() >= JIT_MIN_INSTR && c.n_logup_cols() > 0) : c.prog.size() >= JIT_MIN_INSTR;
-    if ((worth_it || !interp_fallback) && jit_enabled()) {
-      nb200_status st = kind == JIT_COUNT ? jit_compile_count(ctx, c, air_h->fracs[comp_idx], &jk)
-                      : kind == JIT_CHECK ? jit_compile_check(ctx, c, &jk)
-                      : kind == JIT_LOGUP ? jit_compile_logup(ctx, c, &jk) : jit_compile_constraints(ctx, c, kind == JIT_D2, &jk);
+    if ((!interp_fallback || jit_specialised(kind, c, air_h->fracs[comp_idx])) && jit_enabled()) {
+      nb200_status st = jit_compile(ctx, kind, c, air_h->fracs[comp_idx], &jk);
       if (st != NB200_OK) jk.err = ctx->err;   // kept with the kernel: a later call that finds it missing reports why
       if (interp_fallback) {
-        static const char* what[] = {"component", "component (D2)", "logup program", "constraint check"};
+        static const char* what[] = {"component", "logup program", "component (D2)", "constraint check"};
         if (st != NB200_OK && ctx->trace) fprintf(stderr, "[nb200] jit unavailable for %s: %s\n", what[kind], ctx->err.c_str());
         trace_mark(ctx, kind == JIT_LOGUP ? "jit: compile logup (one-time)" : "jit: compile (one-time)");
       }
@@ -1276,18 +1267,21 @@ nb200_status check_constraints(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, c
   }
   const JitKernel* jk = ensure_jit(ctx, air_h, comp_idx, JIT_CHECK, false);
   if (!jk)
-    return set_err(ctx, NB200_ERR_STATE, jit_enabled() ? "check_constraints: the constraint-check kernel could not be compiled: " + air_h->jit_check[comp_idx].err
+    return set_err(ctx, NB200_ERR_STATE, jit_enabled() ? "check_constraints: the constraint-check kernel could not be compiled: " + air_h->jit[JIT_CHECK][comp_idx].err
                                                        : std::string("check_constraints: the constraint check runs only as a generated kernel (NB200_JIT=0)"));
-  // device side: the parameter table, the column pointers (copied into the kernel's constant table) and one count + one row per constraint
-  DevBuf d_params, d_cols, d_res;
+  // device side: the parameter table and one count + one row per constraint
+  DevBuf d_params, d_res;
   NB_TRY(upload_params(ctx, params, n_params, d_params));
-  NB_TRY(alloc(ctx, d_cols, std::max<size_t>(mask_cols.size(), 1) * 2));
-  if (!mask_cols.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_cols.p, mask_cols.data(), mask_cols.size() * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream));
   NB_TRY(alloc(ctx, d_res, 2 * n));
   NB_CUDA(ctx, cudaMemsetAsync(d_res.p, 0, n * 4, ctx->stream));
   NB_CUDA(ctx, cudaMemsetAsync(d_res.p + n, 0xff, n * 4, ctx->stream));
   trace_mark(ctx, nullptr);
-  NB_TRY(jit_launch_check(ctx, *jk, (const u32* const*)d_cols.p, d_params.p, d_res.p, d_res.p + n));
+  // one thread per trace row; a domain smaller than a CTA (MultiMachine has 2^4-row components) runs as one CTA of exactly its rows
+  const size_t rows = (size_t)1 << jk->log_size;
+  const u32 block = (u32)std::min<size_t>(rows, JIT_LAUNCH_BLOCK);
+  u32* d_nfail = d_res.p; u32* d_first = d_res.p + n;
+  void* args[] = {(void*)&d_params.p, (void*)&d_nfail, (void*)&d_first};
+  NB_TRY(jit_launch(ctx, *jk, mask_cols.data(), mask_cols.size(), dim3((u32)((rows + block - 1) / block)), dim3(block), args));
   std::vector<u32> res(2 * n);
   NB_CUDA(ctx, cudaMemcpyAsync(res.data(), d_res.p, 2 * n * 4, cudaMemcpyDeviceToHost, ctx->stream));
   NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // also: the host tables above have been consumed
@@ -1372,7 +1366,7 @@ nb200_status table_multiplicities(nb200_ctx* ctx, nb200_air* air_h, const nb200_
     if (!builds[k] && !probes[k]) continue;
     jk[k] = ensure_jit(ctx, air_h, k, JIT_COUNT, false);
     if (!jk[k])
-      return set_err(ctx, NB200_ERR_STATE, jit_enabled() ? "table_multiplicities: the count kernel could not be compiled: " + air_h->jit_count[k].err
+      return set_err(ctx, NB200_ERR_STATE, jit_enabled() ? "table_multiplicities: the count kernel could not be compiled: " + air_h->jit[JIT_COUNT][k].err
                                                          : std::string("table_multiplicities: the count runs only as a generated kernel (NB200_JIT=0)"));
   }
   // hash: at most half full; keys: relation, length, values per bin
@@ -1382,40 +1376,43 @@ nb200_status table_multiplicities(nb200_ctx* ctx, nb200_air* air_h, const nb200_
   std::vector<u32> tb;
   std::vector<size_t> tb_at(air.comps.size(), 0);
   for (size_t k = 0; k < air.comps.size(); ++k) { tb_at[k] = tb.size(); tb.insert(tb.end(), tbase[k].begin(), tbase[k].end()); }
-  DevBuf d_slots, d_keys, d_cnt, d_um, d_err, d_tb, d_cols;
+  DevBuf d_slots, d_keys, d_cnt, d_um, d_tb;
   NB_TRY(alloc(ctx, d_slots, cap));
   NB_TRY(alloc(ctx, d_keys, n_bins * kw));
   NB_TRY(alloc(ctx, d_cnt, 2 * n_bins));
   NB_TRY(alloc(ctx, d_um, 4 + 1));
   NB_TRY(alloc(ctx, d_tb, std::max<size_t>(tb.size(), 1)));
-  NB_TRY(alloc(ctx, d_cols, std::max<size_t>(cols_all.size(), 1) * 2));
   NB_CUDA(ctx, cudaMemsetAsync(d_slots.p, 0xff, (size_t)cap * 4, ctx->stream));
   NB_CUDA(ctx, cudaMemsetAsync(d_cnt.p, 0, n_bins * 8, ctx->stream));
   const uint64_t um_init[2] = {0, UINT64_MAX};
   NB_CUDA(ctx, cudaMemcpyAsync(d_um.p, um_init, 16, cudaMemcpyHostToDevice, ctx->stream));
   NB_CUDA(ctx, cudaMemsetAsync(d_um.p + 4, 0, 4, ctx->stream));
   if (!tb.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_tb.p, tb.data(), tb.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
-  if (!cols_all.empty()) NB_CUDA(ctx, cudaMemcpyAsync(d_cols.p, cols_all.data(), cols_all.size() * sizeof(u32*), cudaMemcpyHostToDevice, ctx->stream));
-  CountArgs a;
-  a.slots = d_slots.p; a.keys = d_keys.p; a.kw = kw; a.mask = (u32)(cap - 1);
-  a.cnt = (unsigned long long*)d_cnt.p; a.um = (unsigned long long*)d_um.p; a.err = d_um.p + 4;
+  // component k's count kernel in `mode` (jit.cu gen_count_source); rows by a grid-stride loop: at most 8 CTAs per SM, so that the probe's
+  // private bins are zeroed and flushed a bounded number of times
+  const u32 mask = (u32)(cap - 1);
+  unsigned long long *cnt = (unsigned long long*)d_cnt.p, *um_dev = (unsigned long long*)d_um.p;
+  u32* err = d_um.p + 4;
+  auto count = [&](size_t k, u32 mode, const u32* tbase, u32 nsh) {
+    const size_t rows = (size_t)1 << jk[k]->log_size;
+    const u32 block = (u32)std::min<size_t>(rows, 256);
+    const u32 grid = (u32)std::min<size_t>((rows + block - 1) / block, (size_t)ctx->sm_count * 8);
+    u32 comp = (u32)k;
+    void* args[] = {(void*)&mode, (void*)&comp, (void*)&tbase, (void*)&d_slots.p, (void*)&d_keys.p, (void*)&kw, (void*)&mask,
+                    (void*)&cnt, (void*)&nsh, (void*)&um_dev, (void*)&err};
+    return jit_launch(ctx, *jk[k], cols_all.data() + cols_at[k], air.comps[k].masks.size(), dim3(grid), dim3(block), args, mode ? (size_t)nsh * 8 : 0);
+  };
   trace_mark(ctx, nullptr);
-  for (size_t k = 0; k < air.comps.size(); ++k) {
-    if (!builds[k]) continue;
-    a.mode = 0; a.comp = (u32)k; a.tbase = d_tb.p + tb_at[k]; a.nsh = 0;
-    NB_TRY(jit_launch_count(ctx, *jk[k], (const u32* const*)d_cols.p + cols_at[k], a));
-  }
+  for (size_t k = 0; k < air.comps.size(); ++k)
+    if (builds[k]) NB_TRY(count(k, 0, d_tb.p + tb_at[k], 0));
   u32 dup = 0;
   NB_CUDA(ctx, cudaMemcpyAsync(&dup, d_um.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
   NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // also: the host tables above have been consumed
   if (dup) return set_err(ctx, NB200_ERR_ARG, "table_multiplicities: a table lists the same tuple in two rows of one relation");
   // bins privatised per CTA when they fit in 32 KB of shared memory (the v1 machine's Range256 + Range32: 288 bins)
   const u32 nsh = n_bins * 8 <= 32768 ? (u32)n_bins : 0u;
-  for (size_t k = 0; k < air.comps.size(); ++k) {
-    if (!probes[k]) continue;
-    a.mode = 1; a.comp = (u32)k; a.tbase = d_tb.p; a.nsh = nsh;
-    NB_TRY(jit_launch_count(ctx, *jk[k], (const u32* const*)d_cols.p + cols_at[k], a));
-  }
+  for (size_t k = 0; k < air.comps.size(); ++k)
+    if (probes[k]) NB_TRY(count(k, 1, d_tb.p, nsh));
   uint64_t bin = 0;
   for (auto& m : mult) {
     NB_TRY(table_mult_store(ctx, m.first, (const unsigned long long*)d_cnt.p + bin, (size_t)1 << m.second));
@@ -1585,19 +1582,22 @@ nb200_status nb200_air_d2_masks(const nb200_air* a, uint32_t component, uint8_t*
   for (size_t m = 0; m < n; ++m) flags[m] = used[m] ? 1 : 0;
   return NB200_OK;
 }
-nb200_status nb200_air_kernel_source(const nb200_air* a, uint32_t component, int which, char** out) {
-  if (!a || !out || component >= a->prog.comps.size() || which < 0 || which > 3) return NB200_ERR_ARG;
+// the source the prover compiles for this kind and component; NB200_ERR_STATE when it compiles none (the interpreter runs the program, or
+// there is nothing to evaluate)
+static nb200_status kernel_source(const nb200_air* a, uint32_t component, JitKind kind, char** out) {
   const AirComponent& c = a->prog.comps[component];
-  *out = nullptr;
-  if (which == 3 && c.n_constraints == 0) return NB200_ERR_STATE;   // nothing to check (the check has no interpreter: any length is compiled)
-  if (which != 3 && ((which == 1 ? c.logup_prog.size() : c.prog.size()) < JIT_MIN_INSTR || (which == 1 && c.n_logup_cols() == 0))) return NB200_ERR_STATE;  // runs on the interpreter
-  if (which == 2 && count_high(high_constraints(c)) == 0) return NB200_ERR_STATE;   // nothing to evaluate on D2
-  std::string src = which == 3 ? jit_check_source(c) : which == 1 ? jit_logup_source(c) : jit_source(c, which == 2);
+  if (!jit_specialised(kind, c, a->fracs[component])) return NB200_ERR_STATE;
+  const std::string src = jit_kernel_source(kind, c, a->fracs[component]);
   char* o = (char*)malloc(src.size() + 1);
   if (!o) return NB200_ERR_OOM;
   memcpy(o, src.c_str(), src.size() + 1);
   *out = o;
   return NB200_OK;
+}
+nb200_status nb200_air_kernel_source(const nb200_air* a, uint32_t component, int which, char** out) {
+  if (!a || !out || component >= a->prog.comps.size() || which < 0 || which > 3) return NB200_ERR_ARG;
+  *out = nullptr;
+  return kernel_source(a, component, (JitKind)which, out);
 }
 
 // ---- CommitmentSchemeProver ----
@@ -1694,18 +1694,9 @@ nb200_status nb200_air_lookup_tables(const nb200_air* a, uint32_t component, uin
 nb200_status nb200_air_count_kernel_source(const nb200_air* a, uint32_t component, char** out) {
   if (!a || !out || component >= a->prog.comps.size()) return NB200_ERR_ARG;
   *out = nullptr;
-  bool any = false;
-  for (const AirFrac& f : a->fracs[component]) {
+  for (const AirFrac& f : a->fracs[component])
     if (f.kind == FRAC_BAD) return NB200_ERR_ARG;
-    any = any || f.kind == FRAC_TABLE || f.kind == FRAC_LOOKUP;
-  }
-  if (!any) return NB200_ERR_STATE;   // neither a table nor a lookup: nothing to count
-  const std::string src = jit_count_source(a->prog.comps[component], a->fracs[component]);
-  char* o = (char*)malloc(src.size() + 1);
-  if (!o) return NB200_ERR_OOM;
-  memcpy(o, src.c_str(), src.size() + 1);
-  *out = o;
-  return NB200_OK;
+  return kernel_source(a, component, JIT_COUNT, out);
 }
 
 // ---- backend-trait level operations (the per-trait surface a `CudaBackend` shim binds; the coarse nb200_prove runs the same code) ----

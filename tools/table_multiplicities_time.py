@@ -30,7 +30,7 @@ def card():
 
 
 def nvrtc_compile_ms(words):
-    """{component: ms} of one NVRTC compile of each component's count kernel (the options of csrc/jit.cu jit_compile_source)."""
+    """{component: ms} of one NVRTC compile of each component's count kernel (the options of csrc/jit.cu jit_compile)."""
     import ctypes as C
     import numpy as np
 
