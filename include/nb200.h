@@ -168,6 +168,23 @@ nb200_status nb200_commit_host_packed(nb200_ctx*, const void* const* host_batche
 nb200_status nb200_keccak_main_trace(nb200_ctx*, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
                                      nb200_cols** out);
 
+/* ---- RamInitFinal's main trace, filled on the device from the keccak side note and the public initial memory -------------------
+ * The reference builds RamInitFinal's columns (prover/src/extensions/ram_init_final.rs:458-511) on the host from the side note's
+ * `last_access` map: one row per RAM byte address in ascending order, with the address bytes, the flag 1, the final value and the
+ * final access counter bytes.  Here the map is rebuilt on the device from the same inputs nb200_keccak_main_trace takes plus the
+ * public initial memory (n_init entries, init_addresses strictly ascending, init_values one byte each): permutation p reads the 200
+ * bytes at addresses[p] with previous counters timestamps[p][k] and leaves the bytes of Keccak-f[1600](inputs[p]) with counter
+ * timestamps[p][k] + 1; an initial-memory entry no permutation touches keeps its value with counter 0.  Rows are ordered by address,
+ * and for each address the last access in permutation order gives the final state.
+ * out: a caller-owned batch of 10 columns and 2^log_size rows, overwritten in finalized order; rows past the last address are zero.
+ * *n_rows_out = the number of distinct addresses.
+ * NB200_ERR_ARG: n_perms == 0 or above 2^18, an address above 2^32 - 200, a timestamp of 2^32 - 1, init addresses not strictly
+ * ascending, more than 2^30 init entries, log_size outside [4, 30], `out` of another shape, or more distinct addresses than 2^log_size
+ * (then *n_rows_out still holds the count: learning it costs one device-to-host read).  Scratch memory is released in stream order. */
+nb200_status nb200_ram_init_final_trace(nb200_ctx*, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
+                                        size_t n_init, const uint32_t* init_addresses, const uint8_t* init_values, uint32_t log_size,
+                                        nb200_cols* out, size_t* n_rows_out);
+
 /* ---- one commitment over N GPUs (SURVEY §8e; one process per GPU, NCCL over NVLink inside the library) ------------------------
  * The reference has no multi-device path (SURVEY App. C); these entry points are what a multi-GPU `CudaBackend` would drive from
  * TreeBuilder::commit (machine.rs:208-263).  Rank 0 creates the id and hands it to the other ranks out of band (MPI, a file,

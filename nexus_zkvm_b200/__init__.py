@@ -249,6 +249,27 @@ class Context:
                                                 ts.ctypes.data_as(u32p), out))
         return [Columns(self, C.c_void_p(out[i])) for i in range(5)]
 
+    def ram_init_final_trace(self, inputs, addresses, timestamps, init_addresses, init_values, log_size, out=None):
+        """nb200_ram_init_final_trace: RamInitFinal's 10 main columns in finalized order, filled on the device from the keccak side note (as
+        keccak_main_trace takes it) and the public initial memory (init_addresses: (n_init,) uint32, strictly ascending; init_values:
+        (n_init,) bytes).  `out`: a batch of 10 columns of 2^log_size rows to overwrite (default: a new one).  Returns (out, number of
+        distinct addresses)."""
+        inp = np.ascontiguousarray(inputs, dtype=np.uint64)
+        addr = np.ascontiguousarray(addresses, dtype=np.uint32)
+        ts = np.ascontiguousarray(timestamps, dtype=np.uint32)
+        n = inp.shape[0] if inp.ndim == 2 else 0
+        assert inp.shape == (n, 25) and addr.shape == (n,) and ts.shape == (n, 200), "side note shapes"
+        ia = np.ascontiguousarray(init_addresses, dtype=np.uint32)
+        iv = np.ascontiguousarray(init_values, dtype=np.uint8)
+        assert ia.shape == iv.shape and ia.ndim == 1, "initial memory shapes"
+        if out is None:
+            out = self.alloc(10, log_size)
+        n_rows = C.c_size_t()
+        self._chk(lib().nb200_ram_init_final_trace(self._h, C.c_size_t(n), inp.ctypes.data_as(u64p), addr.ctypes.data_as(u32p), ts.ctypes.data_as(u32p),
+                                                   C.c_size_t(ia.size), ia.ctypes.data_as(u32p), iv.ctypes.data_as(u8p), C.c_uint32(log_size),
+                                                   out._h, C.byref(n_rows)))
+        return out, int(n_rows.value)
+
     def table_multiplicities(self, air, tree0, tree1):
         """nb200_table_multiplicities: every table fraction's multiplicity column of `tree1` (device batches, finalized order) is overwritten
         with the count of the AIR's lookups into it.  `air` is a loaded AIR (prover.Air).  Returns (n_unmatched, first_unmatched), the latter

@@ -26,6 +26,9 @@ nb200_status merkle_decommit(nb200_ctx* ctx, const nb200_tree* tree, const std::
 nb200_status eval_at_points(nb200_ctx* ctx, const u32* coeffs, size_t n_cols, u32 log_size, const u32* points_xy, size_t n_points, u32* out_qm31);
 nb200_status keccak_main_trace(nb200_ctx* ctx, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
                                nb200_cols** out);
+nb200_status ram_init_final_trace(nb200_ctx* ctx, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
+                                  size_t n_init, const uint32_t* init_addresses, const uint8_t* init_values, uint32_t log_size, nb200_cols* out,
+                                  size_t* n_rows_out);
 }  // namespace nb
 using namespace nb;
 
@@ -462,6 +465,14 @@ nb200_status nb200_keccak_main_trace(nb200_ctx* ctx, size_t n_perms, const uint6
                                      nb200_cols** out) {
   if (!ctx) return NB200_ERR_ARG;
   return keccak_main_trace(ctx, n_perms, inputs, addresses, timestamps, out);
+}
+
+// ---- RamInitFinal's main trace from the keccak side note and the public initial memory (csrc/ram_init_final.cu) ----
+nb200_status nb200_ram_init_final_trace(nb200_ctx* ctx, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
+                                        size_t n_init, const uint32_t* init_addresses, const uint8_t* init_values, uint32_t log_size,
+                                        nb200_cols* out, size_t* n_rows_out) {
+  if (!ctx) return NB200_ERR_ARG;
+  return ram_init_final_trace(ctx, n_perms, inputs, addresses, timestamps, n_init, init_addresses, init_values, log_size, out, n_rows_out);
 }
 
 }  // extern "C"

@@ -90,6 +90,238 @@ R8 = [("INoShift", ["OpC8_10"]), ("J", ["OpC1_3", "OpC8_10"]), ("B", ["OpC5_7", 
 R32 = ["OpA", "OpB", "Reg1Address", "Reg2Address", "Reg3Address"]
 
 
+def main_preprocessed_columns(log_size):
+    """The main component's 18 preprocessed and 9 program columns for an empty program: {column id: (2^log_size,) uint32}."""
+    n = 1 << log_size
+    out = {}
+
+    def put(name, limbs):
+        for i, v in enumerate(limbs):
+            out[f"{name}_{i}"] = v
+
+    z = np.zeros(n, np.uint32)
+    first, last = z.copy(), z.copy()
+    first[0], last[n - 1] = 1, 1
+    put("IsFirst", [first]); put("IsLast", [last])
+    clk = np.arange(1, n + 1, dtype=np.uint64)                              # preprocessed.rs:75-100
+    le = lambda x: [((x >> (8 * k)) & 0xFF).astype(np.uint32) for k in range(4)]
+    put("Clk", le(clk)); put("Reg1TsCur", le(3 * clk + 1)); put("Reg2TsCur", le(3 * clk + 2)); put("Reg3TsCur", le(3 * clk + 3))
+    for name, size in PROGRAM_COLUMNS:                                      # empty program: the program trace is all zero
+        put(name, [z] * size)
+    return out
+
+
+def padding_witness(log_size, seed=0):
+    """The main component's padding-only witness (NexusV1Machine's docstring): {column name: its limbs, (2^log_size,) uint32 each}."""
+    n = 1 << log_size
+    rng = np.random.default_rng(seed)
+    t = {name: [np.zeros(n, np.uint32) for _ in range(size)] for name, size in MAIN_COLUMNS}
+    t["IsPadding"][0][:] = 1
+    t["ValueAEffectiveFlagAux"][0][:] = 1
+    t["ValueAEffectiveFlagAuxInv"][0][:] = 1
+    rb = lambda: rng.integers(0, 256, n, dtype=np.uint64).astype(np.uint32)
+    free_words = [w for w in R256_WORDS if w not in ("Reg1TsPrev", "Reg2TsPrev", "Reg3TsPrev", "CReg1TsPrev", "CReg2TsPrev", "CReg3TsPrev")]
+    for w in free_words + R256_HALF_WORDS + R256_BYTES + ["ValueAEffective", "Reg1ValPrev", "Reg2ValPrev", "Reg3ValPrev", "PcNext"]:
+        if w == "ValueAEffective":
+            continue                                                    # = ValueA * flag = 0 (register_mem_check.rs:129-136)
+        for limb in t[w]:
+            limb[:] = rb()
+    for limb in t["Pc"]:
+        limb[0] = 0                                                    # is_first * (pc - PrgInitialPc) with an empty program
+    for w in ("ValueA4_7", "ValueB4_7", "ValueC4_7"):                   # high nibbles of the (free) values; only looked up when a bit-op flag is set
+        src = {"ValueA4_7": "ValueA", "ValueB4_7": "ValueB", "ValueC4_7": "ValueC"}[w]
+        for k in range(4):
+            t[w][k][:] = t[src][k] >> 4
+    for w in ("OpB", "Reg1Address", "Reg2Address", "Reg3Address"):       # Range32-checked; OpA = ValueAEffectiveFlag / aux = 0
+        t[w][0][:] = rng.integers(0, 32, n, dtype=np.uint64).astype(np.uint32)
+    # timestamps: prev < cur = 3 clk + k, c = cur - 1 - prev with the chip's per-16-bit borrows (timestamp.rs:101-150)
+    clk = np.arange(1, n + 1, dtype=np.uint64)
+    for k in (1, 2, 3):
+        cur = 3 * clk + k
+        prev = (rng.integers(0, 1 << 62, n, dtype=np.uint64) % cur).astype(np.uint64)
+        cc = cur - 1 - prev
+        lo = (cc & 0xFFFF) + (prev & 0xFFFF) + 1
+        b0 = (lo >> 16).astype(np.uint32)
+        hi = (cc >> 16) + (prev >> 16) + b0
+        assert np.all(lo - (b0.astype(np.uint64) << 16) == (cur & 0xFFFF)) and np.all(hi == (cur >> 16))
+        for i in range(4):
+            t[f"Reg{k}TsPrev"][i][:] = ((prev >> (8 * i)) & 0xFF).astype(np.uint32)
+            t[f"CReg{k}TsPrev"][i][:] = ((cc >> (8 * i)) & 0xFF).astype(np.uint32)
+        t[f"CH{k}Minus"][0][:] = b0
+    return t
+
+
+def record_main_component(air, log_size, rel, keccak=False):
+    """Record the main component (`MachineEval<BaseComponent>`, NexusV1Machine's docstring) into `air`: the chips in BaseComponent's order
+    against the relations `rel` (name -> air.Relation: BitOp, LoadStore, ProgramCheck, RegisterCheck, Range8/16/32/128/256), then
+    `finalize_logup()`.  `keccak`: the keccak extension is enabled, so KeccakChip (CustomInstructionChip, after LoadStoreChip) adds its
+    booleanity constraint on IsCustomKeccak (chips/custom.rs:178-196).  Returns (component, {column name: its masks})."""
+    m = air.component(log_size, 2)
+    pre, col = {}, {}
+    for name, size in PREPROCESSED_COLUMNS + PROGRAM_COLUMNS:           # TraceEval::new: preprocessed ids, then program ids
+        pre[name] = [m.get_preprocessed_column(f"{name}_{i}") for i in range(size)]
+    nxt = {}
+    for name, size in MAIN_COLUMNS:
+        if name in ("Pc", "IsPadding"):                                 # Column::reads_next_row_mask
+            pairs = [m.next_interaction_mask(A.ORIGINAL_TRACE_IDX, [0, 1]) for _ in range(size)]
+            col[name], nxt[name] = [p[0] for p in pairs], [p[1] for p in pairs]
+        else:
+            col[name] = [m.next_trace_mask() for _ in range(size)]
+
+    def ssum(names):
+        acc = col[names[0]][0]
+        for n in names[1:]:
+            acc = acc + col[n][0]
+        return acc
+
+    c = lambda n: col[n][0]
+    imm_c = c("ImmC")
+    is_type_r = (1 - imm_c) * ssum(TYPE_R_OPS)
+    is_load, is_type_s, is_type_sys, is_type_u = ssum(IS_LOAD), ssum(IS_TYPE_S), ssum(IS_TYPE_SYS), ssum(IS_TYPE_U)
+    is_type_b, is_type_j = ssum(IS_TYPE_B), c("IsJal")
+    alu_imm_no_shift, alu_imm_shift = imm_c * ssum(ALU_IMM_NO_SHIFT), imm_c * ssum(ALU_IMM_SHIFT)
+    is_type_i_no_shift = is_load + alu_imm_no_shift + c("IsJalr")
+    is_type_i = is_load + c("IsJalr") + alu_imm_no_shift + alu_imm_shift
+    op_b_flag = ssum(OP_B_FLAG)
+    is_pc_incremented = ssum(IS_ALU) + is_load + is_type_s + is_type_sys * (1 - c("IsSysHalt")) + is_type_u + c("IsCustomKeccak")
+    reg3_accessed = (is_type_s + is_type_b + is_type_r + is_type_i + is_type_u + is_type_j
+                     + is_type_sys * (c("IsSysPrivInput") + c("IsSysHeapReset") + c("IsSysStackReset")))
+    vtype = {"R": is_type_r, "U": is_type_u, "INoShift": is_type_i_no_shift, "IShift": alu_imm_shift, "J": is_type_j, "B": is_type_b, "S": is_type_s}
+
+    # ---------------- CpuChip (cpu.rs:318-566) ----------------
+    is_padding, next_is_padding = c("IsPadding"), nxt["IsPadding"][0]
+    next_is_first = pre["IsLast"][0]
+    m.add_constraint((1 - next_is_first) * is_padding * (1 - next_is_padding))
+    m.add_constraint(c("ValueAEffectiveFlagAux") * c("ValueAEffectiveFlagAuxInv") - 1)
+    op_a, op_b, op_c = c("OpA"), c("OpB"), c("OpC")
+    m.add_constraint(op_a * c("ValueAEffectiveFlagAux") - c("ValueAEffectiveFlag"))
+    m.add_constraint(ssum(CPU_OP_FLAGS) + is_padding + c("IsCustomKeccak") - 1)
+    r1a, r2a, r3a = c("Reg1Address"), c("Reg2Address"), c("Reg3Address")
+    m.add_constraint((is_type_r + is_type_i) * (op_b - r1a))
+    m.add_constraint(is_type_r * (op_c - r2a))
+    m.add_constraint((is_type_r + is_type_i) * (op_a - r3a))
+    r1v, r2v, r3v = col["Reg1ValPrev"], col["Reg2ValPrev"], col["Reg3ValPrev"]
+    va, vb, vc = col["ValueA"], col["ValueB"], col["ValueC"]
+    for k in (0, 2):
+        m.add_constraint(op_b_flag * (r1v[k] + r1v[k + 1] * 256 - (vb[k] + vb[k + 1] * 256)))
+        m.add_constraint(is_type_r * (r2v[k] + r2v[k + 1] * 256 - (vc[k] + vc[k + 1] * 256)))
+    is_type_b_s = is_type_b + is_type_s
+    m.add_constraint(is_type_b_s * (op_b - r1a))
+    m.add_constraint(is_type_b_s * (op_a - r3a))
+    for k in (0, 2):
+        m.add_constraint(is_type_b_s * (r3v[k] + r3v[k + 1] * 256 - va[k] - va[k + 1] * 256))
+    is_sys_halt = c("IsSysHalt")
+    m.add_constraint(is_type_sys * (op_b - r1a))
+    m.add_constraint(is_type_sys * (op_c - r2a))
+    m.add_constraint(is_type_sys * (op_a - r3a))
+    pc, pc_next, pc_carry, pc_on_next_row = col["Pc"], col["PcNext"], col["PcCarry"], nxt["Pc"]
+    for k in (0, 2):
+        m.add_constraint((1 - next_is_first) * (1 - next_is_padding)
+                         * (pc_next[k] + pc_next[k + 1] * 256 - (pc_on_next_row[k] + pc_on_next_row[k + 1] * 256)))
+    m.add_constraint(is_pc_incremented * (pc_next[0] + pc_next[1] * 256 + pc_carry[0] * 65536 - (pc[0] + pc[1] * 256) - 4))
+    m.add_constraint(is_pc_incremented * (pc_next[2] + pc_next[3] * 256 + pc_carry[1] * 65536 - (pc[2] + pc[3] * 256) - pc_carry[0]))
+    for k in (0, 2):
+        m.add_constraint(is_type_sys * is_sys_halt * (pc[k] + pc[k + 1] * 256 - (pc_next[k] + pc_next[k + 1] * 256)))
+    # ---------------- AddChip / SubChip ----------------
+    cf = col["CarryFlag"]
+    is_add, is_sub = c("IsAdd"), c("IsSub")
+    m.add_constraint(is_add * (va[0] + va[1] * 256 + cf[0] * 65536 - (vb[0] + vb[1] * 256 + vc[0] + vc[1] * 256)))
+    m.add_constraint(is_add * (va[2] + va[3] * 256 + cf[1] * 65536 - (vb[2] + vb[3] * 256 + vc[2] + vc[3] * 256 + cf[0])))
+    m.add_constraint(is_sub * (va[0] + va[1] * 256 - cf[0] * 65536 - (vb[0] + vb[1] * 256 - vc[0] - vc[1] * 256)))
+    m.add_constraint(is_sub * (va[2] + va[3] * 256 - cf[1] * 65536 - (vb[2] + vb[3] * 256 - vc[2] - vc[3] * 256 - cf[0])))
+    # ---------------- BitOpChip: lookup structure (bit_op.rs:380-431; 4 limbs x {And, Or, Xor} x {low, high nibble} = 24 fractions) ----------------
+    va47, vb47, vc47 = col["ValueA4_7"], col["ValueB4_7"], col["ValueC4_7"]
+    for k in range(4):
+        for op_code, flag in ((1, c("IsAnd")), (2, c("IsOr")), (3, c("IsXor"))):
+            m.add_to_relation(rel["BitOp"], flag, [m.const(op_code), vb[k] - vb47[k] * 16, vc[k] - vc47[k] * 16, va[k] - va47[k] * 16])
+            m.add_to_relation(rel["BitOp"], flag, [m.const(op_code), vb47[k], vc47[k], va47[k]])
+    # ---------------- LoadStoreChip: lookup structure (load_store.rs:650-685,788-903; 4 bytes x {subtract prev, add cur} = 8 fractions) ----------------
+    ram1 = ssum(["IsSb", "IsSh", "IsSw", "IsLb", "IsLh", "IsLbu", "IsLhu", "IsLw"])
+    ram2 = ssum(["IsSh", "IsSw", "IsLh", "IsLhu", "IsLw"])
+    ram34 = ssum(["IsSw", "IsLw"])
+    base, clk = col["RamBaseAddr"], pre["Clk"]
+    for off, acc in ((0, ram1), (1, ram2), (2, ram34), (3, ram34)):
+        addr_lo, addr_hi = base[0] + off + base[1] * 256, base[2] + base[3] * 256
+        ts = col[f"Ram{off + 1}TsPrev"]
+        m.add_to_relation(rel["LoadStore"], -acc, [addr_lo, addr_hi, c(f"Ram{off + 1}ValPrev"), ts[0] + ts[1] * 256, ts[2] + ts[3] * 256])
+        m.add_to_relation(rel["LoadStore"], acc, [addr_lo, addr_hi, c(f"Ram{off + 1}ValCur"), clk[0] + clk[1] * 256, clk[2] + clk[3] * 256])
+    # ---------------- KeccakChip in CustomInstructionChip (chips/custom.rs:178-196), with the keccak extension enabled ----------------
+    if keccak:
+        m.add_constraint(c("IsCustomKeccak") * (1 - c("IsCustomKeccak")))
+    # ---------------- ProgramMemCheckChip (program_mem_check.rs:152-200 and the four constrain_* helpers :255-537) ----------------
+    is_first = pre["IsFirst"][0]
+    for k in range(4):
+        m.add_constraint(is_first * (pc[k] - pre["PrgInitialPc"][k]))
+    pcur, pprev, pcarry = col["ProgCtrCur"], col["ProgCtrPrev"], col["ProgCtrCarry"]
+    m.add_constraint((1 - is_padding) * (pcur[0] + pcur[1] * 256 + pcarry[0] * 65536 - (pprev[0] + pprev[1] * 256 + 1)))
+    m.add_constraint((1 - is_padding) * (pcur[2] + pcur[3] * 256 + pcarry[1] * 65536 - (pprev[2] + pprev[3] * 256 + pcarry[0])))
+    m.add_constraint(pcarry[1])
+    pm_pc, pm_word, pm_flag = pre["PrgMemoryPc"], pre["PrgMemoryWord"], pre["PrgMemoryFlag"][0]
+    zero = m.const(0)
+    m.add_to_relation(rel["ProgramCheck"], pm_flag, pm_pc + pm_word + [zero] * 4)                       # add_initial_digest
+    m.add_to_relation(rel["ProgramCheck"], -pm_flag, pm_pc + pm_word + col["FinalPrgMemoryCtr"])        # subtract_final_digest
+    iv = col["InstrVal"]
+    acc_tuple = [pc[0] + pc[1] * 256, pc[2] + pc[3] * 256, iv[0] + iv[1] * 256, iv[2] + iv[3] * 256]
+    m.add_to_relation(rel["ProgramCheck"], -(1 - is_padding), acc_tuple + pprev)                         # subtract_access
+    m.add_to_relation(rel["ProgramCheck"], 1 - is_padding, acc_tuple + pcur)                             # add_access
+    # ---------------- RegisterMemCheckChip ----------------
+    vae, vaef = col["ValueAEffective"], c("ValueAEffectiveFlag")
+    for k in range(4):
+        m.add_constraint(vae[k] - va[k] * vaef)
+    for flag, addr, ts, val in ((op_b_flag, "Reg1Address", col["Reg1TsPrev"], r1v), (is_type_r, "Reg2Address", col["Reg2TsPrev"], r2v),
+                                (reg3_accessed, "Reg3Address", col["Reg3TsPrev"], r3v)):
+        m.add_to_relation(rel["RegisterCheck"], -flag, [c(addr)] + ts + val)
+    for flag, addr, ts, val in ((op_b_flag, "Reg1Address", pre["Reg1TsCur"], vb), (is_type_r, "Reg2Address", pre["Reg2TsCur"], vc),
+                                (reg3_accessed, "Reg3Address", pre["Reg3TsCur"], vae)):
+        m.add_to_relation(rel["RegisterCheck"], flag, [c(addr)] + ts + val)
+    # ---------------- TimestampChip ----------------
+    chm = [col["CH1Minus"], col["CH2Minus"], col["CH3Minus"]]
+    for k in range(3):
+        m.add_constraint(chm[k][1])
+    for k, (cprev, cur, prev) in enumerate(((col["CReg1TsPrev"], pre["Reg1TsCur"], col["Reg1TsPrev"]),
+                                            (col["CReg2TsPrev"], pre["Reg2TsCur"], col["Reg2TsPrev"]),
+                                            (col["CReg3TsPrev"], pre["Reg3TsCur"], col["Reg3TsPrev"]))):
+        m.add_constraint(cprev[0] + cprev[1] * 256 + prev[0] + prev[1] * 256 + 1 - (chm[k][0] * 65536 + cur[0] + cur[1] * 256))
+        m.add_constraint(cprev[2] + cprev[3] * 256 + prev[2] + prev[3] * 256 + chm[k][0] - (chm[k][1] * 65536 + cur[2] + cur[3] * 256))
+    # ---------------- RangeCheckChip = (Range8, Range16, Range32, Range128, Range256, RangeBool) ----------------
+    for t, cols_ in R8:
+        for n in cols_:
+            m.add_to_relation(rel["Range8"], vtype[t], [c(n)])
+    m.add_to_relation(rel["Range8"], ssum(ALU_IMM_SHIFT), [col["Helper1"][0]])          # Helper1MsbChecked = IsSll + IsSrl + IsSra
+    for t, cols_ in R16:
+        for n in cols_:
+            m.add_to_relation(rel["Range16"], vtype[t], [c(n)])
+    for n in R32:
+        m.add_to_relation(rel["Range32"], 1, [c(n)])
+    num = c("IsSlt") + c("IsBge") + c("IsBlt")
+    for n in ("Helper2", "Helper3"):
+        m.add_to_relation(rel["Range128"], num, [col[n][3]])
+    m.add_to_relation(rel["Range128"], c("IsJalr"), [c("QtAux")])
+    m.add_to_relation(rel["Range128"], c("IsSra"), [col["Helper2"][0]])
+    m.add_to_relation(rel["Range128"], c("IsLh") + c("IsLb"), [c("QtAux")])
+    for n in R256_WORDS:
+        for limb in col[n]:
+            m.add_to_relation(rel["Range256"], 1, [limb])
+    for n in R256_HALF_WORDS:
+        for limb in col[n]:
+            m.add_to_relation(rel["Range256"], 1, [limb])
+    for n in R256_BYTES:
+        m.add_to_relation(rel["Range256"], 1, [c(n)])
+    for n in R256_TYPE_U_BYTES:
+        m.add_to_relation(rel["Range256"], is_type_u, [c(n)])
+    for n in BOOL_SINGLE:
+        m.add_constraint(c(n) * (c(n) - 1))
+    for n in BOOL_HALF_WORD:
+        for limb in col[n]:
+            m.add_constraint(limb * (limb - 1))
+    for t, names in (("R", BOOL_TYPE_R), ("INoShift", BOOL_TYPE_I_NO_SHIFT), ("IShift", BOOL_TYPE_I_SHIFT), ("J", BOOL_TYPE_J),
+                     ("B", BOOL_TYPE_B), ("S", BOOL_TYPE_S)):
+        for n in names:
+            m.add_constraint(vtype[t] * c(n) * (c(n) - 1))
+    m.finalize_logup()                                                     # components/mod.rs:52-54
+    return m, col
+
+
 class NexusV1Machine:
     """The reference's v1 main component (`MachineEval<BaseComponent>`, nexus-zkvm prover/src/components/mod.rs:39-57) recorded as data —
     the REAL trace layout (all 347 main columns of prover/src/column.rs:22-604 in enum order, `Pc` and `IsPadding` with the [0, 1] mask of
@@ -128,167 +360,8 @@ class NexusV1Machine:
         self.rel8, self.rel16, self.rel32 = air.relation("Range8", 1), air.relation("Range16", 1), air.relation("Range32", 1)
         self.rel128, self.rel256 = air.relation("Range128", 1), air.relation("Range256", 1)
         self.relations = [self.rel_bitop, self.rel_ls, self.rel_prog, self.rel_reg, self.rel8, self.rel16, self.rel32, self.rel128, self.rel256]
-        m = air.component(log_size, 2)
-        pre, col = {}, {}
-        for name, size in PREPROCESSED_COLUMNS + PROGRAM_COLUMNS:           # TraceEval::new: preprocessed ids, then program ids
-            pre[name] = [m.get_preprocessed_column(f"{name}_{i}") for i in range(size)]
-        nxt = {}
-        for name, size in MAIN_COLUMNS:
-            if name in ("Pc", "IsPadding"):                                 # Column::reads_next_row_mask
-                pairs = [m.next_interaction_mask(A.ORIGINAL_TRACE_IDX, [0, 1]) for _ in range(size)]
-                col[name], nxt[name] = [p[0] for p in pairs], [p[1] for p in pairs]
-            else:
-                col[name] = [m.next_trace_mask() for _ in range(size)]
+        m, _col = record_main_component(air, log_size, {r.name: r for r in self.relations})
         self.n_main = sum(s for _, s in MAIN_COLUMNS)
-
-        def ssum(names):
-            acc = col[names[0]][0]
-            for n in names[1:]:
-                acc = acc + col[n][0]
-            return acc
-
-        c = lambda n: col[n][0]
-        imm_c = c("ImmC")
-        is_type_r = (1 - imm_c) * ssum(TYPE_R_OPS)
-        is_load, is_type_s, is_type_sys, is_type_u = ssum(IS_LOAD), ssum(IS_TYPE_S), ssum(IS_TYPE_SYS), ssum(IS_TYPE_U)
-        is_type_b, is_type_j = ssum(IS_TYPE_B), c("IsJal")
-        alu_imm_no_shift, alu_imm_shift = imm_c * ssum(ALU_IMM_NO_SHIFT), imm_c * ssum(ALU_IMM_SHIFT)
-        is_type_i_no_shift = is_load + alu_imm_no_shift + c("IsJalr")
-        is_type_i = is_load + c("IsJalr") + alu_imm_no_shift + alu_imm_shift
-        op_b_flag = ssum(OP_B_FLAG)
-        is_pc_incremented = ssum(IS_ALU) + is_load + is_type_s + is_type_sys * (1 - c("IsSysHalt")) + is_type_u + c("IsCustomKeccak")
-        reg3_accessed = (is_type_s + is_type_b + is_type_r + is_type_i + is_type_u + is_type_j
-                         + is_type_sys * (c("IsSysPrivInput") + c("IsSysHeapReset") + c("IsSysStackReset")))
-        vtype = {"R": is_type_r, "U": is_type_u, "INoShift": is_type_i_no_shift, "IShift": alu_imm_shift, "J": is_type_j, "B": is_type_b, "S": is_type_s}
-
-        # ---------------- CpuChip (cpu.rs:318-566) ----------------
-        is_padding, next_is_padding = c("IsPadding"), nxt["IsPadding"][0]
-        next_is_first = pre["IsLast"][0]
-        m.add_constraint((1 - next_is_first) * is_padding * (1 - next_is_padding))
-        m.add_constraint(c("ValueAEffectiveFlagAux") * c("ValueAEffectiveFlagAuxInv") - 1)
-        op_a, op_b, op_c = c("OpA"), c("OpB"), c("OpC")
-        m.add_constraint(op_a * c("ValueAEffectiveFlagAux") - c("ValueAEffectiveFlag"))
-        m.add_constraint(ssum(CPU_OP_FLAGS) + is_padding + c("IsCustomKeccak") - 1)
-        r1a, r2a, r3a = c("Reg1Address"), c("Reg2Address"), c("Reg3Address")
-        m.add_constraint((is_type_r + is_type_i) * (op_b - r1a))
-        m.add_constraint(is_type_r * (op_c - r2a))
-        m.add_constraint((is_type_r + is_type_i) * (op_a - r3a))
-        r1v, r2v, r3v = col["Reg1ValPrev"], col["Reg2ValPrev"], col["Reg3ValPrev"]
-        va, vb, vc = col["ValueA"], col["ValueB"], col["ValueC"]
-        for k in (0, 2):
-            m.add_constraint(op_b_flag * (r1v[k] + r1v[k + 1] * 256 - (vb[k] + vb[k + 1] * 256)))
-            m.add_constraint(is_type_r * (r2v[k] + r2v[k + 1] * 256 - (vc[k] + vc[k + 1] * 256)))
-        is_type_b_s = is_type_b + is_type_s
-        m.add_constraint(is_type_b_s * (op_b - r1a))
-        m.add_constraint(is_type_b_s * (op_a - r3a))
-        for k in (0, 2):
-            m.add_constraint(is_type_b_s * (r3v[k] + r3v[k + 1] * 256 - va[k] - va[k + 1] * 256))
-        is_sys_halt = c("IsSysHalt")
-        m.add_constraint(is_type_sys * (op_b - r1a))
-        m.add_constraint(is_type_sys * (op_c - r2a))
-        m.add_constraint(is_type_sys * (op_a - r3a))
-        pc, pc_next, pc_carry, pc_on_next_row = col["Pc"], col["PcNext"], col["PcCarry"], nxt["Pc"]
-        for k in (0, 2):
-            m.add_constraint((1 - next_is_first) * (1 - next_is_padding)
-                             * (pc_next[k] + pc_next[k + 1] * 256 - (pc_on_next_row[k] + pc_on_next_row[k + 1] * 256)))
-        m.add_constraint(is_pc_incremented * (pc_next[0] + pc_next[1] * 256 + pc_carry[0] * 65536 - (pc[0] + pc[1] * 256) - 4))
-        m.add_constraint(is_pc_incremented * (pc_next[2] + pc_next[3] * 256 + pc_carry[1] * 65536 - (pc[2] + pc[3] * 256) - pc_carry[0]))
-        for k in (0, 2):
-            m.add_constraint(is_type_sys * is_sys_halt * (pc[k] + pc[k + 1] * 256 - (pc_next[k] + pc_next[k + 1] * 256)))
-        # ---------------- AddChip / SubChip ----------------
-        cf = col["CarryFlag"]
-        is_add, is_sub = c("IsAdd"), c("IsSub")
-        m.add_constraint(is_add * (va[0] + va[1] * 256 + cf[0] * 65536 - (vb[0] + vb[1] * 256 + vc[0] + vc[1] * 256)))
-        m.add_constraint(is_add * (va[2] + va[3] * 256 + cf[1] * 65536 - (vb[2] + vb[3] * 256 + vc[2] + vc[3] * 256 + cf[0])))
-        m.add_constraint(is_sub * (va[0] + va[1] * 256 - cf[0] * 65536 - (vb[0] + vb[1] * 256 - vc[0] - vc[1] * 256)))
-        m.add_constraint(is_sub * (va[2] + va[3] * 256 - cf[1] * 65536 - (vb[2] + vb[3] * 256 - vc[2] - vc[3] * 256 - cf[0])))
-        # ---------------- BitOpChip: lookup structure (bit_op.rs:380-431; 4 limbs x {And, Or, Xor} x {low, high nibble} = 24 fractions) ----------------
-        va47, vb47, vc47 = col["ValueA4_7"], col["ValueB4_7"], col["ValueC4_7"]
-        for k in range(4):
-            for op_code, flag in ((1, c("IsAnd")), (2, c("IsOr")), (3, c("IsXor"))):
-                m.add_to_relation(self.rel_bitop, flag, [m.const(op_code), vb[k] - vb47[k] * 16, vc[k] - vc47[k] * 16, va[k] - va47[k] * 16])
-                m.add_to_relation(self.rel_bitop, flag, [m.const(op_code), vb47[k], vc47[k], va47[k]])
-        # ---------------- LoadStoreChip: lookup structure (load_store.rs:650-685,788-903; 4 bytes x {subtract prev, add cur} = 8 fractions) ----------------
-        ram1 = ssum(["IsSb", "IsSh", "IsSw", "IsLb", "IsLh", "IsLbu", "IsLhu", "IsLw"])
-        ram2 = ssum(["IsSh", "IsSw", "IsLh", "IsLhu", "IsLw"])
-        ram34 = ssum(["IsSw", "IsLw"])
-        base, clk = col["RamBaseAddr"], pre["Clk"]
-        for off, acc in ((0, ram1), (1, ram2), (2, ram34), (3, ram34)):
-            addr_lo, addr_hi = base[0] + off + base[1] * 256, base[2] + base[3] * 256
-            ts = col[f"Ram{off + 1}TsPrev"]
-            m.add_to_relation(self.rel_ls, -acc, [addr_lo, addr_hi, c(f"Ram{off + 1}ValPrev"), ts[0] + ts[1] * 256, ts[2] + ts[3] * 256])
-            m.add_to_relation(self.rel_ls, acc, [addr_lo, addr_hi, c(f"Ram{off + 1}ValCur"), clk[0] + clk[1] * 256, clk[2] + clk[3] * 256])
-        # ---------------- ProgramMemCheckChip (program_mem_check.rs:152-200 and the four constrain_* helpers :255-537) ----------------
-        is_first = pre["IsFirst"][0]
-        for k in range(4):
-            m.add_constraint(is_first * (pc[k] - pre["PrgInitialPc"][k]))
-        pcur, pprev, pcarry = col["ProgCtrCur"], col["ProgCtrPrev"], col["ProgCtrCarry"]
-        m.add_constraint((1 - is_padding) * (pcur[0] + pcur[1] * 256 + pcarry[0] * 65536 - (pprev[0] + pprev[1] * 256 + 1)))
-        m.add_constraint((1 - is_padding) * (pcur[2] + pcur[3] * 256 + pcarry[1] * 65536 - (pprev[2] + pprev[3] * 256 + pcarry[0])))
-        m.add_constraint(pcarry[1])
-        pm_pc, pm_word, pm_flag = pre["PrgMemoryPc"], pre["PrgMemoryWord"], pre["PrgMemoryFlag"][0]
-        zero = m.const(0)
-        m.add_to_relation(self.rel_prog, pm_flag, pm_pc + pm_word + [zero] * 4)                       # add_initial_digest
-        m.add_to_relation(self.rel_prog, -pm_flag, pm_pc + pm_word + col["FinalPrgMemoryCtr"])        # subtract_final_digest
-        iv = col["InstrVal"]
-        acc_tuple = [pc[0] + pc[1] * 256, pc[2] + pc[3] * 256, iv[0] + iv[1] * 256, iv[2] + iv[3] * 256]
-        m.add_to_relation(self.rel_prog, -(1 - is_padding), acc_tuple + pprev)                         # subtract_access
-        m.add_to_relation(self.rel_prog, 1 - is_padding, acc_tuple + pcur)                             # add_access
-        # ---------------- RegisterMemCheckChip ----------------
-        vae, vaef = col["ValueAEffective"], c("ValueAEffectiveFlag")
-        for k in range(4):
-            m.add_constraint(vae[k] - va[k] * vaef)
-        for flag, addr, ts, val in ((op_b_flag, "Reg1Address", col["Reg1TsPrev"], r1v), (is_type_r, "Reg2Address", col["Reg2TsPrev"], r2v),
-                                    (reg3_accessed, "Reg3Address", col["Reg3TsPrev"], r3v)):
-            m.add_to_relation(self.rel_reg, -flag, [c(addr)] + ts + val)
-        for flag, addr, ts, val in ((op_b_flag, "Reg1Address", pre["Reg1TsCur"], vb), (is_type_r, "Reg2Address", pre["Reg2TsCur"], vc),
-                                    (reg3_accessed, "Reg3Address", pre["Reg3TsCur"], vae)):
-            m.add_to_relation(self.rel_reg, flag, [c(addr)] + ts + val)
-        # ---------------- TimestampChip ----------------
-        chm = [col["CH1Minus"], col["CH2Minus"], col["CH3Minus"]]
-        for k in range(3):
-            m.add_constraint(chm[k][1])
-        for k, (cprev, cur, prev) in enumerate(((col["CReg1TsPrev"], pre["Reg1TsCur"], col["Reg1TsPrev"]),
-                                                (col["CReg2TsPrev"], pre["Reg2TsCur"], col["Reg2TsPrev"]),
-                                                (col["CReg3TsPrev"], pre["Reg3TsCur"], col["Reg3TsPrev"]))):
-            m.add_constraint(cprev[0] + cprev[1] * 256 + prev[0] + prev[1] * 256 + 1 - (chm[k][0] * 65536 + cur[0] + cur[1] * 256))
-            m.add_constraint(cprev[2] + cprev[3] * 256 + prev[2] + prev[3] * 256 + chm[k][0] - (chm[k][1] * 65536 + cur[2] + cur[3] * 256))
-        # ---------------- RangeCheckChip = (Range8, Range16, Range32, Range128, Range256, RangeBool) ----------------
-        for t, cols_ in R8:
-            for n in cols_:
-                m.add_to_relation(self.rel8, vtype[t], [c(n)])
-        m.add_to_relation(self.rel8, ssum(ALU_IMM_SHIFT), [col["Helper1"][0]])          # Helper1MsbChecked = IsSll + IsSrl + IsSra
-        for t, cols_ in R16:
-            for n in cols_:
-                m.add_to_relation(self.rel16, vtype[t], [c(n)])
-        for n in R32:
-            m.add_to_relation(self.rel32, 1, [c(n)])
-        num = c("IsSlt") + c("IsBge") + c("IsBlt")
-        for n in ("Helper2", "Helper3"):
-            m.add_to_relation(self.rel128, num, [col[n][3]])
-        m.add_to_relation(self.rel128, c("IsJalr"), [c("QtAux")])
-        m.add_to_relation(self.rel128, c("IsSra"), [col["Helper2"][0]])
-        m.add_to_relation(self.rel128, c("IsLh") + c("IsLb"), [c("QtAux")])
-        for n in R256_WORDS:
-            for limb in col[n]:
-                m.add_to_relation(self.rel256, 1, [limb])
-        for n in R256_HALF_WORDS:
-            for limb in col[n]:
-                m.add_to_relation(self.rel256, 1, [limb])
-        for n in R256_BYTES:
-            m.add_to_relation(self.rel256, 1, [c(n)])
-        for n in R256_TYPE_U_BYTES:
-            m.add_to_relation(self.rel256, is_type_u, [c(n)])
-        for n in BOOL_SINGLE:
-            m.add_constraint(c(n) * (c(n) - 1))
-        for n in BOOL_HALF_WORD:
-            for limb in col[n]:
-                m.add_constraint(limb * (limb - 1))
-        for t, names in (("R", BOOL_TYPE_R), ("INoShift", BOOL_TYPE_I_NO_SHIFT), ("IShift", BOOL_TYPE_I_SHIFT), ("J", BOOL_TYPE_J),
-                         ("B", BOOL_TYPE_B), ("S", BOOL_TYPE_S)):
-            for n in names:
-                m.add_constraint(vtype[t] * c(n) * (c(n) - 1))
-        m.finalize_logup()                                                     # components/mod.rs:52-54
         # ---------------- extensions: Multiplicity256, Multiplicity32 (extensions/multiplicity.rs) ----------------
         t256 = air.component(8, 1)
         v256 = t256.get_preprocessed_column("Range256Values")
@@ -314,64 +387,17 @@ class NexusV1Machine:
         return list(self._pre_cache)
 
     def _preprocessed_list(self):
-        n = 1 << self.log_size
         cols = [None] * self.air.n_columns()[0]
         ids = self.air.preprocessed_ids
-
-        def put(name, limbs):
-            for i, v in enumerate(limbs):
-                cols[ids[f"{name}_{i}"]] = v
-
-        z = np.zeros(n, np.uint32)
-        first, last = z.copy(), z.copy()
-        first[0], last[n - 1] = 1, 1
-        put("IsFirst", [first]); put("IsLast", [last])
-        clk = np.arange(1, n + 1, dtype=np.uint64)                          # preprocessed.rs:75-100
-        le = lambda x: [((x >> (8 * k)) & 0xFF).astype(np.uint32) for k in range(4)]
-        put("Clk", le(clk)); put("Reg1TsCur", le(3 * clk + 1)); put("Reg2TsCur", le(3 * clk + 2)); put("Reg3TsCur", le(3 * clk + 3))
-        for name, size in PROGRAM_COLUMNS:                                  # empty program: the program trace is all zero
-            put(name, [z] * size)
+        for col_id, v in main_preprocessed_columns(self.log_size).items():
+            cols[ids[col_id]] = v
         cols[ids["Range256Values"]] = np.arange(256, dtype=np.uint32)
         cols[ids["Range32Values"]] = np.arange(32, dtype=np.uint32)
         return cols
 
     def fill_main_trace(self, seed=0):
         """The padding-only witness (class docstring).  Returns the tree-1 columns in commitment order: 347 main, then the two multiplicity columns."""
-        n = 1 << self.log_size
-        rng = np.random.default_rng(seed)
-        t = {name: [np.zeros(n, np.uint32) for _ in range(size)] for name, size in MAIN_COLUMNS}
-        t["IsPadding"][0][:] = 1
-        t["ValueAEffectiveFlagAux"][0][:] = 1
-        t["ValueAEffectiveFlagAuxInv"][0][:] = 1
-        rb = lambda: rng.integers(0, 256, n, dtype=np.uint64).astype(np.uint32)
-        free_words = [w for w in R256_WORDS if w not in ("Reg1TsPrev", "Reg2TsPrev", "Reg3TsPrev", "CReg1TsPrev", "CReg2TsPrev", "CReg3TsPrev")]
-        for w in free_words + R256_HALF_WORDS + R256_BYTES + ["ValueAEffective", "Reg1ValPrev", "Reg2ValPrev", "Reg3ValPrev", "PcNext"]:
-            if w == "ValueAEffective":
-                continue                                                    # = ValueA * flag = 0 (register_mem_check.rs:129-136)
-            for limb in t[w]:
-                limb[:] = rb()
-        for limb in t["Pc"]:
-            limb[0] = 0                                                    # is_first * (pc - PrgInitialPc) with an empty program
-        for w in ("ValueA4_7", "ValueB4_7", "ValueC4_7"):                   # high nibbles of the (free) values; only looked up when a bit-op flag is set
-            src = {"ValueA4_7": "ValueA", "ValueB4_7": "ValueB", "ValueC4_7": "ValueC"}[w]
-            for k in range(4):
-                t[w][k][:] = t[src][k] >> 4
-        for w in ("OpB", "Reg1Address", "Reg2Address", "Reg3Address"):       # Range32-checked; OpA = ValueAEffectiveFlag / aux = 0
-            t[w][0][:] = rng.integers(0, 32, n, dtype=np.uint64).astype(np.uint32)
-        # timestamps: prev < cur = 3 clk + k, c = cur - 1 - prev with the chip's per-16-bit borrows (timestamp.rs:101-150)
-        clk = np.arange(1, n + 1, dtype=np.uint64)
-        for k in (1, 2, 3):
-            cur = 3 * clk + k
-            prev = (rng.integers(0, 1 << 62, n, dtype=np.uint64) % cur).astype(np.uint64)
-            cc = cur - 1 - prev
-            lo = (cc & 0xFFFF) + (prev & 0xFFFF) + 1
-            b0 = (lo >> 16).astype(np.uint32)
-            hi = (cc >> 16) + (prev >> 16) + b0
-            assert np.all(lo - (b0.astype(np.uint64) << 16) == (cur & 0xFFFF)) and np.all(hi == (cur >> 16))
-            for i in range(4):
-                t[f"Reg{k}TsPrev"][i][:] = ((prev >> (8 * i)) & 0xFF).astype(np.uint32)
-                t[f"CReg{k}TsPrev"][i][:] = ((cc >> (8 * i)) & 0xFF).astype(np.uint32)
-            t[f"CH{k}Minus"][0][:] = b0
+        t = padding_witness(self.log_size, seed)
         cols = [limb for name, _ in MAIN_COLUMNS for limb in t[name]]
         h256, h32 = np.zeros(256, np.int64), np.zeros(32, np.int64)
         for w in R256_WORDS + R256_HALF_WORDS + R256_BYTES:

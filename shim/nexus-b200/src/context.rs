@@ -94,6 +94,24 @@ impl Context {
         })?;
         Ok(out.iter().map(|&h| Columns { ctx: self.clone(), h }).collect())
     }
+    /// RamInitFinal's 10 main columns (prover/src/extensions/ram_init_final.rs:458-511) filled on the device, finalized, into a new batch of
+    /// 2^log_size rows: the side note's `rw_mem_check.last_access` rebuilt from the keccak side note (as `keccak_main_trace` takes it) and the
+    /// public initial memory (`init_addresses` strictly ascending, one byte each in `init_values`).  Returns the batch and the number of
+    /// distinct addresses; `nb200_ram_init_final_trace` refuses a log_size too small for them.
+    pub fn ram_init_final_trace(&self, inputs: &[[u64; 25]], addresses: &[u32], timestamps: &[Vec<u32>], init_addresses: &[u32], init_values: &[u8],
+                                log_size: u32) -> Result<(Columns, usize)> {
+        assert!(addresses.len() == inputs.len() && timestamps.len() == inputs.len() && init_values.len() == init_addresses.len());
+        let ts: Vec<u32> = timestamps.iter().flat_map(|t| { assert_eq!(t.len(), 200); t.iter().copied() }).collect();
+        let mut h = ptr::null_mut();
+        self.check(unsafe { nb200_cols_alloc(self.raw(), 10, log_size, &mut h) })?;
+        let out = Columns { ctx: self.clone(), h };
+        let mut n_rows = 0usize;
+        self.check(unsafe {
+            nb200_ram_init_final_trace(self.raw(), inputs.len(), inputs.as_ptr() as *const u64, addresses.as_ptr(), ts.as_ptr(), init_addresses.len(),
+                                       init_addresses.as_ptr(), init_values.as_ptr(), log_size, h, &mut n_rows)
+        })?;
+        Ok((out, n_rows))
+    }
     /// NCCL communicator of this context (one process per GPU): rank 0 calls `comm_unique_id()`, ships the bytes to the other ranks, all call `comm_init`.
     pub fn comm_unique_id() -> Result<Vec<u8>> {
         let mut id = vec![0u8; unsafe { nb200_comm_unique_id_bytes() }];
