@@ -325,6 +325,14 @@ nb200_status nb200_air_count_kernel_source(const nb200_air*, uint32_t component,
  * lookup fractions); NB200_ERR_STATE with NB200_JIT=0 (the count has no interpreter).  Scratch is released in stream order. */
 nb200_status nb200_table_multiplicities(nb200_ctx*, const nb200_air*, const nb200_cols* const* tree0, size_t n0, nb200_cols* const* tree1, size_t n1,
                                         uint64_t* n_unmatched, uint32_t first_unmatched[3]);
+/* The same count, except for a tuple that several table rows of one relation list: the first of those rows (smallest component, table
+ * fraction and row in trace order) gets its count and every other one is written as 0, as the reference's trace fill credits value k of a
+ * padded range table to row k (Multiplicity8's table lists 0 nine times).  n_repeated = the rows written as 0 (table rows minus distinct
+ * (relation, tuple) keys).  Arguments, outputs and every other refusal as nb200_table_multiplicities; its scratch adds 8 bytes per hash
+ * slot (about 16 per table row), released in stream order. */
+nb200_status nb200_table_multiplicities_first_row(nb200_ctx*, const nb200_air*, const nb200_cols* const* tree0, size_t n0,
+                                                  nb200_cols* const* tree1, size_t n1, uint64_t* n_unmatched, uint32_t first_unmatched[3],
+                                                  uint64_t* n_repeated);
 
 /* ---- one PROOF over N GPUs ---------------------------------------------------------------------------------------------------
  * Every rank calls the same sequence (the Machine::prove order, machine.rs:197-290) with its own shard; transcript, roots and proof

@@ -270,16 +270,24 @@ class Context:
                                                    out._h, C.byref(n_rows)))
         return out, int(n_rows.value)
 
-    def table_multiplicities(self, air, tree0, tree1):
+    def table_multiplicities(self, air, tree0, tree1, first_row=False):
         """nb200_table_multiplicities: every table fraction's multiplicity column of `tree1` (device batches, finalized order) is overwritten
         with the count of the AIR's lookups into it.  `air` is a loaded AIR (prover.Air).  Returns (n_unmatched, first_unmatched), the latter
-        (component, fraction, row in trace order) of the smallest unmatched lookup, or None."""
+        (component, fraction, row in trace order) of the smallest unmatched lookup, or None.  `first_row`: nb200_table_multiplicities_first_row,
+        which credits a tuple listed by several table rows of one relation to the first of them and writes 0 into the others, and also
+        returns the number of rows written as 0: (n_unmatched, first_unmatched, n_repeated)."""
         t0 = (C.c_void_p * max(len(tree0), 1))(*[b._h for b in tree0])
         t1 = (C.c_void_p * max(len(tree1), 1))(*[b._h for b in tree1])
         n = C.c_uint64()
         first = (C.c_uint32 * 3)()
-        self._chk(lib().nb200_table_multiplicities(self._h, air._h, t0, C.c_size_t(len(tree0)), t1, C.c_size_t(len(tree1)), C.byref(n), first))
-        return int(n.value), (None if n.value == 0 else tuple(int(x) for x in first))
+        if first_row:
+            rep = C.c_uint64()
+            self._chk(lib().nb200_table_multiplicities_first_row(self._h, air._h, t0, C.c_size_t(len(tree0)), t1, C.c_size_t(len(tree1)), C.byref(n),
+                                                                 first, C.byref(rep)))
+        else:
+            self._chk(lib().nb200_table_multiplicities(self._h, air._h, t0, C.c_size_t(len(tree0)), t1, C.c_size_t(len(tree1)), C.byref(n), first))
+        out = int(n.value), (None if n.value == 0 else tuple(int(x) for x in first))
+        return out + (int(rep.value),) if first_row else out
 
     # ---- multi-GPU (one process per GPU): NCCL communicator inside the library
     @staticmethod

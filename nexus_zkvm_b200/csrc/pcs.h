@@ -27,6 +27,10 @@ nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, co
 nb200_status channel_mix_draw(nb200_ctx* ctx, DevChannel* d_ch, const uint8_t* d_root, u32* d_rec, int domain_sep);
 nb200_status add_inplace(nb200_ctx* ctx, u32* a, const u32* b, size_t n);
 nb200_status table_mult_store(nb200_ctx* ctx, u32* dst, const unsigned long long* cnt, size_t n);   // dst[i] = cnt[i] mod P
+// table_first_row.cu: every occupied slot of the built count hash names its key's first bin; *distinct += the occupied slots.  tables =
+// (first bin, log size) per table fraction in bin order; owner = cap words of ~0.
+nb200_status table_first_row_resolve(nb200_ctx* ctx, u32* slots, const u32* keys, u32 kw, u64 cap, u32 n_bins, const u32* tables, u32 n_tables,
+                                     unsigned long long* owner, u32* distinct);
 nb200_status grind(nb200_ctx* ctx, const uint8_t digest[32], u32 pow_bits, uint64_t* nonce_out);
 
 // rows [0, 2^rows_log) of CanonicCoset(dom_log).circle_domain() (bit-reversed); rows_log == dom_log - 1 selects the first half of

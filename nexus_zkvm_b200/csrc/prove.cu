@@ -1296,9 +1296,10 @@ nb200_status check_constraints(nb200_ctx* ctx, nb200_air* air_h, u32 comp_idx, c
 // Every table fraction's multiplicity column, counted on the GPU from the AIR's own lookups (air_lookup_tables, jit.cu gen_count_source).
 // Each row of each table fraction is a bin (tables in component then fraction order, rows in finalized order).  The build kernels hash
 // every table tuple to its bin, the probe kernels add every lookup's numerator to its tuple's bin, and the bins are written mod P into the
-// multiplicity columns of tree 1, in place.
+// multiplicity columns of tree 1, in place.  A tuple listed by two rows of one relation is refused, or with `first_row` credited to its
+// first row (table_first_row.cuh, between build and probe): *n_repeated = the rows written as 0.
 nb200_status table_multiplicities(nb200_ctx* ctx, nb200_air* air_h, const nb200_cols* const* const trees[2], const size_t n_trees[2],
-                                  uint64_t* n_unmatched, uint32_t first[3]) {
+                                  uint64_t* n_unmatched, uint32_t first[3], bool first_row = false, uint64_t* n_repeated = nullptr) {
   const AirProgram& air = air_h->prog;
   const std::vector<std::vector<AirFrac>>& fr = air_h->fracs;
   std::vector<std::vector<u32*>> flat(2);
@@ -1341,6 +1342,7 @@ nb200_status table_multiplicities(nb200_ctx* ctx, nb200_air* air_h, const nb200_
   }
   *n_unmatched = 0;
   first[0] = first[1] = first[2] = UINT32_MAX;
+  if (n_repeated) *n_repeated = 0;
   if (n_bins == 0) return NB200_OK;   // no table: nothing to count
   NB_ARG(ctx, n_bins <= (1ull << 30), "table_multiplicities: at most 2^30 table rows");
   // a numerator is below 2^31, so a u64 bin is exact for up to 2^33 additions: more lookups than that in one call could wrap it
@@ -1405,10 +1407,25 @@ nb200_status table_multiplicities(nb200_ctx* ctx, nb200_air* air_h, const nb200_
   trace_mark(ctx, nullptr);
   for (size_t k = 0; k < air.comps.size(); ++k)
     if (builds[k]) NB_TRY(count(k, 0, d_tb.p + tb_at[k], 0));
-  u32 dup = 0;
-  NB_CUDA(ctx, cudaMemcpyAsync(&dup, d_um.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // also: the host tables above have been consumed
-  if (dup) return set_err(ctx, NB200_ERR_ARG, "table_multiplicities: a table lists the same tuple in two rows of one relation");
+  // first_row: the build's duplicate flag is ignored; each key's slot is pointed at its first bin (owner: one u64 claim per slot, then the
+  // count of distinct keys)
+  DevBuf d_owner;
+  std::vector<u32> tables;   // (first bin, log size) per table fraction, bin order
+  if (first_row) {
+    for (size_t t = 0, b = 0; t < mult.size(); b += (size_t)1 << mult[t].second, ++t) { tables.push_back((u32)b); tables.push_back(mult[t].second); }
+    NB_TRY(alloc(ctx, d_owner, 2 * cap + 1 + tables.size()));
+    unsigned long long* owner = (unsigned long long*)d_owner.p;
+    u32 *distinct = d_owner.p + 2 * cap, *d_tables = distinct + 1;
+    NB_CUDA(ctx, cudaMemsetAsync(owner, 0xff, (size_t)cap * 8, ctx->stream));
+    NB_CUDA(ctx, cudaMemsetAsync(distinct, 0, 4, ctx->stream));
+    NB_CUDA(ctx, cudaMemcpyAsync(d_tables, tables.data(), tables.size() * 4, cudaMemcpyHostToDevice, ctx->stream));
+    NB_TRY(table_first_row_resolve(ctx, d_slots.p, d_keys.p, kw, cap, (u32)n_bins, d_tables, (u32)mult.size(), owner, distinct));
+  } else {
+    u32 dup = 0;
+    NB_CUDA(ctx, cudaMemcpyAsync(&dup, d_um.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // also: the host tables above have been consumed
+    if (dup) return set_err(ctx, NB200_ERR_ARG, "table_multiplicities: a table lists the same tuple in two rows of one relation");
+  }
   // bins privatised per CTA when they fit in 32 KB of shared memory (the v1 machine's Range256 + Range32: 288 bins)
   const u32 nsh = n_bins * 8 <= 32768 ? (u32)n_bins : 0u;
   for (size_t k = 0; k < air.comps.size(); ++k)
@@ -1419,9 +1436,12 @@ nb200_status table_multiplicities(nb200_ctx* ctx, nb200_air* air_h, const nb200_
     bin += (uint64_t)1 << m.second;
   }
   uint64_t um[2];
+  u32 distinct = 0;
   NB_CUDA(ctx, cudaMemcpyAsync(um, d_um.p, 16, cudaMemcpyDeviceToHost, ctx->stream));
-  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (first_row) NB_CUDA(ctx, cudaMemcpyAsync(&distinct, d_owner.p + 2 * cap, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));   // also: the host tables above have been consumed
   trace_mark(ctx, "table multiplicities");
+  if (n_repeated) *n_repeated = n_bins - distinct;
   *n_unmatched = um[0];
   if (um[0]) { first[0] = (uint32_t)(um[1] >> 48); first[1] = (uint32_t)((um[1] >> 28) & 0xFFFFF); first[2] = (uint32_t)(um[1] & 0xFFFFFFF); }
   return NB200_OK;
@@ -1678,6 +1698,14 @@ nb200_status nb200_table_multiplicities(nb200_ctx* ctx, const nb200_air* air, co
   const nb200_cols* const* trees[2] = {tree0, (const nb200_cols* const*)tree1};
   const size_t n_trees[2] = {n0, n1};
   return table_multiplicities(ctx, const_cast<nb200_air*>(air), trees, n_trees, n_unmatched, first_unmatched);
+}
+nb200_status nb200_table_multiplicities_first_row(nb200_ctx* ctx, const nb200_air* air, const nb200_cols* const* tree0, size_t n0,
+                                                  nb200_cols* const* tree1, size_t n1, uint64_t* n_unmatched, uint32_t first_unmatched[3],
+                                                  uint64_t* n_repeated) {
+  if (!ctx || !air || (n0 && !tree0) || (n1 && !tree1) || !n_unmatched || !first_unmatched || !n_repeated) return NB200_ERR_ARG;
+  const nb200_cols* const* trees[2] = {tree0, (const nb200_cols* const*)tree1};
+  const size_t n_trees[2] = {n0, n1};
+  return table_multiplicities(ctx, const_cast<nb200_air*>(air), trees, n_trees, n_unmatched, first_unmatched, true, n_repeated);
 }
 nb200_status nb200_air_lookup_tables(const nb200_air* a, uint32_t component, uint32_t* kind, uint32_t* relation, uint32_t* arg, size_t n) {
   if (!a || component >= a->prog.comps.size()) return NB200_ERR_ARG;

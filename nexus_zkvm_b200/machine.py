@@ -163,11 +163,13 @@ def check_constraints(machine, backend, main_cols, mult, associated_data=b"", re
     return report, verify_claimed_sums(claimed)
 
 
-def fill_table_multiplicities(machine, ctx, tree0, tree1, air=None):
+def fill_table_multiplicities(machine, ctx, tree0, tree1, air=None, first_row=False):
     """Overwrite the multiplicity columns of `tree1` (device batches, finalized order, before tree 1 is committed) with the counts of the
     machine's own lookups, on the GPU (nb200_table_multiplicities): what each machine's fill_main_trace counts on the host.  Raises
     Nb200Error naming the first lookup whose tuple is in no table row.  `air`: the machine's loaded AIR (prover.Air) on `ctx`; by default
-    one is loaded on the first call per context and kept on the machine, so the count kernels are compiled or loaded once, not per call."""
+    one is loaded on the first call per context and kept on the machine, so the count kernels are compiled or loaded once, not per call.
+    `first_row`: a tuple that several table rows list is credited to the first of them (nb200_table_multiplicities_first_row), and the
+    number of rows written as 0 is returned."""
     from . import Nb200Error
     from .prover import Air
     if air is None:
@@ -175,10 +177,11 @@ def fill_table_multiplicities(machine, ctx, tree0, tree1, air=None):
         air = cache.get(id(ctx))
         if air is None or air.ctx is not ctx:
             air = cache[id(ctx)] = Air(ctx, machine.words)
-    n, first = ctx.table_multiplicities(air, list(tree0), list(tree1))
+    n, first, *repeated = ctx.table_multiplicities(air, list(tree0), list(tree1), first_row=first_row)
     if n:
         comp, frac, row = first
         raise Nb200Error(f"{n} lookup(s) match no table row; the first: component {comp}, fraction {frac}, trace row {row}")
+    return repeated[0] if first_row else None
 
 
 def _commit_trees(machine, backend, main_cols, mult, config, associated_data, resident):

@@ -25,10 +25,13 @@ Rows are filled in trace order as in the other machines here: the reference's ex
 order (extensions/trace.rs:18-34 does not permute them), and a row of that order is a row of ours; the device fill writes row r at its
 finalized position, as nb200_keccak_main_trace does.
 
-Table multiplicities are counted on the host, as the reference's side note does: Range256 also counts RamInitFinal's nine lookups per row,
-whose numerator is 1 on padding rows too (ram_init_final.rs:219-248).  nb200_table_multiplicities cannot count this machine: Multiplicity8's
-preprocessed column is 0..7 then eight zeros (multiplicity8.rs:48), so the Range8 table lists the tuple (0) nine times, and the generic count
-refuses a relation that lists one tuple twice (its known limit).  The keccak tables' columns come from the keccak fill."""
+Table multiplicities.  fill_main_trace counts them on the host, as the reference's side note does: Range256 also counts RamInitFinal's nine
+lookups per row, whose numerator is 1 on padding rows too (ram_init_final.rs:219-248), and the keccak tables' columns come from the keccak
+extension's host fill.  device_trees counts every table column on the device from the filled trace with
+nb200_table_multiplicities_first_row: Multiplicity8's preprocessed column is 0..7 then eight zeros (multiplicity8.rs:48), so the Range8 table
+lists the tuple (0) nine times; the first of those rows gets the count and the eight padding rows 0, as the reference's
+`side_note.range8.multiplicity[checked] += 1` (chips/range_check/range8.rs:298, multiplicity8.rs:194-204) does.  The plain
+nb200_table_multiplicities refuses this machine, as it refuses any relation that lists one tuple twice."""
 import numpy as np
 
 from . import air as A
@@ -286,9 +289,11 @@ class NexusV1KeccakMachine:
         return cols
 
     # ---- tree 1
-    def _main_and_hist(self, seed):
+    def _main_and_hist(self, seed, hist=True):
         t = V.padding_witness(self.log_size_main, seed)
         cols = [limb for name, _ in V.MAIN_COLUMNS for limb in t[name]]
+        if not hist:
+            return cols, None, None
         # lookups with a nonzero numerator in the padding witness: Range32's five columns and Range256's words, half words and bytes (numerator
         # 1); every other relation's lookups are gated by an opcode flag, all zero here
         h256, h32 = np.zeros(256, np.int64), np.zeros(32, np.int64)
@@ -328,9 +333,13 @@ class NexusV1KeccakMachine:
         return self.air.column_log_sizes()
 
     def device_trees(self, ctx, seed=0):
-        """(tree-0 device batches, tree-1 device batches), finalized order, for machine.prove(..., resident=...): tree 0 uploaded; tree 1 =
-        the main component's columns and the base tables' host-counted multiplicity columns uploaded, RamInitFinal filled on the device
-        (nb200_ram_init_final_trace) and the keccak extension filled on the device (nb200_keccak_main_trace), both from the side note."""
+        """(tree-0 device batches, tree-1 device batches), finalized order, for machine.prove(..., resident=...): tree 0 uploaded; of tree 1
+        only the main component's columns and FinalReg's and BitOpMultiplicity's are uploaded.  RamInitFinal is filled on the device
+        (nb200_ram_init_final_trace) and the keccak extension too (nb200_keccak_main_trace), both from the side note; then every table's
+        multiplicity column (BitOp, Range8 to Range256 and the keccak tables) is counted from that trace (nb200_table_multiplicities_first_row),
+        so Range256 picks up RamInitFinal's lookups from the filled batch, after RamInitFinal as the reference orders them (machine.rs:81)."""
+        from .machine import fill_table_multiplicities
+
         def upload_runs(cols):
             out, i = [], 0
             while i < len(cols):
@@ -342,13 +351,21 @@ class NexusV1KeccakMachine:
             return out
 
         tree0 = upload_runs(self.preprocessed_columns())
-        main, h256, h32 = self._main_and_hist(seed)
-        ram_cols = self.ram_init_final_columns()
-        base = self.base_extension_columns(h256, h32, ram_cols)
-        ram, n_rows = ctx.ram_init_final_trace(*self.side_note(), self.init_addresses, self.init_values, self.ram_log_size)
-        assert n_rows == self.init_addresses.size
+        main, _h256, _h32 = self._main_and_hist(seed, hist=False)
         tree1 = [ctx.upload(np.stack(main), coset_order=True)]
         del main
-        tree1 += upload_runs(base[:11]) + [ram] + upload_runs(base[11 + RAM_COLS:])
+        tree1 += upload_runs([np.zeros(1 << FINAL_REG_LOG_SIZE, np.uint32)] * 8)      # no register is accessed: final state = initial state
+        tree1 += upload_runs([np.zeros(1 << BIT_OP_LOG_SIZE, np.uint32)] * 3)         # BitOp's multiplicities: counted below
+        ram, n_rows = ctx.ram_init_final_trace(*self.side_note(), self.init_addresses, self.init_values, self.ram_log_size)
+        assert n_rows == self.init_addresses.size
+        tree1.append(ram)
+        i = 0                                                                 # Multiplicity8 ... 256: one batch per run of equal sizes
+        while i < len(MULTIPLICITY_TABLES):
+            j = i
+            while j < len(MULTIPLICITY_TABLES) and MULTIPLICITY_TABLES[j][2] == MULTIPLICITY_TABLES[i][2]:
+                j += 1
+            tree1.append(ctx.alloc(j - i, MULTIPLICITY_TABLES[i][2]))
+            i = j
         tree1 += ctx.keccak_main_trace(*self.side_note())
+        fill_table_multiplicities(self, ctx, tree0, tree1, first_row=True)
         return tree0, tree1

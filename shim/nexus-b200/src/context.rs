@@ -175,6 +175,18 @@ impl Context {
         self.check(unsafe { nb200_table_multiplicities(self.raw(), air.h, t0.as_ptr(), t0.len(), t1.as_ptr(), t1.len(), &mut n, first.as_mut_ptr()) })?;
         Ok((n, if n == 0 { None } else { Some((first[0], first[1], first[2])) }))
     }
+    /// `table_multiplicities` for tables that list one tuple in several rows (Multiplicity8's padded Range8 table): the first such row, in
+    /// (component, table, trace row) order, gets the count and the others 0, as the reference's trace fill does.  Also returns the number of
+    /// rows written as 0.
+    pub fn table_multiplicities_first_row(&self, air: &Air, tree0: &[&Columns], tree1: &mut [&mut Columns])
+        -> Result<(u64, Option<(u32, u32, u32)>, u64)> {
+        let t0: Vec<*const nb200_cols> = tree0.iter().map(|c| c.h as *const _).collect();
+        let t1: Vec<*mut nb200_cols> = tree1.iter().map(|c| c.h).collect();
+        let (mut n, mut first, mut repeated) = (0u64, [u32::MAX; 3], 0u64);
+        self.check(unsafe { nb200_table_multiplicities_first_row(self.raw(), air.h, t0.as_ptr(), t0.len(), t1.as_ptr(), t1.len(), &mut n,
+                                                                 first.as_mut_ptr(), &mut repeated) })?;
+        Ok((n, if n == 0 { None } else { Some((first[0], first[1], first[2])) }, repeated))
+    }
 }
 
 /// `PcsConfig { pow_bits, fri_config: FriConfig { log_blowup_factor, log_last_layer_degree_bound, n_queries } }`

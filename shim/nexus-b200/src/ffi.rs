@@ -143,6 +143,9 @@ extern "C" {
     pub fn nb200_air_count_kernel_source(air: *const nb200_air, component: u32, out: *mut *mut c_char) -> c_int;
     pub fn nb200_table_multiplicities(ctx: *mut nb200_ctx, air: *const nb200_air, tree0: *const *const nb200_cols, n0: usize,
                                       tree1: *const *mut nb200_cols, n1: usize, n_unmatched: *mut u64, first_unmatched: *mut u32) -> c_int;
+    pub fn nb200_table_multiplicities_first_row(ctx: *mut nb200_ctx, air: *const nb200_air, tree0: *const *const nb200_cols, n0: usize,
+                                                tree1: *const *mut nb200_cols, n1: usize, n_unmatched: *mut u64, first_unmatched: *mut u32,
+                                                n_repeated: *mut u64) -> c_int;
     // ---- backend-trait level operations
     pub fn nb200_constraint_quotients(s: *mut nb200_scheme, air: *const nb200_air, component: u32, params: *const u32, n_params: usize,
                                       coeffs: *const u32, n_coeffs: usize, accum: *mut nb200_cols) -> c_int;

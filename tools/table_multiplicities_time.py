@@ -1,13 +1,17 @@
 """Time the table-multiplicity count (nb200_table_multiplicities) on one GPU.
 
-    python tools/table_multiplicities_time.py [--v1-log-size 20] [--keccak-log-perms 14] [--reps 20] [--out FILE]
+    python tools/table_multiplicities_time.py [--v1-log-size 20] [--keccak-log-perms 14] [--whole-log-size 20 --whole-log-perms 12]
+                                              [--reps 20] [--out FILE]
 
 Two workloads, each timed `reps` times after a warm-up with CUDA events recorded on the library's stream (one call: scratch allocation, hash
 build, probes, stores, and the two synchronisations of the call):
   * NexusV1Machine(v1_log_size), padding witness, trees 0 and 1 uploaded from host columns; next to it the host's numpy bincount over the
     same lookup columns (what fill_main_trace does for the Range256 / Range32 columns);
   * KeccakMachine(keccak_log_perms) from device_trees (the side-note fill); next to it, in the same run, the device time of the side-note
-    fill's hand-written lookup histogram (keccak_round_count_kernel) and of the count's own kernels, both from torch.profiler.
+    fill's hand-written lookup histogram (keccak_round_count_kernel) and of the count's own kernels, both from torch.profiler;
+  * with --whole-log-size, NexusV1KeccakMachine(whole_log_size, 2^whole_log_perms) from device_trees, counted by
+    nb200_table_multiplicities_first_row (its Range8 table lists 0 nine times); next to it the device time of the first-row resolve's two
+    kernels (table_first_row_claim_kernel, table_first_row_slot_kernel) and of all the count's kernels, from torch.profiler.
 The one-time NVRTC compile time of every component's count kernel (nb200_air_count_kernel_source) is measured on its own, with libnvrtc and
 the options the library compiles with.  The library's cubin cache points to an empty directory under the system's temporary directory, so
 nothing is read from or written to the tree.  Prints one JSON line with the card name, power limit and SM clock read in the same run."""
@@ -81,27 +85,30 @@ def kernel_ms(fn, names, reps):
     return tot / reps / 1e3
 
 
-def timed(ctx, stream, air, tree0, tree1, reps):
+def timed(ctx, stream, air, tree0, tree1, reps, first_row=False):
     import torch
-    ctx.table_multiplicities(air, tree0, tree1)                  # warm-up: loads (or compiles) every count kernel
+    call = lambda: ctx.table_multiplicities(air, tree0, tree1, first_row=first_row)
+    call()                                                       # warm-up: loads (or compiles) every count kernel
     ms = []
     for _ in range(reps):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record(stream)
-        n, _first = ctx.table_multiplicities(air, tree0, tree1)
+        n = call()[0]
         e1.record(stream)
         e1.synchronize()
         assert n == 0
         ms.append(e0.elapsed_time(e1))
     ms.sort()
-    return {"ms_median": ms[len(ms) // 2], "ms_min": ms[0], "ms_max": ms[-1],
-            "count_kernels_ms": kernel_ms(lambda: ctx.table_multiplicities(air, tree0, tree1), ("nbjit", "table_mult_store"), 5)}
+    names = ("nbjit", "table_mult_store") + (("table_first_row",) if first_row else ())
+    return {"ms_median": ms[len(ms) // 2], "ms_min": ms[0], "ms_max": ms[-1], "count_kernels_ms": kernel_ms(call, names, 5)}
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--v1-log-size", type=int, default=20)
     ap.add_argument("--keccak-log-perms", type=int, default=14)
+    ap.add_argument("--whole-log-size", type=int, default=0, help="main component log size of the whole-machine workload (0: not run)")
+    ap.add_argument("--whole-log-perms", type=int, default=12)
     ap.add_argument("--reps", type=int, default=20)
     ap.add_argument("--out")
     a = ap.parse_args()
@@ -163,6 +170,21 @@ def main():
     fill()
     res["keccak"]["fill_round_count_kernel_ms"] = kernel_ms(fill, ("keccak_round_count_kernel",), 5)
     res["keccak"]["nvrtc_compile_ms"] = nvrtc_compile_ms(km.words)
+    del tree0, tree1
+
+    if a.whole_log_size:
+        from nexus_zkvm_b200.whole_machine import NexusV1KeccakMachine
+        wm = NexusV1KeccakMachine(a.whole_log_size, 1 << a.whole_log_perms)
+        tree0, tree1 = wm.device_trees(ctx)
+        air = Air(ctx, wm.words)
+        n_repeated = ctx.table_multiplicities(air, tree0, tree1, first_row=True)[2]
+        w = timed(ctx, stream, air, tree0, tree1, a.reps, first_row=True)
+        w["resolve_kernels_ms"] = kernel_ms(lambda: ctx.table_multiplicities(air, tree0, tree1, first_row=True), ("table_first_row",), 5)
+        w["resolve_share_of_call"] = w["resolve_kernels_ms"] / w["ms_median"]
+        table_rows = sum(1 << wm.air.components[k].log_size for k, row in enumerate(ref.classify(wm.air)) for (kind, _r, _c) in row if kind == "table")
+        res["whole"] = dict(what="nb200_table_multiplicities_first_row", log_size=a.whole_log_size, n_perms=wm.n_perms,
+                            component_log_sizes=wm.log_sizes, table_rows=table_rows, n_repeated=n_repeated, **w)
+        del tree0, tree1
     line = json.dumps(res)
     print(line)
     if a.out:

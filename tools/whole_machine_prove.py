@@ -4,8 +4,9 @@
     python tools/whole_machine_prove.py [--log-size 20] [--log-perms 12] [--steps 3] [--warmup 1] [--fill-calls 20] [--out-dir DIR]
 
 Two arms alternate step by step after the warm-up: `host` proves from the host columns (machine.prove with the tree-1 columns built on the
-host, RamInitFinal and the keccak blocks included), `device` from NexusV1KeccakMachine.device_trees (tree 0 and the main component's and base
-tables' columns uploaded, RamInitFinal filled by nb200_ram_init_final_trace and the keccak extension by nb200_keccak_main_trace), both timed
+host, RamInitFinal and the keccak blocks included), `device` from NexusV1KeccakMachine.device_trees (tree 0 and the main component's,
+FinalReg's and BitOpMultiplicity's columns uploaded, RamInitFinal filled by nb200_ram_init_final_trace, the keccak extension by
+nb200_keccak_main_trace and every table column counted by nb200_table_multiplicities_first_row), both timed
 with a host clock from the call to the proof bytes on the host.  The host arm's columns are built once, before the steps; the device arm
 builds its main columns inside the timed call.  The two arms' proof bytes must be equal; the oracle's verifier checks the last one.  The peak
 of each arm is the memory pool's used-memory high-water mark over its steps (reset before each step).  RamInitFinal's fill alone is timed with
