@@ -53,31 +53,33 @@ _committed = {}
 
 
 def committed(m, kind, seed=11):
-    """(oracle prover, params, trees as committed) of the witness `kind` ("padding" or a random_witness kind), one per kind and size."""
-    key = (m.log_size, kind, seed)
+    """(oracle prover, params, trees as committed) of the witness `kind` ("padding" or a random_witness kind), one per machine and kind.
+    Keyed on the machine itself: two machines of one log_size (the whole machine's is its largest component's) have different trees."""
+    key = (m, kind, seed)
     if key not in _committed:
         w = rw.padding(m) if kind == "padding" else rw.random_trees(m, seed, kind)
         _committed[key] = rw.on_oracle(m, w)
     return _committed[key]
 
 
-def high_flags(m):
-    return np.array([d > 2 for d in _walk_degrees(m.air.components[0])])
+def high_flags(m, k=0):
+    return np.array([d > 2 for d in _walk_degrees(m.air.components[k])])
 
 
-def quotient_mismatches(m, lib1, lib2, d2_masks, kind, dinv_from=None):
-    """Where the host-run D1 kernel (every constraint into a0..a3, the high ones into h0..h3) and D2 kernel (the high ones, from the columns
-    they read) differ from the oracle's quotients with all coefficients / with the low-degree ones zeroed, over canonic(eval_log): [] when
-    they agree everywhere.  The oracle's quotients carry 1 / vanishing, one field element per block of 2^log_size rows, recovered from one
-    row of the D1 kernel's sum, or of the sum of the D1 kernel `dinv_from` when the kernel under test is not to be trusted with it."""
+def quotient_mismatches(m, lib1, lib2, d2_masks, kind, dinv_from=None, k=0):
+    """Where the host-run D1 kernel of component k (every constraint into a0..a3, the high ones into h0..h3) and D2 kernel (the high ones,
+    from the columns they read; lib2 None: the component has none) differ from the oracle's quotients with all coefficients / with the
+    low-degree ones zeroed, over canonic(eval_log): [] when they agree everywhere.  The oracle's quotients carry 1 / vanishing, one field
+    element per block of 2^log_size rows, recovered from one row of the D1 kernel's sum, or of the sum of the D1 kernel `dinv_from` when the
+    kernel under test is not to be trusted with it."""
     p, params, trees = committed(m, kind)
-    log_size, log_expand, n, masks = parse_component(m.words, 0)
+    log_size, log_expand, n, masks = parse_component(m.words, k)
     elog = log_size + log_expand
-    high = high_flags(m)
+    high = high_flags(m, k)
     coeffs = np.random.default_rng(3).integers(0, P, size=(n, 4), dtype=np.uint32)
     prm_q = np.array(params, dtype=np.uint32)
-    want_all = p.p.constraint_quotients(0, elog, prm_q, coeffs)
-    want_high = p.p.constraint_quotients(0, elog, prm_q, np.where(high[:, None], coeffs, 0).astype(np.uint32))
+    want_all = p.p.constraint_quotients(k, elog, prm_q, coeffs)
+    want_high = p.p.constraint_quotients(k, elog, prm_q, np.where(high[:, None], coeffs, 0).astype(np.uint32))
     ext = {}
     for (t, c, _off) in masks:
         if (t, c) not in ext:
@@ -91,8 +93,9 @@ def quotient_mismatches(m, lib1, lib2, d2_masks, kind, dinv_from=None):
     lib1.run_rows(ptrs([True] * len(masks)), prm.ctypes.data_as(u32p), tab.ctypes.data_as(u32p), dinv.ctypes.data_as(u32p),
                   *[a.ctypes.data_as(u32p) for a in acc], C.c_uint32(elog), C.c_uint32(rows))
     acc2 = [np.zeros(rows, np.uint32) for _ in range(4)]
-    lib2.run_rows(ptrs(d2_masks), prm.ctypes.data_as(u32p), tab.ctypes.data_as(u32p), dinv.ctypes.data_as(u32p),
-                  *[a.ctypes.data_as(u32p) for a in acc2], C.c_uint32(elog), C.c_uint32(rows))
+    if lib2 is not None:
+        lib2.run_rows(ptrs(d2_masks), prm.ctypes.data_as(u32p), tab.ctypes.data_as(u32p), dinv.ctypes.data_as(u32p),
+                      *[a.ctypes.data_as(u32p) for a in acc2], C.c_uint32(elog), C.c_uint32(rows))
     got_all, got_high, got_d2 = np.stack(acc[:4]), np.stack(acc[4:]), np.stack(acc2)
     if dinv_from is not None:
         acc = [np.zeros(rows, np.uint32) for _ in range(8)]
@@ -111,7 +114,7 @@ def quotient_mismatches(m, lib1, lib2, d2_masks, kind, dinv_from=None):
             bad.append(f"block {blk}: D1 kernel, every constraint")
         if not np.array_equal((got_high[:, sl].astype(object) * d) % P, want_high[:, sl].astype(object)):
             bad.append(f"block {blk}: D1 kernel, the high constraints")
-        if not np.array_equal((got_d2[:, sl].astype(object) * d) % P, want_high[:, sl].astype(object)):
+        if lib2 is not None and not np.array_equal((got_d2[:, sl].astype(object) * d) % P, want_high[:, sl].astype(object)):
             bad.append(f"block {blk}: D2 kernel")
     return bad
 
@@ -201,10 +204,10 @@ def test_check_kernel_matches_the_oracle(v1, tmp_path, kind):
 
 # ---- mutations: a one-token change of the emitted source inside a constraint that the padding witness makes identically zero
 
-def _zero_masks(m):
-    """Per mask of the v1 component: its column is zero in every row of the padding witness (trees 0 and 1)."""
+def _zero_masks(m, comp=0):
+    """Per mask of component `comp`: its column is zero in every row of the padding witness (trees 0 and 1)."""
     _p, _params, trees = committed(m, "padding")
-    return [t < 2 and not np.any(trees[t][c]) for (t, c, _o) in parse_component(m.words, 0)[3]]
+    return [t < 2 and not np.any(trees[t][c]) for (t, c, _o) in parse_component(m.words, comp)[3]]
 
 
 def _statements(src, k):
@@ -218,11 +221,12 @@ def _statements(src, k):
     return lines, start, end
 
 
-def mutate_neighbour_mask(src, m, candidates, allowed):
-    """Constraint k (the first of `candidates` where this applies) reads mask M + 1 instead of mask M, where both masks are columns of
-    their own that are zero under the padding witness (so every value under it is unchanged) and M + 1 is in `allowed`."""
-    masks = parse_component(m.words, 0)[3]
-    zero = _zero_masks(m)
+def mutate_neighbour_mask(src, m, candidates, allowed, comp=0):
+    """Constraint k of component `comp` (the first of `candidates` where this applies) reads mask M + 1 instead of mask M, where both
+    masks are columns of their own that are zero under the padding witness (so every value under it is unchanged) and M + 1 is in
+    `allowed`."""
+    masks = parse_component(m.words, comp)[3]
+    zero = _zero_masks(m, comp)
     src = src.decode()
     for k in candidates:
         lines, start, end = _statements(src, k)
