@@ -359,7 +359,9 @@ nb200_status nb200_gen_interaction_trace_sharded(nb200_scheme*, const nb200_air*
 /* ComponentProver::<B>::evaluate_constraint_quotients_on_domain for one component (built at machine.rs:265-285): extend
  * the committed polynomials the component reads to CanonicCoset(log_size + log_expand).circle_domain(), evaluate
  * sum_k coeffs[k] * constraint_k / vanishing on every row and ADD into accum (4 columns of that domain size).
- * coeffs = n_coeffs QM31 (= the component's n_constraints random-coefficient powers, first constraint first). */
+ * coeffs = n_coeffs QM31 (= the component's n_constraints random-coefficient powers, first constraint first).
+ * NB200_ERR_ARG for a component that reads columns of a sharded tree (nb200_scheme_commit_sharded): nb200_prove evaluates such a
+ * component on the half domains only (nb200_constraint_quotients_half). */
 nb200_status nb200_constraint_quotients(nb200_scheme*, const nb200_air*, uint32_t component, const uint32_t* params, size_t n_params,
                                         const uint32_t* coeffs, size_t n_coeffs, nb200_cols* accum);
 /* The half-domain route nb200_prove takes (Q_HALF) for a component with log_expand = log_blowup + 1 whose LDE has more than 2^8 rows: ADDs
@@ -370,7 +372,11 @@ nb200_status nb200_constraint_quotients(nb200_scheme*, const nb200_air*, uint32_
  *   q_high_d1 = the same on D1.
  * Where the bytecode interpreter evaluates the component instead of the generated kernels (NB200_JIT=0, or an LDE of fewer than 2^10 rows)
  * every constraint counts as a high one: q_high_d2 and q_high_d1 then hold q itself.
- * NB200_ERR_ARG for a component that nb200_prove evaluates with Q_FULL (nb200_constraint_quotients). */
+ * NB200_ERR_ARG for a component that nb200_prove evaluates with Q_FULL (nb200_constraint_quotients).
+ * A component that reads columns of a sharded tree takes the sharded route, as in nb200_prove: each rank evaluates its own rows, from its
+ * LDE and D2 row slices and the full copies of the columns read at a row offset, and the accumulators are all-gathered, so every rank
+ * holds all rows.  It needs the generated kernels (NB200_ERR_ARG without them), and NB200_ERR_ARG names a column read at a row offset
+ * that was not listed in replicate_cols when its tree was committed. */
 nb200_status nb200_constraint_quotients_half(nb200_scheme*, const nb200_air*, uint32_t component, const uint32_t* params, size_t n_params,
                                              const uint32_t* coeffs, size_t n_coeffs, nb200_cols* q_d1, nb200_cols* q_high_d2, nb200_cols* q_high_d1);
 /* AccumulationOps::accumulate: a += b (element-wise, M31), same shapes */

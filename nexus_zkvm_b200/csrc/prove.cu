@@ -582,6 +582,9 @@ nb200_status component_quotients(nb200_scheme* s, nb200_air* air_h, size_t comp_
     NB_ARG(ctx, mk.tree < s->trees.size() && mk.col < s->trees[mk.tree].cols.size(), "prove: AIR references a column that was not committed");
     const SchemeTree& tr = s->trees[mk.tree];
     const SchemeTree::ColLoc& loc = tr.cols[mk.col];
+    // a sharded column has no batch in ldes / coeffs: only component_quotients_sharded can read it
+    NB_ARG(ctx, loc.batch != SchemeTree::BIG, "constraint quotients: column " + std::to_string(mk.col) + " of tree " + std::to_string(mk.tree) +
+                                              " is sharded; only the sharded route (the half-domain entry) evaluates this component");
     NB_ARG(ctx, loc.log == c.log_size, "prove: column size differs from its component's log_size");
     mask_lde[m] = tr.ldes[loc.batch]->col(loc.idx);
     if (reuse_lde) { mask_cols[m] = mask_lde[m]; continue; }
@@ -648,7 +651,8 @@ static nb200_status component_quotients_sharded(nb200_scheme* s, nb200_air* air_
   nb200_ctx* ctx = s->ctx;
   const AirComponent& c = air_h->prog.comps[comp_idx];
   const u32 elog = c.eval_log(), lde_log = c.log_size + s->log_blowup, k = (u32)comm_log_world(ctx);
-  NB_ARG(ctx, elog == lde_log + 1 && accum && accum_hi && accum_sub && accum->log_size == lde_log && accum_hi->log_size == lde_log && accum_sub->log_size == lde_log,
+  auto half_acc = [&](const nb200_cols* a) { return a && a->n_cols == 4 && a->log_size == lde_log; };
+  NB_ARG(ctx, elog == lde_log + 1 && half_acc(accum) && half_acc(accum_hi) && half_acc(accum_sub),
          "sharded constraint quotients: the component must use the half-domain route");
   NB_ARG(ctx, coeff.size() == c.n_constraints, "constraint quotients: one coefficient per constraint");
   const size_t S = (size_t)1 << (lde_log - k);
@@ -663,7 +667,8 @@ static nb200_status component_quotients_sharded(nb200_scheme* s, nb200_air* air_
     if (mk.off == 0) { m_lde[m] = tr.lde_rows(loc.idx); m_hx[m] = tr.hx_rows(loc.idx); }
     else {
       auto f = tr.full_lde.find(loc.idx); auto h = tr.full_hx.find(loc.idx);
-      NB_ARG(ctx, f != tr.full_lde.end() && h != tr.full_hx.end(), "sharded constraint quotients: a column read at a row offset was not listed for replication at commit time");
+      NB_ARG(ctx, f != tr.full_lde.end() && h != tr.full_hx.end(), "sharded constraint quotients: column " + std::to_string(mk.col) + " of tree " + std::to_string(mk.tree) +
+                                                                   " is read at a row offset but was not listed for replication at commit time");
       m_lde[m] = f->second->d; m_hx[m] = h->second->d;
     }
   }
@@ -1788,6 +1793,9 @@ nb200_status nb200_constraint_quotients(nb200_scheme* s, const nb200_air* air, u
                                         const uint32_t* coeffs, size_t n_coeffs, nb200_cols* accum) {
   if (!s || !air || !accum || (!coeffs && n_coeffs)) return NB200_ERR_ARG;
   nb200_ctx* ctx = s->ctx;
+  NB_ARG(ctx, component < air->prog.comps.size(), "constraint quotients: component index");
+  NB_ARG(ctx, !component_is_sharded(s, air->prog.comps[component]),
+         "constraint quotients: the component reads sharded columns, which only the half-domain entry (nb200_constraint_quotients_half) evaluates");
   NB_ARG(ctx, n_params == air->prog.n_params, "constraint quotients: parameter table size");
   std::vector<qm31> cf(n_coeffs);
   if (n_coeffs) memcpy(cf.data(), coeffs, n_coeffs * 16);
@@ -1809,7 +1817,10 @@ nb200_status nb200_constraint_quotients_half(nb200_scheme* s, const nb200_air* a
   if (n_coeffs) memcpy(cf.data(), coeffs, n_coeffs * 16);
   DevBuf d_params;
   NB_TRY(upload_params(ctx, params, n_params, d_params));
-  NB_TRY(component_quotients(s, const_cast<nb200_air*>(air), component, d_params.p, cf, Q_HALF, q_d1, q_high_d2, q_high_d1));
+  // the same dispatch as commit_composition: a component that reads sharded columns takes the sharded route
+  nb200_air* air_h = const_cast<nb200_air*>(air);
+  if (component_is_sharded(s, air->prog.comps[component])) NB_TRY(component_quotients_sharded(s, air_h, component, d_params.p, cf, q_d1, q_high_d2, q_high_d1));
+  else NB_TRY(component_quotients(s, air_h, component, d_params.p, cf, Q_HALF, q_d1, q_high_d2, q_high_d1));
   NB_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return NB200_OK;
 }

@@ -220,9 +220,9 @@ def _commit_trees(machine, backend, main_cols, mult, config, associated_data, re
     return ch, prover, params, claimed, roots, log_sizes
 
 
-def shard_host_tree(machine, prover, host_cols, rank, world):
+def shard_host_tree(machine, prover, host_cols, rank, world, coset_order=True):
     """Upload this rank's part of one tree's host columns: (column shard of the leading 2^log_size-row batch or None, its total column count,
-    replicated device batches of the smaller columns)."""
+    replicated device batches of the smaller columns).  coset_order=False: the columns are already in finalized order (an interaction trace)."""
     from . import Context
     n, cols = machine.log_size, []
     for c_ in host_cols:
@@ -233,9 +233,67 @@ def shard_host_tree(machine, prover, host_cols, rank, world):
         total_big += 1
     assert all(len(c_) < 1 << n for c_ in cols[total_big:]), "the sharded columns must be the leading, largest batch of the tree"
     first, count = Context.shard_range(total_big, world, rank)
-    shard = prover.ctx.upload(np.stack([np.ascontiguousarray(c_, dtype=np.uint32) for c_ in cols[first:first + count]]), coset_order=True) if count else None
-    small = prover._batches_from_host(cols[total_big:], True) if len(cols) > total_big else []
+    shard = prover.ctx.upload(np.stack([np.ascontiguousarray(c_, dtype=np.uint32) for c_ in cols[first:first + count]]), coset_order=coset_order) if count else None
+    small = prover._batches_from_host(cols[total_big:], coset_order) if len(cols) > total_big else []
     return shard, total_big, small
+
+
+def commit_sharded_tree(machine, prover, t, part, keep_eval_rows, ch):
+    """Commit tree t of a sharded proof from `part` = (column shard or None, total sharded columns, replicated batches), as shard_host_tree returns
+    it.  Every rank keeps a full copy of the sharded columns that the main component reads at a row offset."""
+    shard, total_big, small = part
+    replicate = sorted({c for (tt, c, off) in machine.air.components[0].masks if tt == t and off != 0 and c < total_big})
+    return prover.commit_sharded(shard, total_big, machine.log_size, small, replicate, keep_eval_rows, ch)
+
+
+def interaction_traces_sharded(machine, prover, parts, params):
+    """The interaction traces of a sharded proof, trees 0 and 1 committed from `parts` (their shard_host_tree results) with keep_eval_rows: the
+    main component's column shard, the other components' batches and every component's claimed sum.  Each cumsum shift is set in `params` as
+    its trace is made."""
+    air, ctx, n = machine.air, prover.ctx, machine.log_size
+    # the replicated components read trees 0 and 1 as batch lists in commitment order: a placeholder batch stands for the sharded columns they never read
+    ph = [shard for shard, _total, _small in parts if shard is not None][0]
+    t0_list, t1_list = ([ctx.wrap_device(ph.device_ptr, total, 0)] + small for _shard, total, small in parts)
+    shard2, cs = prover.gen_interaction_sharded(0, params)
+    inter_small, claimed = [], [cs]
+    params[air.components[0].cumsum_shift_param] = F.qm31_mul_m31(cs, F.m31_inv((1 << n) % P))
+    for k_, comp in enumerate(air.components[1:], start=1):
+        cols_k, cs = prover.gen_interaction_replicated(k_, comp.log_size, max(comp.batching) + 1, params, t0_list, t1_list)
+        inter_small.append(cols_k)
+        claimed.append(cs)
+        params[comp.cumsum_shift_param] = F.qm31_mul_m31(cs, F.m31_inv((1 << comp.log_size) % P))
+    return shard2, inter_small, claimed
+
+
+def _commit_trees_sharded(machine, backend, main_cols, mult, rank, world, config, associated_data, resident):
+    """prove_sharded up to and including the tree-2 commit: (channel, prover, params, claimed sums, roots)."""
+    config = config or dict(pow_bits=5, log_blowup=1, log_last=0, n_queries=3)
+    air = machine.air
+    ch = backend.channel()
+    for byte in associated_data:
+        ch.mix_u64(int(byte))
+    for ls in (getattr(machine, "log_sizes", None) or [machine.log_size, 8]):
+        ch.mix_u64(ls)
+    prover = backend.prover(machine.words, config)
+    parts, roots = [], []
+    for t in (0, 1):
+        if resident is not None:
+            parts.append(resident[t])
+        elif t == 0:
+            parts.append(shard_host_tree(machine, prover, machine.preprocessed_columns(), rank, world))
+        else:
+            main_part = [main_cols] if getattr(main_cols, "ndim", 1) == 2 else list(main_cols)
+            parts.append(shard_host_tree(machine, prover, main_part + ([mult] if mult is not None else []), rank, world))
+        roots.append(commit_sharded_tree(machine, prover, t, parts[t], True, ch))
+    params = [(0, 0, 0, 0)] * air.n_params
+    for rel in (getattr(machine, "relations", None) or [machine.range256]):
+        rel.draw(ch, params)
+    # interaction traces: the main component sharded, the others replicated
+    shard2, inter_small, claimed = interaction_traces_sharded(machine, prover, parts, params)
+    ch.mix_felts(claimed)
+    big2 = 4 * (max(air.components[0].batching) + 1)
+    roots.append(commit_sharded_tree(machine, prover, 2, (shard2 if shard2.n_cols else None, big2, inter_small), False, ch))
+    return ch, prover, params, claimed, roots
 
 
 def prove_sharded(machine, backend, main_cols, mult, rank, world, config=None, associated_data=b"", resident=None):
@@ -245,48 +303,9 @@ def prove_sharded(machine, backend, main_cols, mult, rank, world, config=None, a
     hashing, constraint rows and DEEP quotients; the other components' small columns are replicated.  For the harness every rank is handed the full host
     trace and uploads only its nb200_shard_range of it (a real host would fill only that range); `resident` = the two shard_host_tree results of
     trees 0 and 1 when they are already on the device."""
-    config = config or dict(pow_bits=5, log_blowup=1, log_last=0, n_queries=3)
-    air, ctx = machine.air, backend.ctx
-    ch = backend.channel()
-    for byte in associated_data:
-        ch.mix_u64(int(byte))
+    ch, prover, params, claimed, roots = _commit_trees_sharded(machine, backend, main_cols, mult, rank, world, config, associated_data, resident)
     log_sizes = list(getattr(machine, "log_sizes", None) or [machine.log_size, 8])
-    for ls in log_sizes:
-        ch.mix_u64(ls)
-    prover = backend.prover(machine.words, config)
-    n = machine.log_size
-    main = air.components[0]
-
-    def commit_tree(t, host_cols, keep):
-        shard, total_big, small = resident[t] if resident is not None else shard_host_tree(machine, prover, host_cols, rank, world)
-        replicate = sorted({c for (tt, c, off) in main.masks if tt == t and off != 0 and c < total_big})
-        root = prover.commit_sharded(shard, total_big, n, small, replicate, keep, ch)
-        return root, total_big, shard, small
-
-    root0, big0, shard0, small0 = commit_tree(0, machine.preprocessed_columns() if resident is None else None, True)
-    main_part = [] if resident is not None else ([main_cols] if getattr(main_cols, "ndim", 1) == 2 else list(main_cols))
-    root1, big1, shard1, small1 = commit_tree(1, main_part + ([mult] if mult is not None else []), True)
-    params = [(0, 0, 0, 0)] * air.n_params
-    for rel in (getattr(machine, "relations", None) or [machine.range256]):
-        rel.draw(ch, params)
-    # interaction traces: the main component sharded, the others replicated (a placeholder batch stands for the sharded columns they never read)
-    ph = [b for b in (shard0, shard1) if b is not None][0]
-    place = lambda total: ctx.wrap_device(ph.device_ptr, total, 0)
-    t0_list, t1_list = [place(big0)] + small0, [place(big1)] + small1
-    inter_small, claimed = [], []
-    shard2, cs = prover.gen_interaction_sharded(0, params)
-    claimed.append(cs)
-    params[main.cumsum_shift_param] = F.qm31_mul_m31(cs, F.m31_inv((1 << n) % P))
-    for k_, comp in enumerate(air.components[1:], start=1):
-        cols_k, cs = prover.gen_interaction_replicated(k_, comp.log_size, max(comp.batching) + 1, params, t0_list, t1_list)
-        inter_small.append(cols_k)
-        claimed.append(cs)
-        params[comp.cumsum_shift_param] = F.qm31_mul_m31(cs, F.m31_inv((1 << comp.log_size) % P))
-    ch.mix_felts(claimed)
-    big2 = 4 * (max(main.batching) + 1)
-    replicate2 = sorted({c for (tt, c, off) in main.masks if tt == 2 and off != 0})
-    root2 = prover.commit_sharded(shard2 if shard2.n_cols else None, big2, n, inter_small, replicate2, False, ch)
-    aux = {"params": params, "roots": [root0, root1, root2], "log_sizes": log_sizes, "associated_data": bytes(associated_data)}
+    aux = {"params": params, "roots": roots, "log_sizes": log_sizes, "associated_data": bytes(associated_data)}
     proof = prover.prove(ch, params)
     return proof, claimed, aux
 

@@ -77,15 +77,17 @@ def random_trees(m, seed, kind):
     return Witness(t0, t1, t2, params)
 
 
-def commit(backend, m, w):
-    """Machine::prove's commit sequence on `backend` with the witness's trees: (prover, params).  Without a tree 2 of its own the witness
-    gets the interaction trace the backend generates, with the cumsum shifts machine._commit_trees sets."""
+def commit(backend, m, w, log_sizes=()):
+    """Machine::prove's commit sequence on `backend` with the witness's trees: (prover, params); the prover keeps the three roots in `roots`.
+    Without a tree 2 of its own the witness gets the interaction trace the backend generates, with the cumsum shifts machine._commit_trees
+    sets.  `log_sizes` are mixed into the channel first, as Machine::prove mixes the components' log sizes."""
     ch = backend.channel()
+    for ls in log_sizes:
+        ch.mix_u64(ls)
     p = backend.prover(m.words, CONFIG)
-    p.commit(w.tree0, ch, coset_order=True)
-    p.commit(w.tree1, ch, coset_order=True)
+    p.roots = [p.commit(w.tree0, ch, coset_order=True), p.commit(w.tree1, ch, coset_order=True)]
     if w.tree2 is not None:
-        p.commit(w.tree2, ch)
+        p.roots.append(p.commit(w.tree2, ch))
         return p, list(w.params)
     params = [(0, 0, 0, 0)] * m.air.n_params
     for rel in (getattr(m, "relations", None) or [m.range256]):
@@ -95,7 +97,7 @@ def commit(backend, m, w):
         c, cs = p.gen_interaction(k, comp.log_size, max(comp.batching) + 1, params)
         inter.append(c)
         params[comp.cumsum_shift_param] = M.F.qm31_mul_m31(cs, M.F.m31_inv((1 << comp.log_size) % P))
-    p.commit_interaction(inter, ch)
+    p.roots.append(p.commit_interaction(inter, ch))
     p.interaction = inter
     return p, params
 

@@ -58,9 +58,12 @@ def half_route(m, k):
     return expand == CONFIG_BLOWUP + 1 and lg + CONFIG_BLOWUP > 8
 
 
-def check_full_route(ctx, m, gpu, orc_p, params, seed):
+def check_full_route(ctx, m, gpu, orc_p, params, seed, components=None):
+    """nb200_constraint_quotients against the oracle for every component (or those listed in `components`), added to a random accumulator."""
     rng = np.random.default_rng(seed)
     for k, (lg, expand, n) in enumerate(component_headers(m.words)):
+        if components is not None and k not in components:
+            continue
         elog = lg + expand
         coeffs = rw.mixed(rng, 4 * n).reshape(n, 4)
         acc0 = rw.mixed(rng, 4 << elog).reshape(4, -1)
