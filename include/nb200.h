@@ -185,6 +185,24 @@ nb200_status nb200_ram_init_final_trace(nb200_ctx*, size_t n_perms, const uint64
                                         size_t n_init, const uint32_t* init_addresses, const uint8_t* init_values, uint32_t log_size,
                                         nb200_cols* out, size_t* n_rows_out);
 
+/* ---- the v1 main component's main trace, filled on the device from an ADD / ADDI program's step record --------------------------
+ * The reference fills the main component's 347 columns (prover/src/column.rs) on the host, one row per executed step
+ * (Machine::prove's MainTrace stage, machine.rs:147-173).  Here only the step record crosses PCIe: steps = NB200_V1_STEP_FIELDS arrays of
+ * n_steps words each, field-major, in the order
+ *   pc, instruction word, opcode (0 ADD, 1 ADDI), rd, rs1, op_c (rs2 for ADD, the sign-extended immediate for ADDI), value of rs1,
+ *   value of rs2 or the immediate, previous value of rd, previous timestamps of the rs1 read, the rs2 read and the rd write (0 when not
+ *   accessed), previous execution count of the instruction at pc
+ * (add_chain.STEP_FIELDS), and final_ctr = the final execution count of each of the program's n_prog rows (FinalPrgMemoryCtr).  Step t is
+ * trace row t (clk = t + 1, register timestamps 3 clk + {1, 2, 3}); rows from n_steps on are the reference's padding rows.  The rows are
+ * the per-row fills of CpuChip, DecodingCheck types R / I, AddChip, ProgramMemCheck, RegisterMemCheck and Timestamp.
+ * out: a caller-owned batch of 347 columns and 2^log_size rows, overwritten in finalized order.
+ * NB200_ERR_ARG: log_size outside [4, 28], `out` of another shape, n_steps or n_prog above 2^log_size, an opcode other than ADD / ADDI, a
+ * register index above 31, a previous timestamp not below the current one, a previous execution count of 2^32 - 1.  Scratch memory is
+ * released in stream order. */
+#define NB200_V1_STEP_FIELDS 13
+nb200_status nb200_v1_main_trace(nb200_ctx*, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                                 nb200_cols* out);
+
 /* ---- one commitment over N GPUs (SURVEY §8e; one process per GPU, NCCL over NVLink inside the library) ------------------------
  * The reference has no multi-device path (SURVEY App. C); these entry points are what a multi-GPU `CudaBackend` would drive from
  * TreeBuilder::commit (machine.rs:208-263).  Rank 0 creates the id and hands it to the other ranks out of band (MPI, a file,

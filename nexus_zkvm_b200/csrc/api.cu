@@ -29,6 +29,8 @@ nb200_status keccak_main_trace(nb200_ctx* ctx, size_t n_perms, const uint64_t* i
 nb200_status ram_init_final_trace(nb200_ctx* ctx, size_t n_perms, const uint64_t* inputs, const uint32_t* addresses, const uint32_t* timestamps,
                                   size_t n_init, const uint32_t* init_addresses, const uint8_t* init_values, uint32_t log_size, nb200_cols* out,
                                   size_t* n_rows_out);
+nb200_status v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                           nb200_cols* out);
 }  // namespace nb
 using namespace nb;
 
@@ -473,6 +475,13 @@ nb200_status nb200_ram_init_final_trace(nb200_ctx* ctx, size_t n_perms, const ui
                                         nb200_cols* out, size_t* n_rows_out) {
   if (!ctx) return NB200_ERR_ARG;
   return ram_init_final_trace(ctx, n_perms, inputs, addresses, timestamps, n_init, init_addresses, init_values, log_size, out, n_rows_out);
+}
+
+// ---- the v1 main component's main trace from an ADD / ADDI program's step record (csrc/v1_trace.cu) ----
+nb200_status nb200_v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                                 nb200_cols* out) {
+  if (!ctx) return NB200_ERR_ARG;
+  return v1_main_trace(ctx, n_steps, steps, n_prog, final_ctr, log_size, out);
 }
 
 }  // extern "C"

@@ -1,0 +1,58 @@
+// The v1 main component's main trace filled on the device from an ADD / ADDI program's step record (nb200_v1_main_trace): what
+// add_chain.AddChainMachine.fill_main_trace() builds for the main component on the host, followed by finalize_columns, without the host
+// columns or their upload.  The batch is cleared first (the columns no ADD, ADDI or padding row sets stay zero); then one thread per
+// finalized row position writes its row's other columns (v1_trace.cuh), so consecutive threads write consecutive words of every column.
+#include "common.cuh"
+#include "v1_trace.cuh"
+#include <algorithm>
+
+namespace nb {
+namespace {
+
+constexpr u32 V1_BLOCK = 128;
+static_assert(v1::STEP_FIELDS == NB200_V1_STEP_FIELDS, "the step record of include/nb200.h");
+
+__global__ void __launch_bounds__(V1_BLOCK) v1_main_trace_kernel(const u32* __restrict__ steps, u32 n_steps, const u32* __restrict__ final_ctr,
+                                                                 u32 n_prog, u32 log_size, u32* out) {
+  const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (1u << log_size)) return;
+  v1::main_row(steps, n_steps, final_ctr, n_prog, log_size, i, out + i, (size_t)1 << log_size);
+}
+
+}  // namespace
+
+nb200_status v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                           nb200_cols* out) {
+  NB_ARG(ctx, out && (n_steps == 0 || steps) && (n_prog == 0 || final_ctr), "v1_main_trace: null argument");
+  NB_ARG(ctx, log_size >= 4 && log_size <= 28, "v1_main_trace: log_size must be in [4, 28]");
+  NB_ARG(ctx, out->n_cols == v1::MAIN_COLS && out->log_size == log_size, "v1_main_trace: out must be a batch of 347 columns of 2^log_size rows");
+  const size_t n = (size_t)1 << log_size;
+  NB_ARG(ctx, n_steps <= n, "v1_main_trace: more steps than 2^log_size rows");
+  NB_ARG(ctx, n_prog <= n, "v1_main_trace: more program rows than 2^log_size rows");
+  auto f = [&](u32 field, size_t t) { return steps[field * n_steps + t]; };
+  for (size_t t = 0; t < n_steps; ++t) {
+    const u32 op = f(v1::OPCODE, t);
+    NB_ARG(ctx, op == v1::OP_ADD || op == v1::OP_ADDI, "v1_main_trace: step " + std::to_string(t) + " is not ADD or ADDI");
+    NB_ARG(ctx, f(v1::RD, t) < 32 && f(v1::RS1, t) < 32 && (op != v1::OP_ADD || f(v1::OP_C, t) < 32),
+           "v1_main_trace: step " + std::to_string(t) + " has a register index above 31");
+    const u64 clk = t + 1;
+    for (u32 k = 0; k < 3; ++k)
+      NB_ARG(ctx, f(v1::TS1_PREV + k, t) < 3 * clk + k + 1,
+             "v1_main_trace: step " + std::to_string(t) + " has a previous timestamp not below the current one");
+    NB_ARG(ctx, f(v1::PC_CTR_PREV, t) != 0xFFFFFFFFu, "v1_main_trace: a program counter of 2^32 - 1 has no successor");
+  }
+  // scratch, freed in stream order when the call returns: the step record and the final counters
+  DevBuf d_steps, d_ctr;
+  NB_TRY(alloc(ctx, d_steps, std::max<size_t>(n_steps * v1::STEP_FIELDS, 1)));
+  NB_TRY(alloc(ctx, d_ctr, std::max<size_t>(n_prog, 1)));
+  if (n_steps)
+    NB_CUDA(ctx, cudaMemcpyAsync(d_steps.p, steps, n_steps * v1::STEP_FIELDS * 4, cudaMemcpyHostToDevice, ctx->stream));
+  if (n_prog) NB_CUDA(ctx, cudaMemcpyAsync(d_ctr.p, final_ctr, n_prog * 4, cudaMemcpyHostToDevice, ctx->stream));
+  NB_CUDA(ctx, cudaMemsetAsync(out->d, 0, (size_t)v1::MAIN_COLS * n * 4, ctx->stream));
+  v1_main_trace_kernel<<<(u32)((n + V1_BLOCK - 1) / V1_BLOCK), V1_BLOCK, 0, ctx->stream>>>(d_steps.p, (u32)n_steps, d_ctr.p, (u32)n_prog, log_size,
+                                                                                          out->d);
+  NB_LAUNCH_CHECK(ctx);
+  return NB200_OK;
+}
+
+}  // namespace nb

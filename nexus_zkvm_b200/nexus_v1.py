@@ -151,11 +151,74 @@ def padding_witness(log_size, seed=0):
     return t
 
 
-def record_main_component(air, log_size, rel, keccak=False):
+def _record_decoding_r_i(m, c, col, is_type_r, is_load, alu_imm_no_shift, alu_imm_shift, is_type_i_no_shift):
+    """DecodingCheckChip's TypeRChip and TypeIChip = (TypeINoShiftChip, TypeIShiftChip) constraints, in the reference's order: the register
+    and immediate fields of OpA / OpB / OpC and ValueC against their bit pieces, and the instruction word's bytes (InstrVal) against the
+    opcode, funct3 and funct7 of each instruction."""
+    one_m_imm, imm_c = 1 - c("ImmC"), c("ImmC")
+    a0, a14, b0, b14 = c("OpA0"), c("OpA1_4"), c("OpB0"), c("OpB1_4")
+    c03, c4, c47, c810, c11 = c("OpC0_3"), c("OpC4"), c("OpC4_7"), c("OpC8_10"), c("OpC11")
+    op_a, op_b, op_c = c("OpA"), c("OpB"), c("OpC")
+    iv, vc = col["InstrVal"], col["ValueC"]
+    funct3 = lambda f: a14 + f * 16 + b0 * 128 - iv[1]                    # op_a1_4 + funct3 2^4 + op_b0 2^7 - instr_val_2
+    # type R (type_r.rs:67-408)
+    m.add_constraint(is_type_r * (c03 + c4 * 16 - op_c))
+    m.add_constraint(is_type_r * (a0 + a14 * 2 - op_a))
+    m.add_constraint(is_type_r * (b0 + b14 * 2 - op_b))
+    m.add_constraint(is_type_r * (0b0110011 + a0 * 128 - iv[0]))
+    r_funct3 = [("IsAdd", 0b000), ("IsSub", 0b000), ("IsSll", 0b001), ("IsSlt", 0b010), ("IsSltu", 0b011), ("IsXor", 0b100), ("IsSrl", 0b101),
+                ("IsSra", 0b101), ("IsOr", 0b110), ("IsAnd", 0b111), ("IsMul", 0b000), ("IsMulhu", 0b011), ("IsDivu", 0b101), ("IsRemu", 0b111),
+                ("IsDiv", 0b100), ("IsRem", 0b110), ("IsMulhsu", 0b010), ("IsMulh", 0b001)]
+    for flag, f in r_funct3:
+        m.add_constraint(c(flag) * one_m_imm * funct3(f))
+    m.add_constraint(is_type_r * (b14 + c03 * 16 - iv[2]))
+    for flag, f7 in (("IsAdd", 0), ("IsSub", 0b0100000), ("IsSll", 0), ("IsSlt", 0), ("IsSltu", 0), ("IsXor", 0), ("IsSrl", 0),
+                     ("IsSra", 0b0100000), ("IsOr", 0), ("IsAnd", 0)):
+        m.add_constraint(c(flag) * one_m_imm * (c4 + f7 * 2 - iv[3]))
+    m_ops = c("IsMul") + c("IsMulhu") + c("IsDivu") + c("IsRemu") + c("IsDiv") + c("IsRem") + c("IsMulhsu") + c("IsMulh")
+    m.add_constraint(m_ops * one_m_imm * (c4 + 0b0000001 * 2 - iv[3]))
+    # type I without shift (type_i.rs:77-283)
+    t = is_type_i_no_shift
+    m.add_constraint(t * (c03 + c47 * 16 + c810 * 256 + c11 * 2048 - op_c))
+    m.add_constraint(t * (c03 + c47 * 16 - vc[0]))
+    m.add_constraint(t * (c810 + c11 * ((1 << 5) - 1) * 8 - vc[1]))
+    m.add_constraint(t * (c11 * 255 - vc[2]))
+    m.add_constraint(t * (c11 * 255 - vc[3]))
+    m.add_constraint(t * (a0 + a14 * 2 - op_a))
+    m.add_constraint(t * (b0 + b14 * 2 - op_b))
+    m.add_constraint(is_load * (0b0000011 + a0 * 128 - iv[0]))
+    m.add_constraint(alu_imm_no_shift * (0b0010011 + a0 * 128 - iv[0]))
+    m.add_constraint(c("IsJalr") * (0b1100111 + a0 * 128 - iv[0]))
+    for flag, f in (("IsLb", 0b000), ("IsLh", 0b001), ("IsLw", 0b010), ("IsLbu", 0b100), ("IsLhu", 0b101)):
+        m.add_constraint(c(flag) * funct3(f))
+    for flag, f in (("IsAdd", 0b000), ("IsSlt", 0b010), ("IsSltu", 0b011), ("IsXor", 0b100), ("IsOr", 0b110), ("IsAnd", 0b111)):
+        m.add_constraint(c(flag) * imm_c * funct3(f))
+    m.add_constraint(c("IsJalr") * funct3(0b000))
+    m.add_constraint(t * (b14 + c03 * 16 - iv[2]))
+    m.add_constraint(t * (c47 + c810 * 16 + c11 * 128 - iv[3]))
+    # type I with a shift amount (type_i.rs:335-441)
+    s = alu_imm_shift
+    m.add_constraint(s * (c03 + c4 * 16 - op_c))
+    m.add_constraint(s * (c03 + c4 * 16 - vc[0]))
+    for k in (1, 2, 3):
+        m.add_constraint(s * vc[k])
+    m.add_constraint(s * (a0 + a14 * 2 - op_a))
+    m.add_constraint(s * (b0 + b14 * 2 - op_b))
+    m.add_constraint(s * (0b0010011 + a0 * 128 - iv[0]))
+    for flag, f in (("IsSll", 0b001), ("IsSrl", 0b101), ("IsSra", 0b101)):
+        m.add_constraint(c(flag) * imm_c * funct3(f))
+    m.add_constraint(s * (b14 + c03 * 16 - iv[2]))
+    for flag, f7 in (("IsSll", 0), ("IsSrl", 0), ("IsSra", 0b0100000)):
+        m.add_constraint(c(flag) * imm_c * (c4 + f7 * 2 - iv[3]))
+
+
+def record_main_component(air, log_size, rel, keccak=False, decoding=False):
     """Record the main component (`MachineEval<BaseComponent>`, NexusV1Machine's docstring) into `air`: the chips in BaseComponent's order
     against the relations `rel` (name -> air.Relation: BitOp, LoadStore, ProgramCheck, RegisterCheck, Range8/16/32/128/256), then
     `finalize_logup()`.  `keccak`: the keccak extension is enabled, so KeccakChip (CustomInstructionChip, after LoadStoreChip) adds its
-    booleanity constraint on IsCustomKeccak (chips/custom.rs:178-196).  Returns (component, {column name: its masks})."""
+    booleanity constraint on IsCustomKeccak (chips/custom.rs:178-196).  `decoding`: DecodingCheckChip's type R and type I constraints
+    (_record_decoding_r_i) follow CpuChip's, as DecodingCheckChip follows CpuChip in BaseComponent; its types B, J, S, U and SYS are not
+    recorded.  Returns (component, {column name: its masks})."""
     m = air.component(log_size, 2)
     pre, col = {}, {}
     for name, size in PREPROCESSED_COLUMNS + PROGRAM_COLUMNS:           # TraceEval::new: preprocessed ids, then program ids
@@ -222,6 +285,9 @@ def record_main_component(air, log_size, rel, keccak=False):
     m.add_constraint(is_pc_incremented * (pc_next[2] + pc_next[3] * 256 + pc_carry[1] * 65536 - (pc[2] + pc[3] * 256) - pc_carry[0]))
     for k in (0, 2):
         m.add_constraint(is_type_sys * is_sys_halt * (pc[k] + pc[k + 1] * 256 - (pc_next[k] + pc_next[k + 1] * 256)))
+    # ---------------- DecodingCheckChip, types R and I (chips/decoding/type_r.rs:61-409, type_i.rs:71-442) ----------------
+    if decoding:
+        _record_decoding_r_i(m, c, col, is_type_r, is_load, alu_imm_no_shift, alu_imm_shift, is_type_i_no_shift)
     # ---------------- AddChip / SubChip ----------------
     cf = col["CarryFlag"]
     is_add, is_sub = c("IsAdd"), c("IsSub")
