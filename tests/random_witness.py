@@ -1,16 +1,19 @@
-"""Witnesses that are not valid traces, for testing the constraint, LogUp and check kernels where the padding witness says nothing.
+"""Witnesses that are not valid traces, for testing the constraint, LogUp and check kernels where a valid witness says nothing.
 
 The v1 padding witness (NexusV1Machine.fill_main_trace) leaves most of tree 1 zero or constant: a third of the v1 constraints, and 42 of
 the 45 that the half-coset D2 kernel evaluates, are identically zero under it, so a kernel could compute anything for them and still match
-the oracle.  The constraint quotients, the interaction trace and the check report are defined for any trees and parameters, so the tests
-compare them on these witnesses instead:
+the oracle.  The ADD chain's executing trace (add_chain.AddChainMachine, no seed: its program is fixed) does little better: every opcode flag
+but IsAdd / ImmC is zero, so 181 of its main component's 486 constraints, 80 of the 110 of degree > 2 and 55 of the 73 DecodingCheck ones
+are identically zero.  The constraint quotients, the interaction trace and the check report are defined for any trees and parameters, so
+the tests compare them on these witnesses instead:
 
   full         every cell of trees 0 and 1 random, tree 2 and every parameter (lookup elements, cumsum shifts) random as well: the chip
                constraints and the LogUp constraints fail;
   main_random  trees 0 and 1 random, tree 2 from the interaction-trace generator and the cumsum shifts set as machine._commit_trees sets
                them: the chip constraints fail, the LogUp constraints hold;
-  sparse       the valid (padding) witness with about 1 % of the cells of every tree-1 column replaced, rows 0 and N - 1 among them (the
-               masks at a row offset wrap around there): each constraint fails on its own subset of rows.
+  sparse       the valid witness (v1: the padding witness, the ADD chain: its executing trace) with about 1 % of the cells of every
+               tree-1 column replaced, rows 0 and N - 1 among them (the masks at a row offset wrap around there): each constraint fails
+               on its own subset of rows.
 
 Random cells are drawn from a mix that brings the field's edges into every constraint: uniform in [0, P), P - 1, 0, 1, bytes and 16-bit
 values.  Everything is seeded."""
@@ -18,6 +21,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from nexus_zkvm_b200 import add_chain as AC
 from nexus_zkvm_b200 import air as A
 from nexus_zkvm_b200 import machine as M
 from oracle import pyoracle as orc
@@ -49,7 +53,10 @@ def mixed(rng, n):
 
 
 def valid_tree1(m, seed=1):
-    """The machine's own witness (the padding witness for v1), tree-1 host columns in trace order."""
+    """The machine's own witness (the padding witness for v1, the executing trace for the ADD chain, which takes no seed), tree-1 host
+    columns in trace order."""
+    if isinstance(m, AC.AddChainMachine):
+        return ref.flat(m.fill_main_trace())
     if isinstance(m, M.AddMachine):
         cols, mult = m.fill_main_trace(seed=seed, n_padding=2)
         return ref.flat(list(cols) + [mult])
@@ -103,7 +110,7 @@ def commit(backend, m, w, log_sizes=()):
 
 
 def padding(m, seed=1):
-    """The machine's valid witness as a Witness (for v1: the padding witness)."""
+    """The machine's valid witness as a Witness (for v1: the padding witness, for the ADD chain: its executing trace)."""
     return Witness(ref.flat(m.preprocessed_columns()), valid_tree1(m, seed))
 
 
