@@ -407,6 +407,18 @@ typedef struct { uint32_t column; uint32_t value[4]; } nb200_sample_entry;
 nb200_status nb200_fri_quotients(nb200_ctx*, const nb200_cols* const* batches, size_t n_batches, uint32_t log_size,
                                  const nb200_sample_batch* sample_batches, size_t n_sample_batches,
                                  const nb200_sample_entry* entries, size_t n_entries, const uint32_t random_coeff[4], nb200_cols** out);
+/* The same quotient over the LDEs (2^log_size rows) of the columns whose coefficients (2^(log_size - log_blowup) words each) the batches
+ * hold, by the route nb200_prove takes: each sample batch's columns are combined on their coefficients and only the combinations are
+ * extended.  Needs at least one sample batch and log_size >= log_blowup + 2. */
+nb200_status nb200_fri_quotients_from_coeffs(nb200_ctx*, const nb200_cols* const* coeffs, size_t n_batches, uint32_t log_size, uint32_t log_blowup,
+                                             const nb200_sample_batch* sample_batches, size_t n_sample_batches,
+                                             const nb200_sample_entry* entries, size_t n_entries, const uint32_t random_coeff[4], nb200_cols** out);
+/* Host only: the tables of that route.  Sample batches must list their entries in order (first_entry = the entries before them).
+ * lines_out: per sample batch 24 words: point x (CM31 parts 0, 1 of x then of y, then 2, 3 of x then of y), A[4], B[4] (the sums of the
+ * alpha-weighted line coefficients), random_coeff ^ n_entries [4], c[4] = conj(y) - y; alphas_out: per entry its alpha (4 words),
+ * random_coeff ^ (1 + its index in the batch). */
+nb200_status nb200_deep_plan(const nb200_sample_batch* sample_batches, size_t n_sample_batches, const nb200_sample_entry* entries, size_t n_entries,
+                             const uint32_t random_coeff[4], uint32_t* lines_out, uint32_t* alphas_out);
 /* FriOps::fold_circle_into_line: dst = dst * alpha^2 + fold(src); src = secure column on CanonicCoset(k).circle_domain(),
  * dst = secure column of 2^(k-1) values on LineDomain(Coset::half_odds(k-1)) */
 nb200_status nb200_fold_circle_into_line(nb200_ctx*, nb200_cols* dst, const nb200_cols* src, const uint32_t alpha[4]);

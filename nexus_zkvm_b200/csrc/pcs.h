@@ -17,9 +17,23 @@ struct QBatchDev {
 };
 struct QEntryDev { u32 c[4]; const u32* col; u32 pad[2]; };  // 32 bytes; c first so that it loads as one 128-bit word
 
+// a sample batch of the combined route: numerator c G(x) - (A y + B), G = the batch's combination sum_k alpha^k f_k (deep_combine)
+struct QLineDev {
+  u32 prx[2], pry[2], pix[2], piy[2];  // CM31 parts of the sample point
+  u32 A[4], B[4];                      // as in QBatchDev
+  u32 coeff[4];                        // random_coeff ^ (columns in batch)
+  u32 c[4];                            // conj(p.y) - p.y
+};
+
 nb200_status domain_points(nb200_ctx* ctx, u32 log_size, u32* d_x, u32* d_y);
 nb200_status quotients_launch(nb200_ctx* ctx, const QBatchDev* h_batches, size_t n_batches, const QEntryDev* h_entries, size_t n_entries,
                               const u32* dom_x, const u32* dom_y, u32 log_size, u32* out /* 4 columns */, u32 row0 = 0, size_t n_rows = 0);
+// g = per batch (4 columns of 2^log_n each, batch after batch) the sum over entries [first, first + count) of entry.c (QM31) x entry.col
+nb200_status deep_combine(nb200_ctx* ctx, const uint2* h_ranges /* (first, count) */, size_t n_batches, const QEntryDev* h_entries, size_t n_entries,
+                          u32 log_n, u32* g);
+// out (4 columns of 2^log_size) = the DEEP quotient of the batches from their extended combinations g (4 columns of 2^log_size per batch)
+nb200_status quotients_combined(nb200_ctx* ctx, const QLineDev* h_batches, size_t n_batches, const u32* g, const u32* dom_x, const u32* dom_y,
+                                u32 log_size, u32* out);
 nb200_status fold_circle_into_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, qm31 alpha);
 nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, qm31 alpha);
 nb200_status fold_line(nb200_ctx* ctx, u32* dst, const u32* src, u32 src_log, const u32* d_alpha);   // alpha: 4 words in device memory

@@ -25,30 +25,49 @@ static nb200_status ensure_gen_table(nb200_ctx* ctx) {
   return NB200_OK;
 }
 
-// x/y of CanonicCoset(log).circle_domain() in bit-reversed order
-__global__ void domain_points_kernel(u32 log_size, u32* __restrict__ xs, u32* __restrict__ ys) {
+// x/y of CanonicCoset(log).circle_domain() in bit-reversed order.  Position i holds the point of index init + step jj of the half coset
+// half_odds(log-1) (initial = subgroup_gen(log+1), step = subgroup_gen(log-1); jj = bit-reversed i modulo the half), conjugated in the
+// second half.  With jj = lo + 2^k hi that point is P_lo[lo] + P_hi[hi]: two small tables (domain_tables_kernel) and one group addition
+// per point instead of a 31-step scalar multiplication.  The group law is exact, so the words do not depend on how the sum is split.
+__device__ __forceinline__ cpoint point_of_index(u32 idx) {
+  cpoint r{1, 0};
+#pragma unroll 1
+  for (int b = 0; b < 31; ++b) if ((idx >> b) & 1u) r = cp_add(r, c_gen_pow2_pcs[b]);
+  return r;
+}
+// lo[t] = (init + step t) G for t < 2^k; hi[t] = (step 2^k t) G for t < 2^(log_size - 1 - k)
+__global__ void domain_tables_kernel(u32 log_size, u32 k, cpoint* __restrict__ lo, cpoint* __restrict__ hi) {
+  const u32 t = blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 init = 1u << (31 - (log_size + 1));
+  const u32 step = (log_size - 1 == 0) ? 0u : (1u << (31 - (log_size - 1)));
+  const u32 n_lo = 1u << k, n_hi = 1u << (log_size - 1 - k);
+  if (t < n_lo) lo[t] = point_of_index((init + (u32)(((u64)step * t) & 0x7fffffffu)) & 0x7fffffffu);
+  else if (t - n_lo < n_hi) hi[t - n_lo] = point_of_index((u32)(((u64)step * ((u64)(t - n_lo) << k)) & 0x7fffffffu));
+}
+__global__ void domain_points_kernel(u32 log_size, u32 k, const cpoint* __restrict__ lo, const cpoint* __restrict__ hi,
+                                     u32* __restrict__ xs, u32* __restrict__ ys) {
   u32 i = blockIdx.x * blockDim.x + threadIdx.x;
   u32 n = 1u << log_size;
   if (i >= n) return;
   u32 j = __brev(i) >> (32 - log_size);
   u32 half = n >> 1;
-  // half coset = half_odds(log-1): initial = subgroup_gen(log+1), step = subgroup_gen(log-1)
-  u32 init = 1u << (31 - (log_size + 1));
-  u32 step = (log_size - 1 == 0) ? 0u : (1u << (31 - (log_size - 1)));
   u32 jj = j < half ? j : j - half;
-  u32 idx = (init + (u32)(((u64)step * jj) & 0x7fffffffu)) & 0x7fffffffu;
-  cpoint r{1, 0};
-#pragma unroll 1
-  for (int b = 0; b < 31; ++b) if ((idx >> b) & 1u) r = cp_add(r, c_gen_pow2_pcs[b]);
+  const cpoint r = cp_add(lo[jj & ((1u << k) - 1)], hi[jj >> k]);
   xs[i] = r.x;
   ys[i] = j < half ? r.y : m31_neg(r.y);
 }
 nb200_status domain_points(nb200_ctx* ctx, u32 log_size, u32* d_x, u32* d_y) {
   NB_TRY(ensure_gen_table(ctx));
   NB_ARG(ctx, log_size >= 1 && log_size <= 30, "domain_points: log size");
+  const u32 k = (log_size - 1) / 2, n_tab = (1u << k) + (1u << (log_size - 1 - k));
+  cpoint* d_tab = nullptr;
+  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_tab, (size_t)n_tab * sizeof(cpoint)));
   u32 n = 1u << log_size, thr = 256;
-  domain_points_kernel<<<(n + thr - 1) / thr, thr, 0, ctx->stream>>>(log_size, d_x, d_y);
+  domain_tables_kernel<<<(n_tab + thr - 1) / thr, thr, 0, ctx->stream>>>(log_size, k, d_tab, d_tab + (1u << k));
   NB_LAUNCH_CHECK(ctx);
+  domain_points_kernel<<<(n + thr - 1) / thr, thr, 0, ctx->stream>>>(log_size, k, d_tab, d_tab + (1u << k), d_x, d_y);
+  NB_LAUNCH_CHECK(ctx);
+  dfree(ctx, d_tab);   // ordered after the kernels on the stream
   return NB200_OK;
 }
 
@@ -100,9 +119,88 @@ __global__ void __launch_bounds__(256) quotients_kernel(const QBatchDev* __restr
   o0[row] = acc.c[0]; o1[row] = acc.c[1]; o2[row] = acc.c[2]; o3[row] = acc.c[3];
 }
 
-// Four consecutive rows per thread: every column is read with 128-bit loads (512 contiguous bytes per warp and column instead of
-// 128: the sweep jumps 2^log_size words from column to column, so longer bursts matter for DRAM efficiency) and the per-entry
-// constants are fetched once for four rows.  Same arithmetic as quotients_kernel.
+// cm31_inv of four values with one field inversion: Montgomery's trick on their norms a^2 + b^2 (the norm of a nonzero value is nonzero,
+// -1 being no square mod P).  When a norm is zero the product is zero, and each value is inverted on its own as cm31_inv does (0 -> 0).
+__device__ __forceinline__ void cm31_inv4(const cm31 (&d)[4], cm31 (&out)[4]) {
+  u32 n[4], ni[4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) n[r] = m31_add(m31_mul(d[r].a, d[r].a), m31_mul(d[r].b, d[r].b));
+  const u32 p01 = m31_mul(n[0], n[1]), p012 = m31_mul(p01, n[2]), p = m31_mul(p012, n[3]);
+  if (p != 0) {
+    u32 t = m31_inv(p);                              // 1 / (n0 n1 n2 n3)
+    ni[3] = m31_mul(t, p012); t = m31_mul(t, n[3]);  // t = 1 / (n0 n1 n2)
+    ni[2] = m31_mul(t, p01);  t = m31_mul(t, n[2]);  // t = 1 / (n0 n1)
+    ni[1] = m31_mul(t, n[0]); ni[0] = m31_mul(t, n[1]);
+  } else {
+#pragma unroll
+    for (int r = 0; r < 4; ++r) ni[r] = m31_inv(n[r]);
+  }
+#pragma unroll
+  for (int r = 0; r < 4; ++r) out[r] = cm31{m31_mul(d[r].a, ni[r]), m31_neg(m31_mul(d[r].b, ni[r]))};
+}
+
+// s[r][j] += sum over the entries of coordinate j of en[e].c times word (row + r) of column en[e].col, for r < 4: the column reads of
+// quotients_kernel_x4 and deep_combine_kernel.  Every column is read with 128-bit loads (512 contiguous bytes per warp and column instead
+// of 128: the sweep jumps 2^log_size words from column to column, so longer bursts matter for DRAM efficiency) and the per-entry
+// constants are fetched once for four rows.  Lazy reduction: four products (< 2^62 each) plus a reduced carry-in fit in 64 bits, so the
+// sums are reduced after every group of four entries; on return each s[r][j] holds a reduced value plus at most three products.
+__device__ __forceinline__ void sum_entries_x4(const QEntryDev* __restrict__ en, u32 count, u32 row, u64 (&s)[4][4]) {
+  u32 e = 0;
+  for (; e + 8 <= count; e += 8) {   // eight columns (128 bytes) in flight per thread: two groups of four, one reduction per group
+    uint4 f[8];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) f[u] = __ldg(reinterpret_cast<const uint4*>(en[e + u].col + row));
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      uint4 k[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) k[u] = __ldg(reinterpret_cast<const uint4*>(en[e + 4 * h + u].c));
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const u32 fr[4] = {f[4 * h + u].x, f[4 * h + u].y, f[4 * h + u].z, f[4 * h + u].w};
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+          s[r][0] += (u64)fr[r] * k[u].x; s[r][1] += (u64)fr[r] * k[u].y; s[r][2] += (u64)fr[r] * k[u].z; s[r][3] += (u64)fr[r] * k[u].w;
+        }
+      }
+#pragma unroll
+      for (int r = 0; r < 4; ++r)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) s[r][j] = m31_red64(s[r][j]);
+    }
+  }
+  for (; e + 4 <= count; e += 4) {   // four columns in flight per thread (the loop is latency bound otherwise), then one reduction
+    uint4 f[4], k[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) f[u] = __ldg(reinterpret_cast<const uint4*>(en[e + u].col + row));
+#pragma unroll
+    for (int u = 0; u < 4; ++u) k[u] = __ldg(reinterpret_cast<const uint4*>(en[e + u].c));
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const u32 fr[4] = {f[u].x, f[u].y, f[u].z, f[u].w};
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        s[r][0] += (u64)fr[r] * k[u].x; s[r][1] += (u64)fr[r] * k[u].y; s[r][2] += (u64)fr[r] * k[u].z; s[r][3] += (u64)fr[r] * k[u].w;
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[r][j] = m31_red64(s[r][j]);
+  }
+  for (; e < count; ++e) {           // at most three left: still within 64 bits
+    const uint4 f = __ldg(reinterpret_cast<const uint4*>(en[e].col + row));
+    const uint4 k = __ldg(reinterpret_cast<const uint4*>(en[e].c));
+    const u32 fr[4] = {f.x, f.y, f.z, f.w};
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      s[r][0] += (u64)fr[r] * k.x; s[r][1] += (u64)fr[r] * k.y; s[r][2] += (u64)fr[r] * k.z; s[r][3] += (u64)fr[r] * k.w;
+    }
+  }
+}
+
+// Four consecutive rows per thread (sum_entries_x4), their four denominators inverted together (cm31_inv4).  Same field values as
+// quotients_kernel.
 __global__ void __launch_bounds__(128) quotients_kernel_x4(const QBatchDev* __restrict__ batches, u32 n_batches, const QEntryDev* __restrict__ entries,
                                                            const u32* __restrict__ dom_x, const u32* __restrict__ dom_y, u32 log_size,
                                                            u32* __restrict__ o0, u32* __restrict__ o1, u32* __restrict__ o2, u32* __restrict__ o3, u32 row0, u32 row_end) {
@@ -118,71 +216,23 @@ __global__ void __launch_bounds__(128) quotients_kernel_x4(const QBatchDev* __re
     for (int r = 0; r < 4; ++r)
 #pragma unroll
       for (int j = 0; j < 4; ++j) s[r][j] = 0;
-    const u32 first = qb->first, count = qb->count;
-    const QEntryDev* en = entries + first;
-    u32 e = 0;
-    for (; e + 8 <= count; e += 8) {   // eight columns (128 bytes) in flight per thread: two groups of four, one reduction per group
-      uint4 f[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) f[u] = __ldg(reinterpret_cast<const uint4*>(en[e + u].col + row));
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint4 k[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) k[u] = __ldg(reinterpret_cast<const uint4*>(en[e + 4 * h + u].c));
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const u32 fr[4] = {f[4 * h + u].x, f[4 * h + u].y, f[4 * h + u].z, f[4 * h + u].w};
-#pragma unroll
-          for (int r = 0; r < 4; ++r) {
-            s[r][0] += (u64)fr[r] * k[u].x; s[r][1] += (u64)fr[r] * k[u].y; s[r][2] += (u64)fr[r] * k[u].z; s[r][3] += (u64)fr[r] * k[u].w;
-          }
-        }
-#pragma unroll
-        for (int r = 0; r < 4; ++r)
-#pragma unroll
-          for (int j = 0; j < 4; ++j) s[r][j] = m31_red64(s[r][j]);
-      }
-    }
-    for (; e + 4 <= count; e += 4) {   // four columns in flight per thread (the loop is latency bound otherwise), then one reduction
-      uint4 f[4], k[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) f[u] = __ldg(reinterpret_cast<const uint4*>(en[e + u].col + row));
-#pragma unroll
-      for (int u = 0; u < 4; ++u) k[u] = __ldg(reinterpret_cast<const uint4*>(en[e + u].c));
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const u32 fr[4] = {f[u].x, f[u].y, f[u].z, f[u].w};
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-          s[r][0] += (u64)fr[r] * k[u].x; s[r][1] += (u64)fr[r] * k[u].y; s[r][2] += (u64)fr[r] * k[u].z; s[r][3] += (u64)fr[r] * k[u].w;
-        }
-      }
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) s[r][j] = m31_red64(s[r][j]);
-    }
-    for (; e < count; ++e) {           // at most three left: still within 64 bits
-      const uint4 f = __ldg(reinterpret_cast<const uint4*>(en[e].col + row));
-      const uint4 k = __ldg(reinterpret_cast<const uint4*>(en[e].c));
-      const u32 fr[4] = {f.x, f.y, f.z, f.w};
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        s[r][0] += (u64)fr[r] * k.x; s[r][1] += (u64)fr[r] * k.y; s[r][2] += (u64)fr[r] * k.z; s[r][3] += (u64)fr[r] * k.w;
-      }
-    }
+    sum_entries_x4(entries + qb->first, qb->count, row, s);
     const qm31 A = qm31_make(qb->A[0], qb->A[1], qb->A[2], qb->A[3]);
     const qm31 B = qm31_make(qb->B[0], qb->B[1], qb->B[2], qb->B[3]);
     const cm31 prx{qb->prx[0], qb->prx[1]}, pry{qb->pry[0], qb->pry[1]}, pix{qb->pix[0], qb->pix[1]}, piy{qb->piy[0], qb->piy[1]};
     const qm31 cf = qm31_make(qb->coeff[0], qb->coeff[1], qb->coeff[2], qb->coeff[3]);
+    cm31 den[4], inv[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const cm31 dx{m31_sub(prx.a, xs[r]), prx.b}, dy{m31_sub(pry.a, ys[r]), pry.b};
+      den[r] = cm31_sub(cm31_mul(dx, piy), cm31_mul(dy, pix));
+    }
+    cm31_inv4(den, inv);
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
       qm31 numer = qm31_make(m31_red64(s[r][0]), m31_red64(s[r][1]), m31_red64(s[r][2]), m31_red64(s[r][3]));
       numer = qm31_sub(numer, qm31_add(qm31_mul_m31(A, ys[r]), B));
-      cm31 dx{m31_sub(prx.a, xs[r]), prx.b}, dy{m31_sub(pry.a, ys[r]), pry.b};
-      cm31 den = cm31_sub(cm31_mul(dx, piy), cm31_mul(dy, pix));
-      acc[r] = qm31_add(qm31_mul(acc[r], cf), qm31_mul_cm31(numer, cm31_inv(den)));
+      acc[r] = qm31_add(qm31_mul(acc[r], cf), qm31_mul_cm31(numer, inv[r]));
     }
   }
   *reinterpret_cast<uint4*>(o0 + row) = make_uint4(acc[0].c[0], acc[1].c[0], acc[2].c[0], acc[3].c[0]);
@@ -216,6 +266,105 @@ nb200_status quotients_launch(nb200_ctx* ctx, const QBatchDev* h_batches, size_t
   // no sync: the host tables may go once the copies above have returned (a copy from pageable host memory is staged by then), and the
   // frees are ordered after the kernel on the stream
   dfree(ctx, d_b); dfree(ctx, d_e);
+  return NB200_OK;
+}
+
+// ---- DEEP quotients from combined coefficients (deep_quotients in prove.cu) ----
+// The numerator of sample batch b is sum_k (alpha_k c_b) f_k(x) - (A_b y + B_b) = c_b G_b(x) - (A_b y + B_b) with G_b = sum_k alpha_k f_k.
+// G_b is formed on the columns' coefficients (half the words of their LDE) and extended once; the row kernel then reads G_b's four
+// coordinate columns per batch instead of every column.  Field arithmetic is exact, so the quotient is the same word for word.
+
+// g (4 coordinate columns of 2^log_n per batch, batch after batch) = per batch b, sum over its entries of alpha_k (entry.c) times the
+// coefficient column entry.col.  One thread per four coefficients of one batch: grid (coefficient blocks, batches).
+__global__ void __launch_bounds__(128, 8) deep_combine_kernel(const uint2* __restrict__ ranges /* (first entry, count) per batch */,
+                                                           const QEntryDev* __restrict__ entries, u32 log_n, u32* __restrict__ g) {
+  const u32 i = (blockIdx.x * blockDim.x + threadIdx.x) * 4u;
+  const size_t n = (size_t)1 << log_n;
+  if (i >= n) return;
+  const uint2 rg = __ldg(ranges + blockIdx.y);
+  u64 s[4][4];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s[r][j] = 0;
+  sum_entries_x4(entries + rg.x, rg.y, i, s);
+  u32* gb = g + ((size_t)blockIdx.y * 4) * n;
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    *reinterpret_cast<uint4*>(gb + j * n + i) = make_uint4(m31_red64(s[0][j]), m31_red64(s[1][j]), m31_red64(s[2][j]), m31_red64(s[3][j]));
+}
+nb200_status deep_combine(nb200_ctx* ctx, const uint2* h_ranges, size_t n_batches, const QEntryDev* h_entries, size_t n_entries, u32 log_n, u32* g) {
+  NB_ARG(ctx, log_n >= 2 && (((uintptr_t)g) & 15u) == 0, "deep_combine: 4-word aligned columns of at least 4 coefficients");
+  for (size_t e = 0; e < n_entries; ++e) NB_ARG(ctx, (((uintptr_t)h_entries[e].col) & 15u) == 0, "deep_combine: 4-word aligned columns");
+  uint2* d_r = nullptr; QEntryDev* d_e = nullptr;
+  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_r, n_batches * sizeof(uint2)));
+  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_e, n_entries * sizeof(QEntryDev)));
+  NB_CUDA(ctx, cudaMemcpyAsync(d_r, h_ranges, n_batches * sizeof(uint2), cudaMemcpyHostToDevice, ctx->stream));
+  NB_CUDA(ctx, cudaMemcpyAsync(d_e, h_entries, n_entries * sizeof(QEntryDev), cudaMemcpyHostToDevice, ctx->stream));
+  const u32 thr = 128;
+  const size_t nt = ((size_t)1 << log_n) / 4;
+  deep_combine_kernel<<<dim3((u32)((nt + thr - 1) / thr), (u32)n_batches), thr, 0, ctx->stream>>>(d_r, d_e, log_n, g);
+  NB_LAUNCH_CHECK(ctx);
+  dfree(ctx, d_r); dfree(ctx, d_e);   // ordered after the kernel on the stream (see quotients_launch)
+  return NB200_OK;
+}
+
+// out (4 columns of 2^log_size) = the DEEP quotient from g, the extended combinations (4 columns of 2^log_size per batch).  Four rows per
+// thread; the denominators and the chaining by random_coeff ^ (columns in batch) are those of quotients_kernel_x4.
+__global__ void __launch_bounds__(128) quotients_combined_kernel(const QLineDev* __restrict__ batches, u32 n_batches, const u32* __restrict__ g,
+                                                                 const u32* __restrict__ dom_x, const u32* __restrict__ dom_y, u32 log_size,
+                                                                 u32* __restrict__ o0, u32* __restrict__ o1, u32* __restrict__ o2, u32* __restrict__ o3) {
+  const size_t n = (size_t)1 << log_size;
+  const u32 row = (blockIdx.x * blockDim.x + threadIdx.x) * 4u;
+  if (row >= n) return;
+  const uint4 xv = __ldg(reinterpret_cast<const uint4*>(dom_x + row)), yv = __ldg(reinterpret_cast<const uint4*>(dom_y + row));
+  const u32 xs[4] = {xv.x, xv.y, xv.z, xv.w}, ys[4] = {yv.x, yv.y, yv.z, yv.w};
+  qm31 acc[4] = {qm31_zero(), qm31_zero(), qm31_zero(), qm31_zero()};
+  for (u32 b = 0; b < n_batches; ++b) {
+    const QLineDev* qb = batches + b;
+    const u32* gb = g + ((size_t)b * 4) * n + row;
+    uint4 v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) v[j] = __ldg(reinterpret_cast<const uint4*>(gb + j * n));
+    const qm31 A = qm31_make(qb->A[0], qb->A[1], qb->A[2], qb->A[3]);
+    const qm31 B = qm31_make(qb->B[0], qb->B[1], qb->B[2], qb->B[3]);
+    const qm31 c = qm31_make(qb->c[0], qb->c[1], qb->c[2], qb->c[3]);
+    const cm31 prx{qb->prx[0], qb->prx[1]}, pry{qb->pry[0], qb->pry[1]}, pix{qb->pix[0], qb->pix[1]}, piy{qb->piy[0], qb->piy[1]};
+    const qm31 cf = qm31_make(qb->coeff[0], qb->coeff[1], qb->coeff[2], qb->coeff[3]);
+    const u32 gx[4] = {v[0].x, v[0].y, v[0].z, v[0].w}, gy[4] = {v[1].x, v[1].y, v[1].z, v[1].w};
+    const u32 gz[4] = {v[2].x, v[2].y, v[2].z, v[2].w}, gw[4] = {v[3].x, v[3].y, v[3].z, v[3].w};
+    cm31 den[4], inv[4];
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const cm31 dx{m31_sub(prx.a, xs[r]), prx.b}, dy{m31_sub(pry.a, ys[r]), pry.b};
+      den[r] = cm31_sub(cm31_mul(dx, piy), cm31_mul(dy, pix));
+    }
+    cm31_inv4(den, inv);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      qm31 numer = qm31_mul(c, qm31_make(gx[r], gy[r], gz[r], gw[r]));
+      numer = qm31_sub(numer, qm31_add(qm31_mul_m31(A, ys[r]), B));
+      acc[r] = qm31_add(qm31_mul(acc[r], cf), qm31_mul_cm31(numer, inv[r]));
+    }
+  }
+  *reinterpret_cast<uint4*>(o0 + row) = make_uint4(acc[0].c[0], acc[1].c[0], acc[2].c[0], acc[3].c[0]);
+  *reinterpret_cast<uint4*>(o1 + row) = make_uint4(acc[0].c[1], acc[1].c[1], acc[2].c[1], acc[3].c[1]);
+  *reinterpret_cast<uint4*>(o2 + row) = make_uint4(acc[0].c[2], acc[1].c[2], acc[2].c[2], acc[3].c[2]);
+  *reinterpret_cast<uint4*>(o3 + row) = make_uint4(acc[0].c[3], acc[1].c[3], acc[2].c[3], acc[3].c[3]);
+}
+nb200_status quotients_combined(nb200_ctx* ctx, const QLineDev* h_batches, size_t n_batches, const u32* g, const u32* dom_x, const u32* dom_y,
+                                u32 log_size, u32* out /* 4 columns */) {
+  NB_ARG(ctx, log_size >= 2 && ((((uintptr_t)out) | ((uintptr_t)g) | ((uintptr_t)dom_x) | ((uintptr_t)dom_y)) & 15u) == 0,
+         "quotients_combined: 4-word aligned columns of at least 4 rows");
+  QLineDev* d_b = nullptr;
+  NB_CUDA(ctx, dmalloc(ctx, (void**)&d_b, n_batches * sizeof(QLineDev)));
+  NB_CUDA(ctx, cudaMemcpyAsync(d_b, h_batches, n_batches * sizeof(QLineDev), cudaMemcpyHostToDevice, ctx->stream));
+  const size_t n = (size_t)1 << log_size;
+  const u32 thr = 128;
+  quotients_combined_kernel<<<(u32)((n / 4 + thr - 1) / thr), thr, 0, ctx->stream>>>(d_b, (u32)n_batches, g, dom_x, dom_y, log_size,
+                                                                                   out, out + n, out + 2 * n, out + 3 * n);
+  NB_LAUNCH_CHECK(ctx);
+  dfree(ctx, d_b);
   return NB200_OK;
 }
 

@@ -742,6 +742,57 @@ nb200_status accumulate_quotients(nb200_ctx* ctx, u32 lg, const std::vector<Samp
   return quotients_launch(ctx, qb.data(), qb.size(), qe.data(), qe.size(), dom->col(0), dom->col(1), lg, out, row0, n_rows);
 }
 
+// The host tables of the combined route (quotients_from_coeffs): per batch, its columns with their alphas (q_coeff^1, ^2, ... in batch
+// order, as accumulate_quotients numbers them) as deep_combine entries, the entry range, and the line descriptor whose numerator is
+// c G(x) - (A y + B).  A and B are accumulate_quotients' sums; c = conj(p.y) - p.y takes the place of its per-entry alpha c.
+void deep_plan(const std::vector<SampleBatch>& hb, qm31 q_coeff, std::vector<QLineDev>& lines, std::vector<QEntryDev>& entries, std::vector<uint2>& ranges) {
+  lines.assign(hb.size(), QLineDev{}); entries.clear(); ranges.assign(hb.size(), uint2{0, 0});
+  for (size_t b = 0; b < hb.size(); ++b) {
+    QLineDev& L = lines[b];
+    const qpoint& p = hb[b].p;
+    L.prx[0] = p.x.c[0]; L.prx[1] = p.x.c[1]; L.pix[0] = p.x.c[2]; L.pix[1] = p.x.c[3];
+    L.pry[0] = p.y.c[0]; L.pry[1] = p.y.c[1]; L.piy[0] = p.y.c[2]; L.piy[1] = p.y.c[3];
+    const qm31 c = qm31_sub(qm31_conj(p.y), p.y);
+    qm31 alpha = qm31_one(), sa = qm31_zero(), sb = qm31_zero();
+    ranges[b] = uint2{(u32)entries.size(), (u32)hb[b].cols.size()};
+    for (auto& cv : hb[b].cols) {
+      alpha = qm31_mul(alpha, q_coeff);
+      // complex_conjugate_line_coeffs
+      qm31 a = qm31_sub(qm31_conj(cv.second), cv.second);
+      qm31 bq = qm31_sub(qm31_mul(cv.second, c), qm31_mul(a, p.y));
+      sa = qm31_add(sa, qm31_mul(alpha, a)); sb = qm31_add(sb, qm31_mul(alpha, bq));
+      QEntryDev e; e.col = cv.first; memcpy(e.c, alpha.c, 16); e.pad[0] = e.pad[1] = 0;
+      entries.push_back(e);
+    }
+    memcpy(L.A, sa.c, 16); memcpy(L.B, sb.c, 16); memcpy(L.c, c.c, 16);
+    qm31 bc = qm31_pow(q_coeff, hb[b].cols.size());
+    memcpy(L.coeff, bc.c, 16);
+  }
+}
+
+// accumulate_quotients over the LDEs (2^lg rows) of the columns whose coefficients (2^(lg - blow) each) the batches name: each batch's
+// combination G_b = sum_k alpha_k f_k is formed on the coefficients, the 4 x n_batches combination columns are extended to 2^lg rows
+// (LDE evaluation is linear and exact, so these are G_b's values on the LDE), and the row kernel reads them instead of every column.
+nb200_status quotients_from_coeffs(nb200_ctx* ctx, u32 lg, u32 blow, const std::vector<SampleBatch>& hc, qm31 q_coeff, u32* out) {
+  NB_ARG(ctx, !hc.empty() && lg >= blow + 2, "quotients_from_coeffs: at least one batch and 4 coefficients per column");
+  std::vector<QLineDev> lines; std::vector<QEntryDev> entries; std::vector<uint2> ranges;
+  deep_plan(hc, q_coeff, lines, entries, ranges);
+  const u32 n = lg - blow;
+  const size_t nb = hc.size();
+  ColsPtr ext;
+  NB_TRY(alloc(ctx, ext, 4 * nb, lg));
+  {
+    ColsPtr g;
+    NB_TRY(alloc(ctx, g, 4 * nb, n));
+    NB_TRY(deep_combine(ctx, ranges.data(), nb, entries.data(), entries.size(), n, g->d));
+    NB_TRY(fft_evaluate(ctx, g->d, n, ext->d, lg, 4 * nb));
+  }
+  ColsPtr dom;
+  NB_TRY(alloc(ctx, dom, 2, lg));
+  NB_TRY(domain_points(ctx, lg, dom->col(0), dom->col(1)));
+  return quotients_combined(ctx, lines.data(), nb, ext->d, dom->col(0), dom->col(1), lg, out);
+}
+
 // ---- stwo::prover::prove, one function per stage; prove_impl runs them in order ----
 
 static nb200_status zeroed(nb200_ctx* ctx, u32 lg, ColsPtr& out) {
@@ -918,6 +969,17 @@ struct FriState {
   std::vector<FriLayer> inner;
 };
 
+// Whether quotients_from_coeffs beats accumulate_quotients over the LDEs for these batches.  Each entry it combines on the coefficients
+// saves reading half an LDE column (blow-up 2), and each of the 4 x n_batches combination columns it extends costs about as much as
+// reading 6 LDE columns (H100, profiles/README.md: 12 columns extended to 2^21 rows in 0.20 ms; one such column read in 2.9 us).  A group
+// breaks even at about 12 entries per extended column; the rule asks for 32.  The v1 main group (1395 entries at 3 points) passes; a
+// group of a few columns, such as the composition's 4 at one point, stays on the LDEs.
+static bool combine_pays(const std::vector<SampleBatch>& hc) {
+  size_t entries = 0;
+  for (auto& b : hc) entries += b.cols.size();
+  return !hc.empty() && entries >= 32 * 4 * hc.size();
+}
+
 static nb200_status deep_quotients(nb200_scheme* s, const OodsSamples& o, HostChannel& ch, FriState& f) {
   nb200_ctx* ctx = s->ctx;
   qm31 q_coeff = ch.draw_felt();
@@ -929,7 +991,8 @@ static nb200_status deep_quotients(nb200_scheme* s, const OodsSamples& o, HostCh
     size_t j = i; while (j < all.size() && all[j].log == all[i].log) ++j;
     const u32 lg = all[i].log;
     // ColumnSampleBatch::new_vec: group samples by point, first-seen order                   [risk: IndexMap vs BTreeMap]
-    std::vector<SampleBatch> hb;
+    // hb names the columns' LDEs, hc the same batches with their coefficients (the combined route; unused when the group is sharded)
+    std::vector<SampleBatch> hb, hc;
     const SchemeTree* sharded = nullptr;   // a tree whose row slices this group reads
     for (size_t k = i; k < j; ++k) {
       const CRef& r = all[k];
@@ -937,12 +1000,15 @@ static nb200_status deep_quotients(nb200_scheme* s, const OodsSamples& o, HostCh
         const qpoint& p = o.points[r.t][r.g][pi];
         size_t b = 0;
         for (; b < hb.size(); ++b) if (qm31_eq(hb[b].p.x, p.x) && qm31_eq(hb[b].p.y, p.y)) break;
-        if (b == hb.size()) hb.push_back(SampleBatch{p, {}});
+        if (b == hb.size()) { hb.push_back(SampleBatch{p, {}}); hc.push_back(SampleBatch{p, {}}); }
         const SchemeTree& trr = s->trees[r.t];
         if (trr.sharded && trr.cols[r.g].batch == SchemeTree::BIG) {
           sharded = &trr;
           hb[b].cols.push_back({trr.lde_rows(trr.cols[r.g].idx), o.sampled[r.t][r.g][pi]});
-        } else hb[b].cols.push_back({trr.lde_ptr(r.g), o.sampled[r.t][r.g][pi]});
+        } else {
+          hb[b].cols.push_back({trr.lde_ptr(r.g), o.sampled[r.t][r.g][pi]});
+          hc[b].cols.push_back({trr.coeff_ptr(r.g), o.sampled[r.t][r.g][pi]});
+        }
       }
     }
     ColsPtr q;
@@ -952,7 +1018,8 @@ static nb200_status deep_quotients(nb200_scheme* s, const OodsSamples& o, HostCh
       const u32 r0 = (u32)sharded->row0();
       NB_TRY(accumulate_quotients(ctx, lg, hb, q_coeff, q->d, r0, rows));
       for (int qq = 0; qq < 4; ++qq) NB_TRY(comm_all_gather_dev(ctx, q->col(qq) + r0, rows, q->col(qq)));
-    } else NB_TRY(accumulate_quotients(ctx, lg, hb, q_coeff, q->d));
+    } else if (combine_pays(hc) && lg >= s->log_blowup + 2) NB_TRY(quotients_from_coeffs(ctx, lg, s->log_blowup, hc, q_coeff, q->d));
+    else NB_TRY(accumulate_quotients(ctx, lg, hb, q_coeff, q->d));
     f.quotients.push_back(std::move(q)); f.qlogs.push_back(lg);
     i = j;
   }
@@ -1513,6 +1580,29 @@ nb200_status gen_interaction_sharded(nb200_scheme* s, nb200_air* air_h, u32 comp
   return NB200_OK;
 }
 
+// the sample batches of nb200_fri_quotients(_from_coeffs): columns numbered through the device batches, each of 2^col_log words
+static nb200_status sample_batches_of(nb200_ctx* ctx, const nb200_cols* const* batches, size_t n_batches, u32 col_log,
+                                      const nb200_sample_batch* sample_batches, size_t n_sample_batches, const nb200_sample_entry* entries,
+                                      size_t n_entries, std::vector<SampleBatch>& hb) {
+  std::vector<const u32*> cols;
+  for (size_t b = 0; b < n_batches; ++b) {
+    NB_ARG(ctx, batches[b] && batches[b]->log_size == col_log, "fri_quotients: every column must have 2^log_size rows (from coefficients: 2^(log_size - log_blowup) words)");
+    for (size_t c = 0; c < batches[b]->n_cols; ++c) cols.push_back(batches[b]->col(c));
+  }
+  hb.assign(n_sample_batches, SampleBatch{});
+  for (size_t b = 0; b < n_sample_batches; ++b) {
+    const nb200_sample_batch& sb = sample_batches[b];
+    NB_ARG(ctx, sb.first_entry <= n_entries && sb.n_entries <= n_entries - sb.first_entry, "fri_quotients: sample batch entry range");
+    memcpy(hb[b].p.x.c, sb.point, 16); memcpy(hb[b].p.y.c, sb.point + 4, 16);
+    for (size_t e = sb.first_entry; e < sb.first_entry + sb.n_entries; ++e) {
+      NB_ARG(ctx, entries[e].column < cols.size(), "fri_quotients: column index out of range");
+      qm31 v; memcpy(v.c, entries[e].value, 16);
+      hb[b].cols.push_back({cols[entries[e].column], v});
+    }
+  }
+  return NB200_OK;
+}
+
 }  // namespace nb
 
 using namespace nb;
@@ -1766,27 +1856,53 @@ nb200_status nb200_fri_quotients(nb200_ctx* ctx, const nb200_cols* const* batche
                                  const nb200_sample_batch* sample_batches, size_t n_sample_batches,
                                  const nb200_sample_entry* entries, size_t n_entries, const uint32_t random_coeff[4], nb200_cols** out) {
   if (!ctx || (!batches && n_batches) || (!sample_batches && n_sample_batches) || (!entries && n_entries) || !random_coeff || !out) return NB200_ERR_ARG;
-  std::vector<const u32*> cols;
-  for (size_t b = 0; b < n_batches; ++b) {
-    NB_ARG(ctx, batches[b] && batches[b]->log_size == log_size, "fri_quotients: every column must have 2^log_size rows");
-    for (size_t c = 0; c < batches[b]->n_cols; ++c) cols.push_back(batches[b]->col(c));
-  }
-  std::vector<SampleBatch> hb(n_sample_batches);
-  for (size_t b = 0; b < n_sample_batches; ++b) {
-    const nb200_sample_batch& sb = sample_batches[b];
-    NB_ARG(ctx, sb.first_entry <= n_entries && sb.n_entries <= n_entries - sb.first_entry, "fri_quotients: sample batch entry range");
-    memcpy(hb[b].p.x.c, sb.point, 16); memcpy(hb[b].p.y.c, sb.point + 4, 16);
-    for (size_t e = sb.first_entry; e < sb.first_entry + sb.n_entries; ++e) {
-      NB_ARG(ctx, entries[e].column < cols.size(), "fri_quotients: column index out of range");
-      qm31 v; memcpy(v.c, entries[e].value, 16);
-      hb[b].cols.push_back({cols[entries[e].column], v});
-    }
-  }
+  std::vector<SampleBatch> hb;
+  NB_TRY(sample_batches_of(ctx, batches, n_batches, log_size, sample_batches, n_sample_batches, entries, n_entries, hb));
   qm31 rc; memcpy(rc.c, random_coeff, 16);
   ColsPtr q;
   NB_TRY(alloc(ctx, q, 4, log_size));
   NB_TRY(accumulate_quotients(ctx, log_size, hb, rc, q->d));
   *out = q.release();
+  return NB200_OK;
+}
+nb200_status nb200_fri_quotients_from_coeffs(nb200_ctx* ctx, const nb200_cols* const* coeffs, size_t n_batches, uint32_t log_size, uint32_t log_blowup,
+                                             const nb200_sample_batch* sample_batches, size_t n_sample_batches,
+                                             const nb200_sample_entry* entries, size_t n_entries, const uint32_t random_coeff[4], nb200_cols** out) {
+  if (!ctx || (!coeffs && n_batches) || (!sample_batches && n_sample_batches) || (!entries && n_entries) || !random_coeff || !out) return NB200_ERR_ARG;
+  NB_ARG(ctx, log_size >= log_blowup + 2 && n_sample_batches > 0, "fri_quotients_from_coeffs: at least one sample batch and 4 coefficients per column");
+  std::vector<SampleBatch> hc;
+  NB_TRY(sample_batches_of(ctx, coeffs, n_batches, log_size - log_blowup, sample_batches, n_sample_batches, entries, n_entries, hc));
+  NB_TRY(twiddles_prepare(ctx, log_size));
+  qm31 rc; memcpy(rc.c, random_coeff, 16);
+  ColsPtr q;
+  NB_TRY(alloc(ctx, q, 4, log_size));
+  NB_TRY(quotients_from_coeffs(ctx, log_size, log_blowup, hc, rc, q->d));
+  *out = q.release();
+  return NB200_OK;
+}
+nb200_status nb200_deep_plan(const nb200_sample_batch* sample_batches, size_t n_sample_batches, const nb200_sample_entry* entries, size_t n_entries,
+                             const uint32_t random_coeff[4], uint32_t* lines_out, uint32_t* alphas_out) {
+  if ((!sample_batches && n_sample_batches) || (!entries && n_entries) || !random_coeff || (!lines_out && n_sample_batches) || (!alphas_out && n_entries))
+    return NB200_ERR_ARG;
+  std::vector<SampleBatch> hb(n_sample_batches);
+  size_t total = 0;
+  for (size_t b = 0; b < n_sample_batches; ++b) {
+    const nb200_sample_batch& sb = sample_batches[b];
+    if (sb.first_entry != total || sb.n_entries > n_entries - total) return NB200_ERR_ARG;
+    memcpy(hb[b].p.x.c, sb.point, 16); memcpy(hb[b].p.y.c, sb.point + 4, 16);
+    for (size_t e = sb.first_entry; e < sb.first_entry + sb.n_entries; ++e) {
+      qm31 v; memcpy(v.c, entries[e].value, 16);
+      hb[b].cols.push_back({nullptr, v});
+    }
+    total += sb.n_entries;
+  }
+  if (total != n_entries) return NB200_ERR_ARG;
+  qm31 rc; memcpy(rc.c, random_coeff, 16);
+  std::vector<QLineDev> lines; std::vector<QEntryDev> qe; std::vector<uint2> ranges;
+  deep_plan(hb, rc, lines, qe, ranges);
+  static_assert(sizeof(QLineDev) == 24 * 4, "QLineDev: 24 words");
+  if (n_sample_batches) memcpy(lines_out, lines.data(), lines.size() * sizeof(QLineDev));
+  for (size_t e = 0; e < qe.size(); ++e) memcpy(alphas_out + 4 * e, qe[e].c, 16);
   return NB200_OK;
 }
 nb200_status nb200_constraint_quotients(nb200_scheme* s, const nb200_air* air, uint32_t component, const uint32_t* params, size_t n_params,

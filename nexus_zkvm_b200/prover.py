@@ -306,6 +306,44 @@ def fri_quotients(ctx, batches, log_size, sample_batches, random_coeff):
     return Columns(ctx, out)
 
 
+def _sample_tables(sample_batches):
+    n_e = sum(len(e) for _p, e in sample_batches)
+    sb = (SampleBatch * max(len(sample_batches), 1))()
+    se = (SampleEntry * max(n_e, 1))()
+    k = 0
+    for i, (pt, ents) in enumerate(sample_batches):
+        sb[i].point = (C.c_uint32 * 8)(*[int(x) for x in np.asarray(pt, dtype=np.uint32).reshape(8)])
+        sb[i].first_entry, sb[i].n_entries = k, len(ents)
+        for ci, v in ents:
+            se[k].column = int(ci); se[k].value = _q(v); k += 1
+    return sb, se, n_e
+
+
+def fri_quotients_from_coeffs(ctx, coeffs, log_size, log_blowup, sample_batches, random_coeff):
+    """fri_quotients over the LDEs (2^log_size rows) of the columns whose coefficients (2^(log_size - log_blowup) words) `coeffs` holds, by
+    the prover's route: every sample batch's columns combined on their coefficients, then only the combinations extended."""
+    arr = (C.c_void_p * len(coeffs))(*[b._h for b in coeffs])
+    sb, se, n_e = _sample_tables(sample_batches)
+    out = C.c_void_p()
+    ctx._chk(lib().nb200_fri_quotients_from_coeffs(ctx._h, arr, C.c_size_t(len(coeffs)), C.c_uint32(log_size), C.c_uint32(log_blowup), sb,
+                                                   C.c_size_t(len(sample_batches)), se, C.c_size_t(n_e), _q(random_coeff), C.byref(out)))
+    return Columns(ctx, out)
+
+
+def deep_plan(sample_batches, random_coeff):
+    """The host tables of fri_quotients_from_coeffs (no device): (lines, alphas).  lines: n_batches x 24 words (point parts
+    x0 x1 y0 y1 x2 x3 y2 y3, A[4], B[4], random_coeff ^ n_entries [4], c[4]); alphas: one row of 4 words per entry.  Columns are ignored."""
+    sb, se, n_e = _sample_tables(sample_batches)
+    lines = np.zeros((max(len(sample_batches), 1), 24), np.uint32)
+    alphas = np.zeros((max(n_e, 1), 4), np.uint32)
+    u32p = C.POINTER(C.c_uint32)
+    st = lib().nb200_deep_plan(sb, C.c_size_t(len(sample_batches)), se, C.c_size_t(n_e), _q(random_coeff), lines.ctypes.data_as(u32p),
+                               alphas.ctypes.data_as(u32p))
+    if st != 0:
+        raise RuntimeError(f"nb200_deep_plan failed: status {st}")
+    return lines[:len(sample_batches)], alphas[:n_e]
+
+
 class CudaBackend:
     """Backend protocol used by nexus_zkvm_b200.machine.prove (the stand-in for `SimdBackend`)."""
 

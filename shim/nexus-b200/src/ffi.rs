@@ -159,6 +159,11 @@ extern "C" {
     pub fn nb200_fri_quotients(ctx: *mut nb200_ctx, batches: *const *const nb200_cols, n_batches: usize, log_size: u32,
                                sample_batches: *const nb200_sample_batch, n_sample_batches: usize, entries: *const nb200_sample_entry, n_entries: usize,
                                random_coeff: *const u32, out: *mut *mut nb200_cols) -> c_int;
+    pub fn nb200_fri_quotients_from_coeffs(ctx: *mut nb200_ctx, coeffs: *const *const nb200_cols, n_batches: usize, log_size: u32, log_blowup: u32,
+                                           sample_batches: *const nb200_sample_batch, n_sample_batches: usize, entries: *const nb200_sample_entry,
+                                           n_entries: usize, random_coeff: *const u32, out: *mut *mut nb200_cols) -> c_int;
+    pub fn nb200_deep_plan(sample_batches: *const nb200_sample_batch, n_sample_batches: usize, entries: *const nb200_sample_entry, n_entries: usize,
+                           random_coeff: *const u32, lines_out: *mut u32, alphas_out: *mut u32) -> c_int;
     pub fn nb200_fold_circle_into_line(ctx: *mut nb200_ctx, dst: *mut nb200_cols, src: *const nb200_cols, alpha: *const u32) -> c_int;
     pub fn nb200_fold_line(ctx: *mut nb200_ctx, src: *const nb200_cols, alpha: *const u32, dst_out: *mut *mut nb200_cols) -> c_int;
     pub fn nb200_grind(ctx: *mut nb200_ctx, digest: *const u8, pow_bits: u32, nonce_out: *mut u64) -> c_int;
