@@ -203,6 +203,19 @@ nb200_status nb200_ram_init_final_trace(nb200_ctx*, size_t n_perms, const uint64
 nb200_status nb200_v1_main_trace(nb200_ctx*, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
                                  nb200_cols* out);
 
+/* ---- the same fill for a straight-line program of RV32I's ALU instructions -------------------------------------------------------
+ * nb200_v1_main_trace's arguments, step record and kernel, for every RV32I register-register and register-immediate instruction but
+ * LUI / AUIPC (add_chain.OPCODES).  The opcode field takes
+ *    0 ADD     1 ADDI    2 SUB     3 SLL     4 SLT     5 SLTU    6 XOR     7 SRL     8 SRA     9 OR     10 AND
+ *   11 SLTI   12 SLTIU  13 XORI   14 ORI    15 ANDI   16 SLLI   17 SRLI   18 SRAI
+ * ADD, SUB ... AND are type R: op_c is rs2 and value_c its value.  ADDI and SLTI ... ANDI are type I: op_c = value_c = the sign-extended
+ * 12-bit immediate.  SLLI, SRLI and SRAI are type I with a shift amount: op_c = value_c = the 5-bit amount.  The rows add the per-row fills
+ * of SubChip, SltuChip, BitOpChip, SltChip, SllChip, SrlChip and SraChip and DecodingCheck's type I with a shift amount.
+ * NB200_ERR_ARG: what nb200_v1_main_trace refuses but its opcode rule, and an opcode above 18, a shift amount above 31 on SLLI / SRLI /
+ * SRAI, a type-I immediate that is not a sign-extended 12-bit value. */
+nb200_status nb200_v1_alu_trace(nb200_ctx*, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                                nb200_cols* out);
+
 /* ---- one commitment over N GPUs (SURVEY §8e; one process per GPU, NCCL over NVLink inside the library) ------------------------
  * The reference has no multi-device path (SURVEY App. C); these entry points are what a multi-GPU `CudaBackend` would drive from
  * TreeBuilder::commit (machine.rs:208-263).  Rank 0 creates the id and hands it to the other ranks out of band (MPI, a file,

@@ -283,6 +283,18 @@ class Context:
                                             C.c_uint32(log_size), out._h))
         return out
 
+    def v1_alu_trace(self, steps, final_ctr, log_size, out=None):
+        """nb200_v1_alu_trace: v1_main_trace for a program of the 19 ALU opcodes of add_chain.OPCODES (ADD ... SRAI), same arguments and
+        step record.  Returns out."""
+        st = np.ascontiguousarray(steps, dtype=np.uint32)
+        ctr = np.ascontiguousarray(final_ctr, dtype=np.uint32)
+        assert st.ndim == 2 and st.shape[0] == 13 and ctr.ndim == 1, "step record shapes"
+        if out is None:
+            out = self.alloc(347, log_size)
+        self._chk(lib().nb200_v1_alu_trace(self._h, C.c_size_t(st.shape[1]), st.ctypes.data_as(u32p), C.c_size_t(ctr.size), ctr.ctypes.data_as(u32p),
+                                           C.c_uint32(log_size), out._h))
+        return out
+
     def table_multiplicities(self, air, tree0, tree1, first_row=False):
         """nb200_table_multiplicities: every table fraction's multiplicity column of `tree1` (device batches, finalized order) is overwritten
         with the count of the AIR's lookups into it.  `air` is a loaded AIR (prover.Air).  Returns (n_unmatched, first_unmatched), the latter

@@ -12,15 +12,20 @@ step; the view has no initial, input, exit-code or output memory, so RamInitFina
 Components, in the reference's order:
    0 main component              nexus_v1.record_main_component with DecodingCheck's types R and I (decoding=True)
    1 FinalReg                    the final register file: (index, final timestamp, final value) per register
-   2 BitOpMultiplicity           no bit-op lookup here: zero
+   2 BitOpMultiplicity           no bit-op lookup in the ADD chain: zero
    3 RamInitFinal                2^4 zero rows
    4-8 Multiplicity8/16/32/128/256
 Relations: BitOp, LoadStore, ProgramCheck, RegisterCheck, Range8, 16, 32, 128, 256 (draw_lookup_elements over BaseComponent).
 
-The step record (`STEP_FIELDS`, one uint32 row per field, one column per step) is what the device fill (nb200_v1_main_trace,
-csrc/v1_trace.{cu,cuh}) takes; `fill_main_trace` is its numpy reference, a port of the per-row fills of CpuChip (cpu.rs:36-316), DecodingCheck
-R / I (type_r.rs:25-60, type_i.rs:29-69), AddChip (add.rs:64-100), ProgramMemCheck (program_mem_check.rs:44-100), RegisterMemCheck
-(register_mem_check.rs:53-117) and Timestamp (timestamp.rs:33-75) for ADD, ADDI and padding rows."""
+AluMachine runs a straight-line program of every RV32I register-register and register-immediate instruction but LUI / AUIPC (OPCODES,
+alu_program) on the same components, its main component also recorded with SltuChip, SltChip, SllChip, SrlChip and SraChip (alu=True); its
+bit-op instructions make BitOpMultiplicity nonzero.
+
+The step record (`STEP_FIELDS`, one uint32 row per field, one column per step) is what the device fill (nb200_v1_main_trace for ADD / ADDI,
+nb200_v1_alu_trace for the 19 opcodes, csrc/v1_trace.{cu,cuh}) takes; `fill_main_trace` is its numpy reference, a port of the per-row fills
+of CpuChip (cpu.rs:36-316), DecodingCheck R / I / I with a shift amount (type_r.rs:25-60, type_i.rs:29-69,288-330), AddChip (add.rs:64-100),
+SubChip, SltuChip, BitOpChip, SltChip, SllChip, SrlChip, SraChip, ProgramMemCheck (program_mem_check.rs:44-100), RegisterMemCheck
+(register_mem_check.rs:53-117) and Timestamp (timestamp.rs:33-75) for executed and padding rows."""
 import numpy as np
 
 from . import air as A
@@ -30,19 +35,109 @@ from . import whole_machine as W
 P = (1 << 31) - 1
 ELF_TEXT_START = 136                       # PUBLIC_OUTPUT_ADDRESS_LOCATION + 4 (common/src/constants/mod.rs:8-10)
 NUM_REGISTERS = 32
-OP_ADD, OP_ADDI = 0, 1
-# the step record, field by field (nb200_v1_main_trace's `steps`): op_c is rs2 for ADD and the sign-extended immediate for ADDI; the
-# three previous timestamps are those of the rs1 read, the rs2 read and the rd write (0 when the access does not happen); pc_ctr_prev is
-# how often the instruction at pc was executed before
+# the step record's opcode numbers (include/nb200.h): (mnemonic, instruction type, funct3, funct7, the main component's flag column);
+# type "R" reads rs2, "I" takes a 12-bit immediate, "IShift" a 5-bit shift amount (SLLI / SRLI / SRAI, funct7 in the immediate's top bits)
+OPCODES = [("ADD", "R", 0b000, 0, "IsAdd"), ("ADDI", "I", 0b000, 0, "IsAdd"), ("SUB", "R", 0b000, 0b0100000, "IsSub"),
+           ("SLL", "R", 0b001, 0, "IsSll"), ("SLT", "R", 0b010, 0, "IsSlt"), ("SLTU", "R", 0b011, 0, "IsSltu"), ("XOR", "R", 0b100, 0, "IsXor"),
+           ("SRL", "R", 0b101, 0, "IsSrl"), ("SRA", "R", 0b101, 0b0100000, "IsSra"), ("OR", "R", 0b110, 0, "IsOr"), ("AND", "R", 0b111, 0, "IsAnd"),
+           ("SLTI", "I", 0b010, 0, "IsSlt"), ("SLTIU", "I", 0b011, 0, "IsSltu"), ("XORI", "I", 0b100, 0, "IsXor"), ("ORI", "I", 0b110, 0, "IsOr"),
+           ("ANDI", "I", 0b111, 0, "IsAnd"), ("SLLI", "IShift", 0b001, 0, "IsSll"), ("SRLI", "IShift", 0b101, 0, "IsSrl"),
+           ("SRAI", "IShift", 0b101, 0b0100000, "IsSra")]
+(OP_ADD, OP_ADDI, OP_SUB, OP_SLL, OP_SLT, OP_SLTU, OP_XOR, OP_SRL, OP_SRA, OP_OR, OP_AND, OP_SLTI, OP_SLTIU, OP_XORI, OP_ORI, OP_ANDI,
+ OP_SLLI, OP_SRLI, OP_SRAI) = range(len(OPCODES))
+OP_TYPE = [ty for _n, ty, _f3, _f7, _flag in OPCODES]
+R_TWIN = ["SLTU" if n == "SLTIU" else n if ty == "R" else n[:-1] for n, ty, _f3, _f7, _flag in OPCODES]   # what each opcode computes
+# the step record, field by field (nb200_v1_main_trace's and nb200_v1_alu_trace's `steps`): op_c is rs2 for type R, the sign-extended
+# 12-bit immediate for type I and the shift amount for SLLI / SRLI / SRAI, value_c is rs2's value or op_c; the three previous timestamps
+# are those of the rs1 read, the rs2 read and the rd write (0 when the access does not happen); pc_ctr_prev is how often the instruction at
+# pc was executed before
 STEP_FIELDS = ["pc", "word", "opcode", "rd", "rs1", "op_c", "value_b", "value_c", "rd_prev", "ts1_prev", "ts2_prev", "ts3_prev", "pc_ctr_prev"]
 
 
+def encode(op, rd, rs1, c):
+    """The RV32I instruction word of opcode number `op` with rd, rs1 and c = rs2, the immediate or the shift amount."""
+    _name, ty, f3, f7, _flag = OPCODES[op]
+    if ty == "R":
+        return (f7 << 25) | (c << 20) | (rs1 << 15) | (f3 << 12) | (rd << 7) | 0b0110011
+    if ty == "I":
+        return ((c & 0xFFF) << 20) | (rs1 << 15) | (f3 << 12) | (rd << 7) | 0b0010011
+    return (f7 << 25) | ((c & 31) << 20) | (rs1 << 15) | (f3 << 12) | (rd << 7) | 0b0010011
+
+
 def encode_add(rd, rs1, rs2):
-    return (rs2 << 20) | (rs1 << 15) | (rd << 7) | 0b0110011
+    return encode(OP_ADD, rd, rs1, rs2)
 
 
 def encode_addi(rd, rs1, imm):
-    return ((imm & 0xFFF) << 20) | (rs1 << 15) | (rd << 7) | 0b0010011
+    return encode(OP_ADDI, rd, rs1, imm)
+
+
+def encode_sub(rd, rs1, rs2):
+    return encode(OP_SUB, rd, rs1, rs2)
+
+
+def encode_sll(rd, rs1, rs2):
+    return encode(OP_SLL, rd, rs1, rs2)
+
+
+def encode_slt(rd, rs1, rs2):
+    return encode(OP_SLT, rd, rs1, rs2)
+
+
+def encode_sltu(rd, rs1, rs2):
+    return encode(OP_SLTU, rd, rs1, rs2)
+
+
+def encode_xor(rd, rs1, rs2):
+    return encode(OP_XOR, rd, rs1, rs2)
+
+
+def encode_srl(rd, rs1, rs2):
+    return encode(OP_SRL, rd, rs1, rs2)
+
+
+def encode_sra(rd, rs1, rs2):
+    return encode(OP_SRA, rd, rs1, rs2)
+
+
+def encode_or(rd, rs1, rs2):
+    return encode(OP_OR, rd, rs1, rs2)
+
+
+def encode_and(rd, rs1, rs2):
+    return encode(OP_AND, rd, rs1, rs2)
+
+
+def encode_slti(rd, rs1, imm):
+    return encode(OP_SLTI, rd, rs1, imm)
+
+
+def encode_sltiu(rd, rs1, imm):
+    return encode(OP_SLTIU, rd, rs1, imm)
+
+
+def encode_xori(rd, rs1, imm):
+    return encode(OP_XORI, rd, rs1, imm)
+
+
+def encode_ori(rd, rs1, imm):
+    return encode(OP_ORI, rd, rs1, imm)
+
+
+def encode_andi(rd, rs1, imm):
+    return encode(OP_ANDI, rd, rs1, imm)
+
+
+def encode_slli(rd, rs1, shamt):
+    return encode(OP_SLLI, rd, rs1, shamt)
+
+
+def encode_srli(rd, rs1, shamt):
+    return encode(OP_SRLI, rd, rs1, shamt)
+
+
+def encode_srai(rd, rs1, shamt):
+    return encode(OP_SRAI, rd, rs1, shamt)
 
 
 def add_chain_program(log_size, n_instructions=None):
@@ -53,34 +148,77 @@ def add_chain_program(log_size, n_instructions=None):
         ops.append((OP_ADD, k, j, i))
         i, j, k = (i + 1) % NUM_REGISTERS, (j + 1) % NUM_REGISTERS, (k + 1) % NUM_REGISTERS
     ops = ops[:n]
-    words = np.array([encode_add(rd, rs1, c) if op == OP_ADD else encode_addi(rd, rs1, c) for op, rd, rs1, c in ops], np.uint32)
+    words = np.array([encode(*op) for op in ops], np.uint32)
     return words, ops
 
 
+# alu_program's fixed prefix: registers driven through 0, 1, -1, 0x7FFFFFFF and 0x80000000, then the edge cases of each instruction
+ALU_PREFIX = [
+    (OP_ADDI, 1, 0, 1), (OP_ADDI, 2, 0, -1), (OP_SRLI, 3, 2, 1), (OP_SLLI, 4, 1, 31), (OP_ADDI, 5, 0, 0),   # x1..x5 = 1, -1, max, min, 0
+    (OP_SLT, 6, 3, 3), (OP_SLTU, 7, 4, 4), (OP_SLT, 8, 4, 3), (OP_SLTU, 9, 3, 4), (OP_SLT, 10, 2, 5),     # equal operands, both signs
+    (OP_SRA, 11, 4, 2), (OP_SRAI, 12, 4, 31), (OP_SRL, 13, 2, 5), (OP_SLLI, 14, 2, 0), (OP_SLL, 15, 3, 2),  # rs2 = -1: bits above 4 set
+    (OP_ADDI, 16, 0, 33), (OP_SLL, 17, 3, 16), (OP_SRL, 18, 4, 16), (OP_SRA, 19, 4, 16),                 # rs2 = 33: shift by 1
+    (OP_ADDI, 20, 3, -2048), (OP_SLTIU, 21, 2, -2048), (OP_SLTI, 22, 4, -2048), (OP_SLTIU, 23, 5, 1),    # immediate -2048, seqz
+    (OP_XORI, 24, 3, -1), (OP_ORI, 25, 4, -2048), (OP_ANDI, 26, 2, -2048), (OP_SLTI, 27, 1, 1),
+    (OP_SUB, 28, 4, 1), (OP_SUB, 29, 0, 4), (OP_SUB, 30, 5, 2), (OP_ADD, 31, 3, 1),                      # min - 1, -min, 0 - (-1), max + 1
+    (OP_XOR, 1, 3, 4), (OP_OR, 2, 4, 5), (OP_AND, 3, 2, 4), (OP_SRAI, 4, 3, 31),
+    (OP_ADD, 0, 2, 2), (OP_XOR, 0, 3, 4), (OP_SRAI, 0, 2, 31), (OP_SLTU, 0, 0, 2),                       # writes to x0
+]
+IMM_EDGES = [-2048, -2047, -1, 0, 1, 2, 15, 16, 255, 256, 2046, 2047]
+
+
+def alu_program(log_size, n_instructions=None, seed=0):
+    """A seeded straight-line program of `n_instructions` (default 2^log_size) instructions over all 19 opcodes: ALU_PREFIX, then each
+    instruction drawn uniformly with random registers, immediates (a quarter of them from IMM_EDGES) and shift amounts.
+    (words uint32, [(opcode, rd, rs1, rs2 / imm / shift amount)])."""
+    n = (1 << log_size) if n_instructions is None else int(n_instructions)
+    rng = np.random.default_rng(seed)
+    m = max(0, n - len(ALU_PREFIX))
+    op = rng.integers(0, len(OPCODES), m)
+    rd, rs1, rs2 = (rng.integers(0, NUM_REGISTERS, m) for _ in range(3))
+    imm = np.where(rng.integers(0, 4, m) == 0, np.array(IMM_EDGES)[rng.integers(0, len(IMM_EDGES), m)], rng.integers(-2048, 2048, m))
+    shamt = rng.integers(0, 32, m)
+    c = np.select([np.array(OP_TYPE)[op] == "R", np.array(OP_TYPE)[op] == "I"], [rs2, imm], shamt)
+    ops = (ALU_PREFIX + [tuple(int(x) for x in row) for row in zip(op, rd, rs1, c)])[:n]
+    return np.array([encode(*o) for o in ops], np.uint32), ops
+
+
+def alu(op, b, c):
+    """RV32I's result of opcode number `op` on the u32 operands b and c (rs2's value, the sign-extended immediate or the shift amount)."""
+    sb, sc, sh = b - ((b >> 31) << 32), c - ((c >> 31) << 32), c & 31
+    r = {"ADD": b + c, "SUB": b - c, "SLL": b << sh, "SLT": int(sb < sc), "SLTU": int(b < c), "XOR": b ^ c, "SRL": b >> sh, "SRA": sb >> sh,
+         "OR": b | c, "AND": b & c}[R_TWIN[op]]
+    return r & 0xFFFFFFFF
+
+
 def execute(ops, base=ELF_TEXT_START):
-    """Run a straight-line ADD / ADDI program once from the all-zero register file.  Returns (steps, final registers) where steps is
+    """Run a straight-line program of the 19 opcodes once from the all-zero register file.  Returns (steps, final registers) where steps is
     (len(STEP_FIELDS), n_steps) uint32 in STEP_FIELDS order and final registers = (values, timestamps) of the 32 registers after the last
     step (FinalReg's rows).  Step t (clk = t + 1) reads rs1 at 3 clk + 1, rs2 at 3 clk + 2 and writes rd at 3 clk + 3 (preprocessed.rs:75-100);
     a write to x0 stores 0 (ValueAEffective)."""
     val, ts = [0] * NUM_REGISTERS, [0] * NUM_REGISTERS
     pc_ctr = {}
     cols = [[] for _ in STEP_FIELDS]
-    words = [encode_add(rd, rs1, c) if op == OP_ADD else encode_addi(rd, rs1, c) for op, rd, rs1, c in ops]
-    for t, ((op, rd, rs1, c), word) in enumerate(zip(ops, words)):
-        assert op in (OP_ADD, OP_ADDI) and 0 <= rd < 32 and 0 <= rs1 < 32
+    for t, (op, rd, rs1, c) in enumerate(ops):
+        assert 0 <= op < len(OPCODES) and 0 <= rd < 32 and 0 <= rs1 < 32
+        word = encode(op, rd, rs1, c)
         clk = t + 1
         pc = base + 4 * t
         b, ts1 = val[rs1], ts[rs1]
         ts[rs1] = 3 * clk + 1
-        if op == OP_ADD:
+        if OP_TYPE[op] == "R":
             assert 0 <= c < 32
             cv, ts2 = val[c], ts[c]
             ts[c] = 3 * clk + 2
             op_c = c
-        else:
-            op_c = (c & 0xFFF) - ((c & 0x800) << 1) & 0xFFFFFFFF        # the 12-bit immediate, sign-extended
+        elif OP_TYPE[op] == "I":
+            op_c = (c & 0xFFF) - ((c & 0x800) << 1) & 0xFFFFFFFF                # the 12-bit immediate, sign-extended
             cv, ts2 = op_c, 0
-        a = (b + cv) & 0xFFFFFFFF
+        else:
+            assert 0 <= c < 32
+            op_c = cv = c
+            ts2 = 0
+        a = alu(op, b, cv)
         rd_prev, ts3 = val[rd], ts[rd]
         val[rd], ts[rd] = (a if rd else 0), 3 * clk + 3
         ctr = pc_ctr.get(pc, 0)
@@ -105,6 +243,27 @@ def _carries16(x, y):
     return [c0.astype(np.uint32), c1.astype(np.uint32)]
 
 
+def _borrows16(x, y):
+    """The borrows out of the low and the high 16 bits of x - y (subtract_with_borrow's limbs 1 and 3, sub.rs:26-63)."""
+    x, y = np.asarray(x, np.uint64), np.asarray(y, np.uint64)
+    return [((x & 0xFFFF) < (y & 0xFFFF)).astype(np.uint32), (x < y).astype(np.uint32)]
+
+
+def _signed(x):
+    x = np.asarray(x, np.uint64).astype(np.int64)
+    return x - ((x >> 31) << 32)
+
+
+def alu_np(op, b, c):
+    """`alu` over arrays: the u32 results of the opcode numbers `op` on the operands b and c."""
+    b, c = np.asarray(b, np.uint64), np.asarray(c, np.uint64)
+    sh = c & np.uint64(31)
+    sb, sc = _signed(b), _signed(c)
+    by_name = {"ADD": b + c, "SUB": b - c, "SLL": b << sh, "SLT": (sb < sc).astype(np.uint64), "SLTU": (b < c).astype(np.uint64),
+               "XOR": b ^ c, "SRL": b >> sh, "SRA": (sb >> sh.astype(np.int64)).astype(np.uint64), "OR": b | c, "AND": b & c}
+    return np.select([op == k for k in range(len(OPCODES))], [by_name[n] for n in R_TWIN], 0) & np.uint64(0xFFFFFFFF)
+
+
 def main_columns(steps, final_ctr, log_size):
     """The main component's 347 columns in trace order ({column name: its limbs}) for the step record `steps` (rows past n_steps are padding
     rows) and the final access counters of the program's rows (FinalPrgMemoryCtr)."""
@@ -118,9 +277,17 @@ def main_columns(steps, final_ctr, log_size):
         for dst, v in zip(t[name], limbs):
             dst[rows] = v
 
-    is_add, is_addi = s["opcode"] == OP_ADD, s["opcode"] == OP_ADDI
-    rd, rs1 = s["rd"], s["rs1"]
-    a = (s["value_b"] + s["value_c"]) & np.uint64(0xFFFFFFFF)
+    def put_on(ops, name, limbs):
+        """Write `limbs` (arrays over the steps) on the steps whose opcode is in `ops` only."""
+        rows = np.nonzero(np.isin(op, ops))[0]
+        for dst, v in zip(t[name], limbs):
+            dst[rows] = np.broadcast_to(np.asarray(v, np.uint64), (m,))[rows]
+
+    op = s["opcode"]
+    ty = np.array(OP_TYPE)[op.astype(np.int64)]
+    is_r, is_i, is_shift = ty == "R", ty == "I", ty == "IShift"
+    rd, rs1, b, c = s["rd"], s["rs1"], s["value_b"], s["value_c"]
+    a = alu_np(op, b, c)
     flag = (rd != 0).astype(np.uint32)
     # CpuChip (cpu.rs:36-316)
     put("IsPadding", [np.zeros(m, np.uint32)])
@@ -135,28 +302,61 @@ def main_columns(steps, final_ctr, log_size):
     put("PcCarry", _carries16(s["pc"], 4))
     put("PcNext", _le(s["pc"] + 4))
     put("InstrVal", _le(s["word"]))
-    put("IsAdd", [np.ones(m, np.uint32)])
-    put("ValueB", _le(s["value_b"]))
-    put("ValueC", _le(s["value_c"]))
+    for name in dict.fromkeys(f for _n, _ty, _f3, _f7, f in OPCODES):
+        put(name, [np.isin(op, [k for k, o in enumerate(OPCODES) if o[4] == name]).astype(np.uint32)])
+    put("ValueB", _le(b))
+    put("ValueC", _le(c))
     put("OpA", [rd])
     put("OpB", [rs1])
-    put("OpC", [np.where(is_add, s["op_c"], s["op_c"] & 0xFFF)])
-    put("ImmC", [is_addi.astype(np.uint32)])
+    put("OpC", [np.where(is_i, s["op_c"] & 0xFFF, s["op_c"])])
+    put("ImmC", [(~is_r).astype(np.uint32)])
     put("Reg1Address", [rs1])
-    put("Reg2Address", [np.where(is_add, s["op_c"], 0)])
+    put("Reg2Address", [np.where(is_r, s["op_c"], 0)])
     put("Reg3Address", [rd])
-    # DecodingCheck, types R (ADD) and I (ADDI): type_r.rs:43-59, type_i.rs:46-68
-    c = s["op_c"]
+    # DecodingCheck, types R, I without and I with a shift amount: type_r.rs:43-59, type_i.rs:46-68 and 288-330
+    oc = s["op_c"]
     put("OpA0", [rd & 1]); put("OpA1_4", [(rd >> 1) & 0xF])
     put("OpB0", [rs1 & 1]); put("OpB1_4", [(rs1 >> 1) & 0xF])
-    put("OpC0_3", [c & 0xF])
-    put("OpC4", [np.where(is_add, (c >> 4) & 1, 0)])
-    put("OpC4_7", [np.where(is_addi, (c >> 4) & 0xF, 0)])
-    put("OpC8_10", [np.where(is_addi, (c >> 8) & 0x7, 0)])
-    put("OpC11", [np.where(is_addi, (c >> 11) & 1, 0)])
-    # AddChip (add.rs:64-100)
+    put("OpC0_3", [oc & 0xF])
+    put("OpC4", [np.where(is_i, 0, (oc >> 4) & 1)])
+    put("OpC4_7", [np.where(is_i, (oc >> 4) & 0xF, 0)])
+    put("OpC8_10", [np.where(is_i, (oc >> 8) & 0x7, 0)])
+    put("OpC11", [np.where(is_i, (oc >> 11) & 1, 0)])
+    # the instruction chips: ValueA = the result, and each chip's helpers on its own rows
     put("ValueA", _le(a))
-    put("CarryFlag", _carries16(s["value_b"], s["value_c"]))
+    put_on([OP_ADD, OP_ADDI], "CarryFlag", _carries16(b, c))                        # AddChip (add.rs:64-100)
+    slt, sltu = [OP_SLT, OP_SLTI], [OP_SLTU, OP_SLTIU]
+    put_on([OP_SUB] + slt + sltu, "CarryFlag", _borrows16(b, c))                     # SubChip (sub.rs:66-100), and CarryFlag as the borrows
+    put_on(slt + sltu, "Helper1", _le((b - c) & 0xFFFFFFFF))                         # SltuChip (sltu.rs:45-75), SltChip (slt.rs:56-110)
+    put_on(slt, "Helper2", _le(b & 0x7FFFFFFF))
+    put_on(slt, "Helper3", _le(c & 0x7FFFFFFF))
+    put_on(slt, "SgnC", [c >> 31])
+    bit_ops = [OP_XOR, OP_OR, OP_AND, OP_XORI, OP_ORI, OP_ANDI]                      # BitOpChip (bit_op.rs:249-300): the high nibbles
+    for name, v in (("ValueA4_7", a), ("ValueB4_7", b), ("ValueC4_7", c)):
+        put_on(bit_ops, name, [x >> 4 for x in _le(v)])
+    # SllChip, SrlChip, SraChip (sll.rs:72-112, srl.rs:79-119, sra.rs:93-139): the shift amount's bits from ValueC's low byte, Exp1_3 = 2^(its
+    # low three bits); SLL multiplies ValueB by Exp1_3 byte by byte (Rem, carries Qt), SRL / SRA divide it from the top byte (quotients Qt
+    # = the bytes of b >> those bits, remainders Rem)
+    sll, srl, sra = [OP_SLL, OP_SLLI], [OP_SRL, OP_SRLI], [OP_SRA, OP_SRAI]
+    c0 = c & 0xFF
+    e = np.uint64(1) << (c0 & 7)
+    put_on(sll + srl + sra, "Helper1", [c0 >> 5, 0, 0, 0])
+    for k in range(5):
+        put_on(sll + srl + sra, f"ShiftBit{k + 1}", [(c0 >> k) & 1])
+    put_on(sll + srl + sra, "Exp1_3", [e])
+    put_on(sll, "Rem", _le((b * e) & 0xFFFFFFFF))
+    put_on(sll, "Qt", [((b & ((1 << (8 * i + 8)) - 1)) * e) >> (8 * i + 8) for i in range(4)])
+    rem = [x & (e - 1) for x in _le(b)]
+    put_on(srl + sra, "Rem", rem)
+    put_on(srl + sra, "Qt", _le(b >> (c0 & 7)))
+    put_on(srl + sra, "RemDiff", [e - 1 - r for r in rem])
+    sgn_b = b >> 31
+    exp = np.uint64(256) // e
+    put_on(sra, "Helper2", [(b >> 24) & 0x7F, 0, 0, 0])
+    put_on(sra, "Helper3", _le(b >> (c & 31)))
+    put_on(slt + sra, "SgnB", [sgn_b])
+    put_on(sra, "Exp", [exp])
+    put_on(sra, "SraDegreeAux", [sgn_b * (e - 1) * exp])
     # ProgramMemCheck (program_mem_check.rs:44-100): the counters of this access; FinalPrgMemoryCtr on the program's rows
     put("ProgCtrPrev", _le(s["pc_ctr_prev"]))
     put("ProgCtrCur", _le(s["pc_ctr_prev"] + 1))
@@ -164,8 +364,8 @@ def main_columns(steps, final_ctr, log_size):
     put("FinalPrgMemoryCtr", _le(final_ctr), slice(0, len(final_ctr)))
     # RegisterMemCheck (register_mem_check.rs:53-117): ValueAEffective and the previous values / timestamps of the accessed registers
     put("ValueAEffective", _le(a * flag))
-    put("Reg1ValPrev", _le(s["value_b"]))
-    put("Reg2ValPrev", _le(np.where(is_add, s["value_c"], 0)))
+    put("Reg1ValPrev", _le(b))
+    put("Reg2ValPrev", _le(np.where(is_r, c, 0)))
     put("Reg3ValPrev", _le(s["rd_prev"]))
     for k in (1, 2, 3):
         put(f"Reg{k}TsPrev", _le(s[f"ts{k}_prev"]))
@@ -183,16 +383,24 @@ def main_columns(steps, final_ctr, log_size):
     return t
 
 
-def _count(hist, values):
-    hist += np.bincount(np.asarray(values, np.int64), minlength=hist.size)
+def _count(hist, values, weights=None):
+    """Add each value to the histogram, with its numerator when `weights` are given (rows of numerator 0 look nothing up)."""
+    v = np.asarray(values, np.int64)
+    if weights is None:
+        hist += np.bincount(v, minlength=hist.size)
+    else:
+        keep = weights != 0
+        hist += np.bincount(v[keep], weights[keep], minlength=hist.size).astype(np.int64)
 
 
 def table_counts(t, ram_cols):
-    """The multiplicities of Range8, 16, 32, 128, 256 as the main component's lookups (nexus_v1.record_main_component's range checks, their
-    numerators on ADD, ADDI and padding rows) and RamInitFinal's nine Range256 lookups per row count them."""
+    """The multiplicities of BitOp (And, Or, Xor: one per row b nibble * 16 + c nibble), Range8, 16, 32, 128, 256 as the main component's
+    lookups (nexus_v1.record_main_component's bit-op lookups and range checks with their numerators) and RamInitFinal's nine Range256
+    lookups per row count them."""
     h = {r: np.zeros(length, np.int64) for r, length, _ls in W.MULTIPLICITY_TABLES}
-    is_add = (t["IsAdd"][0] == 1) & (t["ImmC"][0] == 0)
-    is_addi = (t["IsAdd"][0] == 1) & (t["ImmC"][0] == 1)
+    f = lambda *names: sum(t[nm][0].astype(np.int64) for nm in names)
+    imm_c = f("ImmC")
+    vtype = {"R": (1 - imm_c) * f(*V.TYPE_R_OPS), "INoShift": imm_c * f(*V.ALU_IMM_NO_SHIFT), "IShift": imm_c * f(*V.ALU_IMM_SHIFT)}
     for w in V.R256_WORDS + V.R256_HALF_WORDS + V.R256_BYTES:
         for limb in t[w]:
             _count(h["Range256"], limb)
@@ -200,32 +408,43 @@ def table_counts(t, ram_cols):
         _count(h["Range256"], v)
     for w in V.R32:
         _count(h["Range32"], t[w][0])
-    vtype = {"R": is_add, "INoShift": is_addi}
     for ty, names in V.R16:
         for nm in names:
             if ty in vtype:
-                _count(h["Range16"], t[nm][0][vtype[ty]])
+                _count(h["Range16"], t[nm][0], vtype[ty])
     for ty, names in V.R8:
         for nm in names:
             if ty in vtype:
-                _count(h["Range8"], t[nm][0][vtype[ty]])
+                _count(h["Range8"], t[nm][0], vtype[ty])
+    _count(h["Range8"], t["Helper1"][0], f(*V.ALU_IMM_SHIFT))
+    for nm in ("Helper2", "Helper3"):
+        _count(h["Range128"], t[nm][3], f("IsSlt"))
+    _count(h["Range128"], t["Helper2"][0], f("IsSra"))
+    h["BitOp"] = [np.zeros(256, np.int64) for _ in range(3)]
+    for hist, flag in zip(h["BitOp"], ("IsAnd", "IsOr", "IsXor")):
+        for k in range(4):
+            b_hi, c_hi = t["ValueB4_7"][k].astype(np.int64), t["ValueC4_7"][k].astype(np.int64)
+            b_lo, c_lo = t["ValueB"][k] - 16 * b_hi, t["ValueC"][k] - 16 * c_hi
+            _count(hist, b_lo * 16 + c_lo, f(flag))
+            _count(hist, b_hi * 16 + c_hi, f(flag))
     return h
 
 
 class AddChainMachine:
     """The ADD chain of the module docstring at 2^log_size rows, `n_steps` executed steps (default 2^log_size); `ops` = [(opcode, rd, rs1,
-    rs2 or imm)] runs another straight-line ADD / ADDI program instead.  Same interface as the other
+    rs2 or imm)] runs another straight-line program instead.  Same interface as the other
     machines: `air`, `words`, `relations`, `log_sizes`, `preprocessed_columns()`, `fill_main_trace()` (tree 1 in commitment order, the
     multiplicity columns counted on the host), `column_log_sizes()`, and `device_trees(ctx)` (the main trace filled on the device by
     nb200_v1_main_trace, the multiplicities counted there)."""
+    ALU = False                                          # record_main_component's `alu`: the machine constrains SLT, SLTU and the shifts
 
     def __init__(self, log_size, n_steps=None, ops=None):
         assert log_size >= 8
         self.log_size = self.log_size_main = log_size
         if ops is None:
             self.n_steps = (1 << log_size) if n_steps is None else int(n_steps)
-            self.program, ops = add_chain_program(log_size, self.n_steps)
-        else:                                                                 # another straight-line ADD / ADDI program
+            self.program, ops = self.default_program(log_size, self.n_steps)
+        else:                                                                 # another straight-line program
             self.n_steps = len(ops)
         assert 1 <= self.n_steps <= 1 << log_size
         self.steps, (self.final_values, self.final_timestamps) = execute(ops)
@@ -238,7 +457,7 @@ class AddChainMachine:
                  ("Range128", 1), ("Range256", 1)]
         self.relations = [air.relation(n, s) for n, s in names]
         rel = {r.name: r for r in self.relations}
-        self.main, _col = V.record_main_component(air, log_size, rel, decoding=True)
+        self.main, _col = V.record_main_component(air, log_size, rel, decoding=True, alu=self.ALU)
         self.final_reg = W._final_reg_component(air, rel["RegisterCheck"])
         self.bit_op = W._bit_op_component(air, rel["BitOp"])
         self.ram = W._ram_init_final_component(air, self.ram_log_size, rel["LoadStore"], rel["Range256"])
@@ -247,6 +466,13 @@ class AddChainMachine:
         self.log_sizes = [log_size, W.FINAL_REG_LOG_SIZE, W.BIT_OP_LOG_SIZE, self.ram_log_size] + [ls for _r, _l, ls in W.MULTIPLICITY_TABLES]
         self.words = air.serialize()
         self._main = None
+
+    def default_program(self, log_size, n_steps):
+        return add_chain_program(log_size, n_steps)
+
+    def device_fill(self, ctx, out=None):
+        """The main component's 347 columns filled on the device from the step record (nb200_v1_main_trace)."""
+        return ctx.v1_main_trace(self.steps, self.final_ctr, self.log_size, out=out)
 
     # ---- tree 0
     def program_columns(self):
@@ -303,7 +529,7 @@ class AddChainMachine:
             h = table_counts(t, ram)
             cols = [limb for name, _ in V.MAIN_COLUMNS for limb in t[name]]
             cols += self.final_reg_columns()
-            cols += [np.zeros(1 << W.BIT_OP_LOG_SIZE, np.uint32) for _ in range(3)]
+            cols += [(v % P).astype(np.uint32) for v in h["BitOp"]]
             cols += list(ram)
             for r, length, ls in W.MULTIPLICITY_TABLES:
                 v = np.zeros(1 << ls, np.int64)
@@ -318,9 +544,9 @@ class AddChainMachine:
 
     def device_trees(self, ctx, out=None):
         """(tree-0 device batches, tree-1 device batches), finalized order, for machine.prove(..., resident=...): tree 0 and FinalReg's
-        columns uploaded, the main component filled on the device from the step record (nb200_v1_main_trace; `out` = a batch of 347 columns
-        of 2^log_size rows to reuse), RamInitFinal and BitOpMultiplicity zero, and every table column counted on the device from the filled
-        trace (nb200_table_multiplicities_first_row)."""
+        columns uploaded, the main component filled on the device from the step record (device_fill; `out` = a batch of 347 columns of
+        2^log_size rows to reuse), RamInitFinal zero, and every table column (BitOpMultiplicity's among them) counted on the device from the
+        filled trace (nb200_table_multiplicities_first_row)."""
         from .machine import fill_table_multiplicities
 
         def upload_runs(cols):
@@ -334,7 +560,7 @@ class AddChainMachine:
             return res
 
         tree0 = upload_runs(self.preprocessed_columns())
-        tree1 = [ctx.v1_main_trace(self.steps, self.final_ctr, self.log_size, out=out)]
+        tree1 = [self.device_fill(ctx, out=out)]
         tree1 += upload_runs(self.final_reg_columns())
         tree1.append(ctx.alloc(3, W.BIT_OP_LOG_SIZE))
         ram = ctx.alloc(W.RAM_COLS, self.ram_log_size)
@@ -349,3 +575,23 @@ class AddChainMachine:
             i = j
         fill_table_multiplicities(self, ctx, tree0, tree1, first_row=True)
         return tree0, tree1
+
+
+class AluMachine(AddChainMachine):
+    """A straight-line program over every RV32I register-register and register-immediate instruction but LUI / AUIPC (OPCODES) at
+    2^log_size rows: alu_program(log_size, n_steps, seed) by default (n_steps defaults to 2^log_size), or `ops` = [(opcode, rd, rs1, rs2 /
+    imm / shift amount)].  AddChainMachine's components, relations, draw order and interface, with the main component recorded with
+    `alu=True` (SltuChip, SltChip, SllChip, SrlChip and SraChip constrained) and filled on the device by nb200_v1_alu_trace.  Its bit-op
+    lookups make BitOpMultiplicity nonzero."""
+    ALU = True
+
+    def __init__(self, log_size, n_steps=None, ops=None, seed=0):
+        self.seed = seed
+        super().__init__(log_size, n_steps, ops)
+
+    def default_program(self, log_size, n_steps):
+        return alu_program(log_size, n_steps, self.seed)
+
+    def device_fill(self, ctx, out=None):
+        """The main component's 347 columns filled on the device from the step record (nb200_v1_alu_trace)."""
+        return ctx.v1_alu_trace(self.steps, self.final_ctr, self.log_size, out=out)

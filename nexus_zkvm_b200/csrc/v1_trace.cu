@@ -1,7 +1,8 @@
-// The v1 main component's main trace filled on the device from an ADD / ADDI program's step record (nb200_v1_main_trace): what
-// add_chain.AddChainMachine.fill_main_trace() builds for the main component on the host, followed by finalize_columns, without the host
-// columns or their upload.  The batch is cleared first (the columns no ADD, ADDI or padding row sets stay zero); then one thread per
-// finalized row position writes its row's other columns (v1_trace.cuh), so consecutive threads write consecutive words of every column.
+// The v1 main component's main trace filled on the device from a program's step record (nb200_v1_main_trace for ADD / ADDI programs,
+// nb200_v1_alu_trace for the 19 ALU opcodes; one kernel behind two host checks): what add_chain.main_columns builds for the main
+// component on the host, followed by finalize_columns, without the host columns or their upload.  The batch is cleared first (the columns
+// no executed or padding row sets stay zero); then one thread per finalized row position writes its row's other columns (v1_trace.cuh),
+// so consecutive threads write consecutive words of every column.
 #include "common.cuh"
 #include "v1_trace.cuh"
 #include <algorithm>
@@ -19,27 +20,35 @@ __global__ void __launch_bounds__(V1_BLOCK) v1_main_trace_kernel(const u32* __re
   v1::main_row(steps, n_steps, final_ctr, n_prog, log_size, i, out + i, (size_t)1 << log_size);
 }
 
-}  // namespace
-
-nb200_status v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
-                           nb200_cols* out) {
-  NB_ARG(ctx, out && (n_steps == 0 || steps) && (n_prog == 0 || final_ctr), "v1_main_trace: null argument");
-  NB_ARG(ctx, log_size >= 4 && log_size <= 28, "v1_main_trace: log_size must be in [4, 28]");
-  NB_ARG(ctx, out->n_cols == v1::MAIN_COLS && out->log_size == log_size, "v1_main_trace: out must be a batch of 347 columns of 2^log_size rows");
+// The host check of a step record and the fill.  `alu`: the 19 opcodes of nb200_v1_alu_trace, with their operand ranges; otherwise ADD and
+// ADDI only, as nb200_v1_main_trace has always taken them.
+nb200_status v1_fill(nb200_ctx* ctx, const char* who, bool alu, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr,
+                     uint32_t log_size, nb200_cols* out) {
+  const std::string me = who;
+  NB_ARG(ctx, out && (n_steps == 0 || steps) && (n_prog == 0 || final_ctr), me + ": null argument");
+  NB_ARG(ctx, log_size >= 4 && log_size <= 28, me + ": log_size must be in [4, 28]");
+  NB_ARG(ctx, out->n_cols == v1::MAIN_COLS && out->log_size == log_size, me + ": out must be a batch of 347 columns of 2^log_size rows");
   const size_t n = (size_t)1 << log_size;
-  NB_ARG(ctx, n_steps <= n, "v1_main_trace: more steps than 2^log_size rows");
-  NB_ARG(ctx, n_prog <= n, "v1_main_trace: more program rows than 2^log_size rows");
+  NB_ARG(ctx, n_steps <= n, me + ": more steps than 2^log_size rows");
+  NB_ARG(ctx, n_prog <= n, me + ": more program rows than 2^log_size rows");
   auto f = [&](u32 field, size_t t) { return steps[field * n_steps + t]; };
   for (size_t t = 0; t < n_steps; ++t) {
-    const u32 op = f(v1::OPCODE, t);
-    NB_ARG(ctx, op == v1::OP_ADD || op == v1::OP_ADDI, "v1_main_trace: step " + std::to_string(t) + " is not ADD or ADDI");
-    NB_ARG(ctx, f(v1::RD, t) < 32 && f(v1::RS1, t) < 32 && (op != v1::OP_ADD || f(v1::OP_C, t) < 32),
-           "v1_main_trace: step " + std::to_string(t) + " has a register index above 31");
+    const u32 op = f(v1::OPCODE, t), op_c = f(v1::OP_C, t);
+    if (alu) {
+      NB_ARG(ctx, op < v1::N_OPCODES, me + ": step " + std::to_string(t) + " has an opcode above 18");
+      NB_ARG(ctx, !v1::is_type_i_shift(op) || op_c < 32, me + ": step " + std::to_string(t) + " has a shift amount above 31");
+      NB_ARG(ctx, !v1::is_type_i(op) || op_c + 2048u < 4096u,
+             me + ": step " + std::to_string(t) + " has an immediate that is not a sign-extended 12-bit value");
+    } else {
+      NB_ARG(ctx, op == v1::OP_ADD || op == v1::OP_ADDI, me + ": step " + std::to_string(t) + " is not ADD or ADDI");
+    }
+    NB_ARG(ctx, f(v1::RD, t) < 32 && f(v1::RS1, t) < 32 && (!v1::is_type_r(op) || op_c < 32),
+           me + ": step " + std::to_string(t) + " has a register index above 31");
     const u64 clk = t + 1;
     for (u32 k = 0; k < 3; ++k)
       NB_ARG(ctx, f(v1::TS1_PREV + k, t) < 3 * clk + k + 1,
-             "v1_main_trace: step " + std::to_string(t) + " has a previous timestamp not below the current one");
-    NB_ARG(ctx, f(v1::PC_CTR_PREV, t) != 0xFFFFFFFFu, "v1_main_trace: a program counter of 2^32 - 1 has no successor");
+             me + ": step " + std::to_string(t) + " has a previous timestamp not below the current one");
+    NB_ARG(ctx, f(v1::PC_CTR_PREV, t) != 0xFFFFFFFFu, me + ": a program counter of 2^32 - 1 has no successor");
   }
   // scratch, freed in stream order when the call returns: the step record and the final counters
   DevBuf d_steps, d_ctr;
@@ -53,6 +62,18 @@ nb200_status v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps
                                                                                           out->d);
   NB_LAUNCH_CHECK(ctx);
   return NB200_OK;
+}
+
+}  // namespace
+
+nb200_status v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                           nb200_cols* out) {
+  return v1_fill(ctx, "v1_main_trace", false, n_steps, steps, n_prog, final_ctr, log_size, out);
+}
+
+nb200_status v1_alu_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                          nb200_cols* out) {
+  return v1_fill(ctx, "v1_alu_trace", true, n_steps, steps, n_prog, final_ctr, log_size, out);
 }
 
 }  // namespace nb

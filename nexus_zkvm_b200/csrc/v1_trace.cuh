@@ -1,9 +1,12 @@
-// One row of the v1 main component's main trace (347 columns, prover/src/column.rs) for an ADD / ADDI program, filled from its step
-// record (add_chain.STEP_FIELDS): the per-row fills of CpuChip (chips/cpu.rs:36-316), DecodingCheck types R and I (decoding/type_r.rs:25-60,
-// type_i.rs:29-69), AddChip (instructions/i/add.rs:64-100), ProgramMemCheck (memory_check/program_mem_check.rs:44-100), RegisterMemCheck
-// (register_mem_check.rs:53-117) and Timestamp (timestamp.rs:33-75), or the reference's padding row past the last step.
-// The same code runs in v1_main_trace_kernel (v1_trace.cu) and, compiled as host C++, in tests/test_add_chain_cpu.py, which compares every
-// row with AddChainMachine.fill_main_trace().  Rows are addressed by their finalized position (finalize_order.cuh).
+// One row of the v1 main component's main trace (347 columns, prover/src/column.rs) for a straight-line program of RV32I's ALU
+// instructions (ADD ... SRAI, add_chain.OPCODES), filled from its step record (add_chain.STEP_FIELDS): the per-row fills of CpuChip
+// (chips/cpu.rs:36-316), DecodingCheck types R, I and I with a shift amount (decoding/type_r.rs:25-60, type_i.rs:29-69,288-330), AddChip,
+// SubChip, SltuChip, BitOpChip, SltChip, SllChip, SrlChip and SraChip (instructions/i/add.rs:64-100, sub.rs:66-100, sltu.rs:45-75,
+// bit_op.rs:249-300, slt.rs:56-110, sll.rs:72-112, srl.rs:79-119, sra.rs:93-139), ProgramMemCheck (memory_check/program_mem_check.rs:44-100),
+// RegisterMemCheck (register_mem_check.rs:53-117) and Timestamp (timestamp.rs:33-75), or the reference's padding row past the last step.
+// The same code runs in v1_main_trace_kernel (v1_trace.cu) and, compiled as host C++, in tests/test_add_chain_cpu.py and
+// tests/test_alu_program_cpu.py, which compare every row with add_chain.main_columns.  Rows are addressed by their finalized position
+// (finalize_order.cuh).
 #pragma once
 #include "m31.cuh"
 #include "finalize_order.cuh"
@@ -14,7 +17,27 @@ namespace v1 {
 constexpr u32 MAIN_COLS = 347;
 // the step record, one array of n_steps words per field (include/nb200.h, nb200_v1_main_trace)
 enum StepField : u32 { PC, WORD, OPCODE, RD, RS1, OP_C, VALUE_B, VALUE_C, RD_PREV, TS1_PREV, TS2_PREV, TS3_PREV, PC_CTR_PREV, STEP_FIELDS };
-constexpr u32 OP_ADD = 0, OP_ADDI = 1;
+// opcode numbers of the step record (include/nb200.h): type R, type I, type I with a shift amount
+enum Opcode : u32 { OP_ADD, OP_ADDI, OP_SUB, OP_SLL, OP_SLT, OP_SLTU, OP_XOR, OP_SRL, OP_SRA, OP_OR, OP_AND, OP_SLTI, OP_SLTIU, OP_XORI, OP_ORI,
+                    OP_ANDI, OP_SLLI, OP_SRLI, OP_SRAI, N_OPCODES };
+NB_HD bool is_type_r(u32 op) { return op == OP_ADD || (op >= OP_SUB && op <= OP_AND); }
+NB_HD bool is_type_i(u32 op) { return op == OP_ADDI || (op >= OP_SLTI && op <= OP_ANDI); }
+NB_HD bool is_type_i_shift(u32 op) { return op >= OP_SLLI && op <= OP_SRAI; }
+// the register-register instruction an opcode computes (SLTIU: SLTU)
+NB_HD u32 base_op(u32 op) {
+  switch (op) {
+    case OP_ADDI: return OP_ADD;
+    case OP_SLTI: return OP_SLT;
+    case OP_SLTIU: return OP_SLTU;
+    case OP_XORI: return OP_XOR;
+    case OP_ORI: return OP_OR;
+    case OP_ANDI: return OP_AND;
+    case OP_SLLI: return OP_SLL;
+    case OP_SRLI: return OP_SRL;
+    case OP_SRAI: return OP_SRA;
+    default: return op;
+  }
+}
 
 // first column of each word this fill writes (MAIN_COLUMNS order, nexus_v1.py; tests/test_add_chain_cpu.py checks them against it).
 // Every other column is zero on ADD, ADDI and padding rows.
@@ -25,6 +48,10 @@ constexpr u32 Pc = 0, PcNext = 4, OpA = 12, OpB = 13, OpC = 14, CarryFlag = 15, 
               Reg3ValPrev = 220, Reg1TsPrev = 224, ProgCtrPrev = 236, ProgCtrCur = 240, ProgCtrCarry = 244, FinalPrgMemoryCtr = 246,
               CReg1TsPrev = 250, CH1Minus = 262, OpC0_3 = 312, OpC4_7 = 315, OpC8_10 = 317, OpC11 = 318, OpA1_4 = 321, OpB1_4 = 323,
               OpC4 = 325, OpA0 = 326, OpB0 = 327, PcCarry = 333;
+// the instruction chips' columns beyond the ADD chain's
+constexpr u32 IsOr = 45, IsAnd = 46, IsXor = 47, IsSub = 48, IsSltu = 49, IsSlt = 50, IsSll = 69, IsSrl = 70, IsSra = 71, Helper1 = 91,
+              Helper2 = 95, Helper3 = 99, SgnB = 108, SgnC = 109, Rem = 115, Qt = 120, ShiftBit1 = 124, Exp1_3 = 129, Exp = 130, RemDiff = 131,
+              SraDegreeAux = 139, ValueA4_7 = 335, ValueB4_7 = 339, ValueC4_7 = 343;
 }  // namespace col
 
 // carries out of the low and high 16 bits of x + y (limbs 1 and 3 of add_with_carries, add.rs:27-45)
@@ -32,6 +59,22 @@ NB_HD void carries16(u32 x, u32 y, u32& c0, u32& c1) {
   const u32 lo = (x & 0xFFFFu) + (y & 0xFFFFu);
   c0 = lo >> 16;
   c1 = ((x >> 16) + (y >> 16) + c0) >> 16;
+}
+
+// RV32I's result of the register-register instruction `base` on b and c (rs2's value, the immediate or the shift amount)
+NB_HD u32 alu_result(u32 base, u32 b, u32 c) {
+  switch (base) {
+    case OP_SUB: return b - c;
+    case OP_SLL: return b << (c & 31);
+    case OP_SLT: return (int32_t)b < (int32_t)c ? 1u : 0u;
+    case OP_SLTU: return b < c ? 1u : 0u;
+    case OP_XOR: return b ^ c;
+    case OP_SRL: return b >> (c & 31);
+    case OP_SRA: return (u32)((int32_t)b >> (c & 31));
+    case OP_OR: return b | c;
+    case OP_AND: return b & c;
+    default: return b + c;
+  }
 }
 
 // Row at finalized position i of 2^log_size rows into out[c * stride]: trace row r = finalized_src_row(i) is step r when r < n_steps and a
@@ -48,12 +91,12 @@ NB_HD void main_row(const u32* steps, u32 n_steps, const u32* final_ctr, u32 n_p
   auto field = [&](u32 f) { return exec ? steps[(size_t)f * n_steps + r] : 0u; };
   const u32 pc = field(PC), word = field(WORD), rd = field(RD), rs1 = field(RS1), op_c = field(OP_C);
   const u32 b = field(VALUE_B), c = field(VALUE_C);
-  const bool is_add = exec && field(OPCODE) == OP_ADD, is_addi = exec && field(OPCODE) == OP_ADDI;
+  const u32 op = field(OPCODE), base = base_op(op);
+  const bool is_r = exec && is_type_r(op), is_i = exec && is_type_i(op), is_shift = exec && is_type_i_shift(op);
   u32 c0, c1;
   // CpuChip
   put(col::IsPadding, exec ? 0u : 1u);
-  put(col::IsAdd, exec ? 1u : 0u);
-  put(col::ImmC, is_addi ? 1u : 0u);
+  put(col::ImmC, is_i || is_shift ? 1u : 0u);
   put(col::ValueAEffectiveFlag, rd != 0);
   put(col::ValueAEffectiveFlagAux, rd ? m31_inv(rd) : 1u);
   put(col::ValueAEffectiveFlagAuxInv, rd ? rd : 1u);
@@ -67,26 +110,69 @@ NB_HD void main_row(const u32* steps, u32 n_steps, const u32* final_ctr, u32 n_p
   put_word(col::ValueC, c);
   put(col::OpA, rd);
   put(col::OpB, rs1);
-  put(col::OpC, is_addi ? op_c & 0xFFFu : op_c);
+  put(col::OpC, is_i ? op_c & 0xFFFu : op_c);
   put(col::Reg1Address, rs1);
-  put(col::Reg2Address, is_add ? op_c : 0u);
+  put(col::Reg2Address, is_r ? op_c : 0u);
   put(col::Reg3Address, rd);
-  // DecodingCheck: type R (ADD) and type I without shift (ADDI)
+  // DecodingCheck: type R, type I without and with a shift amount
   put(col::OpA0, rd & 1);
   put(col::OpA1_4, (rd >> 1) & 0xF);
   put(col::OpB0, rs1 & 1);
   put(col::OpB1_4, (rs1 >> 1) & 0xF);
   put(col::OpC0_3, op_c & 0xF);
-  put(col::OpC4, is_add ? (op_c >> 4) & 1 : 0u);
-  put(col::OpC4_7, is_addi ? (op_c >> 4) & 0xF : 0u);
-  put(col::OpC8_10, is_addi ? (op_c >> 8) & 0x7 : 0u);
-  put(col::OpC11, is_addi ? (op_c >> 11) & 1 : 0u);
-  // AddChip
-  const u32 a = b + c;
+  put(col::OpC4, is_i ? 0u : (op_c >> 4) & 1);
+  put(col::OpC4_7, is_i ? (op_c >> 4) & 0xF : 0u);
+  put(col::OpC8_10, is_i ? (op_c >> 8) & 0x7 : 0u);
+  put(col::OpC11, is_i ? (op_c >> 11) & 1 : 0u);
+  // the instruction chips: ValueA is the result, and each chip's helpers, zero on the rows of other opcodes.  Every column is written by
+  // every thread, so a warp over rows of mixed opcodes still writes whole 128-byte lines instead of one partial store per opcode.
+  const u32 a = alu_result(base, b, c);
   put_word(col::ValueA, a);
-  carries16(b, c, c0, c1);
-  put(col::CarryFlag, c0);
-  put(col::CarryFlag + 1, c1);
+  const bool add = exec && base == OP_ADD, slt = exec && base == OP_SLT, sltx = slt || (exec && base == OP_SLTU);
+  const bool sub = sltx || (exec && base == OP_SUB), bit = exec && (base == OP_XOR || base == OP_OR || base == OP_AND);
+  const bool sll = exec && base == OP_SLL, sra = exec && base == OP_SRA, srx = sra || (exec && base == OP_SRL), shift = sll || srx;
+  carries16(b, c, c0, c1);                                                      // AddChip; SubChip, SltuChip, SltChip: the borrows
+  put(col::CarryFlag, add ? c0 : sub && (b & 0xFFFFu) < (c & 0xFFFFu) ? 1u : 0u);
+  put(col::CarryFlag + 1, add ? c1 : sub && b < c ? 1u : 0u);
+  // Helper1: b - c for SltuChip / SltChip, the shift amount's bits 5..7 for the shift chips; Helper2 / Helper3: SltChip's b and c without
+  // their sign bits, SraChip's top byte of b without it and the logical shift
+  const u32 s3 = c & 7, e = 1u << s3, sh = c & 31, sgn_b = b >> 31;
+  put_word(col::Helper1, sltx ? b - c : shift ? (c & 0xFFu) >> 5 : 0u);
+  put_word(col::Helper2, slt ? b & 0x7FFFFFFFu : sra ? (b >> 24) & 0x7Fu : 0u);
+  put_word(col::Helper3, slt ? c & 0x7FFFFFFFu : sra ? b >> sh : 0u);
+  put(col::SgnB, slt || sra ? sgn_b : 0u);
+  put(col::SgnC, slt ? c >> 31 : 0u);
+#pragma unroll
+  for (u32 k = 0; k < 4; ++k) {                                                 // BitOpChip: the high nibbles
+    put(col::ValueA4_7 + k, bit ? (a >> (8 * k + 4)) & 15u : 0u);
+    put(col::ValueB4_7 + k, bit ? (b >> (8 * k + 4)) & 15u : 0u);
+    put(col::ValueC4_7 + k, bit ? (c >> (8 * k + 4)) & 15u : 0u);
+  }
+  // SllChip, SrlChip, SraChip: Exp1_3 = 2^(low three bits of the amount); SLL multiplies b by it byte by byte (Rem, carries Qt), SRL / SRA
+  // divide b by it from the top byte (quotients Qt, remainders Rem, RemDiff = Exp1_3 - 1 - Rem); SRA's Exp = 2^8 / Exp1_3
+#pragma unroll
+  for (u32 k = 0; k < 5; ++k) put(col::ShiftBit1 + k, shift ? (c >> k) & 1 : 0u);
+  put(col::Exp1_3, shift ? e : 0u);
+#pragma unroll
+  for (u32 k = 0; k < 4; ++k) {
+    const u32 rem = (b >> (8 * k)) & (e - 1);
+    put(col::Rem + k, sll ? ((b << s3) >> (8 * k)) & 255u : srx ? rem : 0u);
+    put(col::Qt + k, sll ? (u32)(((u64)b >> (8 * k + 8 - s3)) & (e - 1)) : srx ? ((b >> s3) >> (8 * k)) & 255u : 0u);
+    put(col::RemDiff + k, srx ? e - 1 - rem : 0u);
+  }
+  put(col::Exp, sra ? 256u >> s3 : 0u);
+  put(col::SraDegreeAux, sra ? sgn_b * (e - 1) * (256u >> s3) : 0u);
+  // CpuChip's opcode flags
+  put(col::IsAdd, add);
+  put(col::IsSub, exec && base == OP_SUB);
+  put(col::IsSltu, exec && base == OP_SLTU);
+  put(col::IsSlt, slt);
+  put(col::IsXor, exec && base == OP_XOR);
+  put(col::IsOr, exec && base == OP_OR);
+  put(col::IsAnd, exec && base == OP_AND);
+  put(col::IsSll, sll);
+  put(col::IsSrl, exec && base == OP_SRL);
+  put(col::IsSra, sra);
   // ProgramMemCheck
   const u32 ctr = field(PC_CTR_PREV);
   put_word(col::ProgCtrPrev, ctr);
@@ -98,7 +184,7 @@ NB_HD void main_row(const u32* steps, u32 n_steps, const u32* final_ctr, u32 n_p
   // RegisterMemCheck
   put_word(col::ValueAEffective, rd ? a : 0u);
   put_word(col::Reg1ValPrev, b);
-  put_word(col::Reg2ValPrev, is_add ? c : 0u);
+  put_word(col::Reg2ValPrev, is_r ? c : 0u);
   put_word(col::Reg3ValPrev, field(RD_PREV));
   // Timestamp, every row: c = cur - 1 - prev against Reg{1,2,3}TsCur = 3 clk + {1,2,3}, the borrows out of the low and high 16 bits
   const u32 clk = r + 1;

@@ -212,13 +212,123 @@ def _record_decoding_r_i(m, c, col, is_type_r, is_load, alu_imm_no_shift, alu_im
         m.add_constraint(c(flag) * imm_c * (c4 + f7 * 2 - iv[3]))
 
 
-def record_main_component(air, log_size, rel, keccak=False, decoding=False):
+def _record_sltu(m, c, col):
+    """SltuChip (sltu.rs:79-131): a = b - c with CarryFlag as the two 16-bit borrows into Helper1, and ValueA = the high borrow."""
+    is_sltu, bf, vb, vc, va, h1 = c("IsSltu"), col["CarryFlag"], col["ValueB"], col["ValueC"], col["ValueA"], col["Helper1"]
+    m.add_constraint(is_sltu * (bf[1] - va[0]))
+    m.add_constraint(is_sltu * (h1[0] + h1[1] * 256 - bf[0] * 65536 - (vb[0] + vb[1] * 256 - vc[0] - vc[1] * 256)))
+    m.add_constraint(is_sltu * (h1[2] + h1[3] * 256 - bf[1] * 65536 - (vb[2] + vb[3] * 256 - vc[2] - vc[3] * 256 - bf[0])))
+    for k in (1, 2, 3):
+        m.add_constraint(is_sltu * va[k])
+
+
+def _record_slt(m, c, col):
+    """SltChip (slt.rs:118-199): the unsigned borrow as SLTU's, combined with the sign bits SgnB / SgnC split off ValueB / ValueC's top
+    bytes (their low seven bits in Helper2[3] / Helper3[3])."""
+    is_slt, bf, vb, vc, va, h1 = c("IsSlt"), col["CarryFlag"], col["ValueB"], col["ValueC"], col["ValueA"], col["Helper1"]
+    sgn_b, sgn_c = c("SgnB"), c("SgnC")
+    m.add_constraint(is_slt * (h1[0] + h1[1] * 256 - bf[0] * 65536 - (vb[0] + vb[1] * 256 - vc[0] - vc[1] * 256)))
+    m.add_constraint(is_slt * (h1[2] + h1[3] * 256 - bf[1] * 65536 - (vb[2] + vb[3] * 256 - vc[2] - vc[3] * 256 - bf[0])))
+    m.add_constraint(is_slt * (sgn_b * (1 - sgn_c) + bf[1] * (sgn_b * sgn_c + (1 - sgn_b) * (1 - sgn_c)) - va[0]))
+    for k in (1, 2, 3):
+        m.add_constraint(is_slt * va[k])
+    m.add_constraint(is_slt * (sgn_b * 128 + col["Helper2"][3] - vb[3]))
+    m.add_constraint(is_slt * (sgn_c * 128 + col["Helper3"][3] - vc[3]))
+
+
+def _shift_amount(m, flag, col):
+    """The first two constraints of SllChip, SrlChip and SraChip: ValueC's low byte = ShiftBit1..5 + 32 Helper1[0], and Exp1_3 = 2^(its
+    low three bits).  Returns ShiftBit1..5."""
+    sh = [col[f"ShiftBit{k}"][0] for k in range(1, 6)]
+    m.add_constraint(flag * (sh[0] + sh[1] * 2 + sh[2] * 4 + sh[3] * 8 + sh[4] * 16 + col["Helper1"][0] * 32 - col["ValueC"][0]))
+    m.add_constraint(flag * ((sh[0] + 1) * (sh[1] * 3 + 1) * (sh[2] * 15 + 1) - col["Exp1_3"][0]))
+    return sh
+
+
+def _right_shift_by_exp(m, flag, col):
+    """SrlChip's and SraChip's byte-wise division of ValueB by Exp1_3: quotients Qt, remainders Rem carried down from the top byte."""
+    vb, rem, qt, e = col["ValueB"], col["Rem"], col["Qt"], col["Exp1_3"][0]
+    m.add_constraint(flag * (vb[3] - rem[3] - qt[3] * e))
+    for i in (2, 1, 0):
+        m.add_constraint(flag * (vb[i] + rem[i + 1] * 256 - rem[i] - qt[i] * e))
+
+
+def _byte_moves(sh4, sh5):
+    """The byte-shift selectors of ShiftBit4 / ShiftBit5 for a move by 0, 1, 2 and 3 bytes."""
+    return [(1 - sh4) * (1 - sh5), sh4 * (1 - sh5), (1 - sh4) * sh5, sh4 * sh5]
+
+
+def _record_sll(m, c, col):
+    """SllChip (sll.rs:114-199): ValueB times Exp1_3 byte by byte (Rem, carries Qt), then moved up by ShiftBit4 + 2 ShiftBit5 bytes."""
+    is_sll, vb, va, rem, qt, e = c("IsSll"), col["ValueB"], col["ValueA"], col["Rem"], col["Qt"], col["Exp1_3"][0]
+    sh = _shift_amount(m, is_sll, col)
+    m.add_constraint(is_sll * (rem[0] + qt[0] * 256 - vb[0] * e))
+    for i in (1, 2, 3):
+        m.add_constraint(is_sll * (rem[i] + qt[i] * 256 - qt[i - 1] - vb[i] * e))
+    sel = _byte_moves(sh[3], sh[4])
+    for i in range(4):
+        acc = va[i]
+        for j in range(i + 1):
+            acc = acc - rem[i - j] * sel[j]
+        m.add_constraint(is_sll * acc)
+
+
+def _record_srl(m, c, col):
+    """SrlChip (srl.rs:121-232): ValueB divided by Exp1_3 byte by byte, the quotients moved down by ShiftBit4 + 2 ShiftBit5 bytes, and
+    RemDiff = Exp1_3 - 1 - Rem (Range256-checked, so Rem < Exp1_3)."""
+    is_srl, va, qt, rem, e = c("IsSrl"), col["ValueA"], col["Qt"], col["Rem"], col["Exp1_3"][0]
+    sh = _shift_amount(m, is_srl, col)
+    _right_shift_by_exp(m, is_srl, col)
+    sel = _byte_moves(sh[3], sh[4])
+    for i in (3, 2, 1, 0):
+        acc = va[i]
+        for j in range(4 - i):
+            acc = acc - qt[i + j] * sel[j]
+        m.add_constraint(is_srl * acc)
+    for i in range(4):
+        m.add_constraint(is_srl * (e - 1 - rem[i] - col["RemDiff"][i]))
+
+
+def _record_sra(m, c, col):
+    """SraChip (sra.rs:141-347): SRL's quotients into Helper3 (the logical shift), SgnB split off ValueB's top byte (low seven bits in
+    Helper2[0]), Exp = 2^8 / Exp1_3, SraDegreeAux = SgnB (Exp1_3 - 1) Exp (the sign bits the byte the shift lands in gets), and ValueA =
+    the logical shift with the sign replicated into the vacated bytes."""
+    is_sra, vb, va, qt, rem, e = c("IsSra"), col["ValueB"], col["ValueA"], col["Qt"], col["Rem"], col["Exp1_3"][0]
+    srl, exp, sgn_b, aux = col["Helper3"], c("Exp"), c("SgnB"), c("SraDegreeAux")
+    sh = _shift_amount(m, is_sra, col)
+    _right_shift_by_exp(m, is_sra, col)
+    m.add_constraint(is_sra * (col["Helper2"][0] + sgn_b * 128 - vb[3]))
+    sel = _byte_moves(sh[3], sh[4])
+    for i in (3, 2, 1, 0):
+        acc = srl[i]
+        for j in range(4 - i):
+            acc = acc - qt[i + j] * sel[j]
+        m.add_constraint(is_sra * acc)
+    sh1, sh2, sh3, sh4, sh5 = sh
+    m.add_constraint(is_sra * (2 * (2 - sh1) * (4 - sh2 * 3) * (16 - sh3 * 15) - exp))
+    m.add_constraint(is_sra * (sgn_b * (e - 1) * exp - aux))
+    m.add_constraint(is_sra * (va[3] - (1 - sh4) * (1 - sh5) * (srl[3] + aux) - (sh4 + sh5 - sh4 * sh5) * sgn_b * 255))
+    m.add_constraint(is_sra * (va[2] - (1 - sh4) * (1 - sh5) * srl[2] - sh4 * (1 - sh5) * (srl[2] + aux) - sh5 * sgn_b * 255))
+    m.add_constraint(is_sra * (va[1] - (1 - sh5) * srl[1] - (1 - sh4) * sh5 * (srl[1] + aux) - sh4 * sh5 * sgn_b * 255))
+    m.add_constraint(is_sra * (va[0] - (1 - sh4 * sh5) * srl[0] - sh4 * sh5 * (srl[0] + aux)))
+    for i in range(4):
+        m.add_constraint(is_sra * (e - 1 - rem[i] - col["RemDiff"][i]))
+
+
+# the instruction chips that alu=True records, in BaseComponent's order (SltuChip before BitOpChip, the others after it)
+ALU_CHIPS_BEFORE_BIT_OP = [("SltuChip", _record_sltu)]
+ALU_CHIPS_AFTER_BIT_OP = [("SltChip", _record_slt), ("SllChip", _record_sll), ("SrlChip", _record_srl), ("SraChip", _record_sra)]
+
+
+def record_main_component(air, log_size, rel, keccak=False, decoding=False, alu=False):
     """Record the main component (`MachineEval<BaseComponent>`, NexusV1Machine's docstring) into `air`: the chips in BaseComponent's order
     against the relations `rel` (name -> air.Relation: BitOp, LoadStore, ProgramCheck, RegisterCheck, Range8/16/32/128/256), then
     `finalize_logup()`.  `keccak`: the keccak extension is enabled, so KeccakChip (CustomInstructionChip, after LoadStoreChip) adds its
     booleanity constraint on IsCustomKeccak (chips/custom.rs:178-196).  `decoding`: DecodingCheckChip's type R and type I constraints
     (_record_decoding_r_i) follow CpuChip's, as DecodingCheckChip follows CpuChip in BaseComponent; its types B, J, S, U and SYS are not
-    recorded.  Returns (component, {column name: its masks})."""
+    recorded.  `alu`: the arithmetic of SltuChip, SltChip, SllChip, SrlChip and SraChip (ALU_CHIPS_*) in their places among the chips, so
+    that every RV32I register-register and register-immediate instruction but LUI / AUIPC is constrained.  Returns (component, {column
+    name: its masks})."""
     m = air.component(log_size, 2)
     pre, col = {}, {}
     for name, size in PREPROCESSED_COLUMNS + PROGRAM_COLUMNS:           # TraceEval::new: preprocessed ids, then program ids
@@ -288,19 +398,27 @@ def record_main_component(air, log_size, rel, keccak=False, decoding=False):
     # ---------------- DecodingCheckChip, types R and I (chips/decoding/type_r.rs:61-409, type_i.rs:71-442) ----------------
     if decoding:
         _record_decoding_r_i(m, c, col, is_type_r, is_load, alu_imm_no_shift, alu_imm_shift, is_type_i_no_shift)
-    # ---------------- AddChip / SubChip ----------------
+    # ---------------- AddChip / SubChip, and SltuChip (sltu.rs) with `alu` ----------------
     cf = col["CarryFlag"]
     is_add, is_sub = c("IsAdd"), c("IsSub")
     m.add_constraint(is_add * (va[0] + va[1] * 256 + cf[0] * 65536 - (vb[0] + vb[1] * 256 + vc[0] + vc[1] * 256)))
     m.add_constraint(is_add * (va[2] + va[3] * 256 + cf[1] * 65536 - (vb[2] + vb[3] * 256 + vc[2] + vc[3] * 256 + cf[0])))
     m.add_constraint(is_sub * (va[0] + va[1] * 256 - cf[0] * 65536 - (vb[0] + vb[1] * 256 - vc[0] - vc[1] * 256)))
     m.add_constraint(is_sub * (va[2] + va[3] * 256 - cf[1] * 65536 - (vb[2] + vb[3] * 256 - vc[2] - vc[3] * 256 - cf[0])))
+    if alu:
+        for _name, record in ALU_CHIPS_BEFORE_BIT_OP:
+            record(m, c, col)
     # ---------------- BitOpChip: lookup structure (bit_op.rs:380-431; 4 limbs x {And, Or, Xor} x {low, high nibble} = 24 fractions) ----------------
     va47, vb47, vc47 = col["ValueA4_7"], col["ValueB4_7"], col["ValueC4_7"]
     for k in range(4):
         for op_code, flag in ((1, c("IsAnd")), (2, c("IsOr")), (3, c("IsXor"))):
             m.add_to_relation(rel["BitOp"], flag, [m.const(op_code), vb[k] - vb47[k] * 16, vc[k] - vc47[k] * 16, va[k] - va47[k] * 16])
             m.add_to_relation(rel["BitOp"], flag, [m.const(op_code), vb47[k], vc47[k], va47[k]])
+    # ---------------- SltChip, SllChip, SrlChip, SraChip (slt.rs, sll.rs, srl.rs, sra.rs; between them the branch, jump, LUI and AUIPC chips,
+    # not recorded) ----------------
+    if alu:
+        for _name, record in ALU_CHIPS_AFTER_BIT_OP:
+            record(m, c, col)
     # ---------------- LoadStoreChip: lookup structure (load_store.rs:650-685,788-903; 4 bytes x {subtract prev, add cur} = 8 fractions) ----------------
     ram1 = ssum(["IsSb", "IsSh", "IsSw", "IsLb", "IsLh", "IsLbu", "IsLhu", "IsLw"])
     ram2 = ssum(["IsSh", "IsSw", "IsLh", "IsLhu", "IsLw"])

@@ -1,7 +1,8 @@
 """Time GPU proofs of the reference's ADD-chain benchmark as an executing v1 trace (nexus_zkvm_b200/add_chain.py), from host columns and from
-device-filled trees, and time the main trace's device fill (nb200_v1_main_trace).
+device-filled trees, and time the main trace's device fill (nb200_v1_main_trace).  `--program alu` does the same for add_chain.AluMachine, a
+seeded program of RV32I's 19 ALU instructions (filled by nb200_v1_alu_trace), and writes alu_program_prove.json instead.
 
-    python tools/add_chain_prove.py [--log-sizes 16 18 20] [--steps 3] [--warmup 1] [--fill-calls 20] [--out-dir DIR]
+    python tools/add_chain_prove.py [--program {add-chain,alu}] [--log-sizes 16 18 20] [--steps 3] [--warmup 1] [--fill-calls 20] [--out-dir DIR]
 
 For each log size n: AddChainMachine(n), 2^n executed steps and no padding rows.  Two arms alternate step by step after the warm-up: `host`
 proves from the host columns (machine.prove with tree 1 built on the host), `device` from AddChainMachine.device_trees (tree 0 and FinalReg
@@ -31,20 +32,20 @@ def one_size(a, log_size, ctx, backend, stream, pool):
     import torch
 
     from nexus_zkvm_b200 import machine as M
-    from nexus_zkvm_b200.add_chain import AddChainMachine
+    from nexus_zkvm_b200.add_chain import AddChainMachine, AluMachine
 
     t0 = time.perf_counter()
-    m = AddChainMachine(log_size)
+    m = AluMachine(log_size) if a.program == "alu" else AddChainMachine(log_size)
     cols = m.fill_main_trace()
     witness_s = time.perf_counter() - t0
     out_batch = ctx.alloc(347, log_size)
-    ctx.v1_main_trace(m.steps, m.final_ctr, log_size, out=out_batch)
+    m.device_fill(ctx, out=out_batch)
     ctx.sync()
     fill_ms = []
     for _ in range(a.fill_calls):
         ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         ev0.record(stream)
-        ctx.v1_main_trace(m.steps, m.final_ctr, log_size, out=out_batch)
+        m.device_fill(ctx, out=out_batch)
         ev1.record(stream)
         ev1.synchronize()
         fill_ms.append(ev0.elapsed_time(ev1))
@@ -88,6 +89,7 @@ def one_size(a, log_size, ctx, backend, stream, pool):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--program", choices=["add-chain", "alu"], default="add-chain")
     ap.add_argument("--log-sizes", type=int, nargs="+", default=[16, 18, 20])
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
@@ -106,9 +108,12 @@ def main():
     backend = CudaBackend(ctx)
     pool = PoolHigh()
     sizes = [one_size(a, ls, ctx, backend, stream, pool) for ls in a.log_sizes]
+    workload = {"add-chain": "AddChainMachine: the reference's ADD-chain benchmark (addi x1,x0,1; add x_k,x_j,x_i), 2^n executed steps, v1 "
+                             "main component with DecodingCheck R / I + the eight base extensions",
+                "alu": "AluMachine: alu_program(n, seed=0), 2^n executed steps over RV32I's 19 ALU instructions (ADD ... SRAI), v1 main "
+                       "component with DecodingCheck R / I and SltuChip, SltChip, SllChip, SrlChip, SraChip + the eight base extensions"}
     out = {
-        "workload": "AddChainMachine: the reference's ADD-chain benchmark (addi x1,x0,1; add x_k,x_j,x_i), 2^n executed steps, v1 main "
-                    "component with DecodingCheck R / I + the eight base extensions",
+        "workload": workload[a.program],
         "config": dict(pow_bits=5, log_blowup=1, log_last=0, n_queries=3),
         "steps": a.steps, "warmup": a.warmup, "fill_calls": a.fill_calls,
         "timing": "host clock from the call to the proof bytes on the host, minimum over the steps (arms alternate); kHz = executed steps / "
@@ -118,7 +123,8 @@ def main():
         "card": card(),
     }
     os.makedirs(a.out_dir, exist_ok=True)
-    with open(os.path.join(a.out_dir, "add_chain_prove.json"), "w") as f:
+    name = "alu_program_prove.json" if a.program == "alu" else "add_chain_prove.json"
+    with open(os.path.join(a.out_dir, name), "w") as f:
         json.dump(out, f, indent=1)
     print(json.dumps(out))
     ctx.close()
