@@ -272,8 +272,9 @@ def valid_alu_steps(steps, final_ctr, log_size):
                 and all(np.all(s[f"ts{k}_prev"] < 3 * clk + k) for k in (1, 2, 3)))
 
 
-@pytest.mark.parametrize("ls,n_steps", [(8, 256), (10, 900), (12, 4096)])
+@pytest.mark.parametrize("ls,n_steps", [(8, 256), (10, 900), (12, 4096), (16, 40000)])
 def test_host_fill_on_edge_step_records(host_fill, ls, n_steps):
+    """(16, 40000): from the 21845th step on the timestamps pass 2^16, and the CH*Minus borrow is taken."""
     steps, final_ctr = alu_edge_steps(ls, n_steps, seed=ls)
     want = _want(steps, final_ctr, ls)
     bad = np.argwhere(host_fill(steps, final_ctr, ls) != want)
