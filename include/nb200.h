@@ -216,6 +216,26 @@ nb200_status nb200_v1_main_trace(nb200_ctx*, size_t n_steps, const uint32_t* ste
 nb200_status nb200_v1_alu_trace(nb200_ctx*, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
                                 nb200_cols* out);
 
+/* ---- the same fill for a looping program: RV32I's branches, jumps, LUI and AUIPC ------------------------------------------------
+ * nb200_v1_alu_trace's arguments, step record and kernel, for its 19 opcodes and the control-flow opcodes (add_chain.CONTROL_OPCODES)
+ *   19 BEQ    20 BNE    21 BLT    22 BGE    23 BLTU   24 BGEU   25 JAL    26 JALR   27 LUI    28 AUIPC
+ * Steps need not follow one another in pc: the row of step t holds its own pc, and the next pc (PcNext) follows from pc, the opcode and
+ * the values.  pc_ctr_prev counts the earlier executions of the instruction at pc, final_ctr each program row's executions (0 for a row
+ * that never ran).  Per type:
+ *   B (BEQ ... BGEU): rd = op_a, the instruction's rs1 field, read through Reg3 (its value in rd_prev, which is ValueA); rs1 = op_b, the
+ *     instruction's rs2 field, read through Reg1 (its value in value_b); op_c = value_c = the sign-extended, even 13-bit offset;
+ *     ts1_prev and ts3_prev are the previous timestamps of op_b and op_a, ts2_prev = 0.  PcNext = pc + value_c when taken, else pc + 4.
+ *   JAL (type J): rs1 = value_b = 0, op_c = value_c = the sign-extended, even 21-bit offset; ValueA = pc + 4, PcNext = pc + value_c.
+ *   JALR (type I): rd, rs1, op_c and value_c as ADDI's; ValueA = pc + 4, PcNext = (value_b + value_c) with bit 0 cleared.
+ *   LUI, AUIPC (type U): rs1 = value_b = 0, op_c = the 20-bit immediate, value_c = op_c << 12; ValueA = value_c, or pc + value_c.
+ * The rows add the per-row fills of BneChip, BeqChip, BltuChip, BltChip, BgeuChip, BgeChip, JalChip, LuiChip, AuipcChip, JalrChip and
+ * DecodingCheck's types B, U and J.  The fill does not check that the steps' pcs chain; the main component's next-row Pc constraint does.
+ * NB200_ERR_ARG: what nb200_v1_alu_trace refuses but its opcode rule, and an opcode above 28, a JALR immediate that is not a sign-extended
+ * 12-bit value, a branch offset that is not an even sign-extended 13-bit value, a JAL offset that is not an even sign-extended 21-bit
+ * value, a U-type immediate of more than 20 bits. */
+nb200_status nb200_v1_control_trace(nb200_ctx*, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr,
+                                    uint32_t log_size, nb200_cols* out);
+
 /* ---- one commitment over N GPUs (SURVEY §8e; one process per GPU, NCCL over NVLink inside the library) ------------------------
  * The reference has no multi-device path (SURVEY App. C); these entry points are what a multi-GPU `CudaBackend` would drive from
  * TreeBuilder::commit (machine.rs:208-263).  Rank 0 creates the id and hands it to the other ranks out of band (MPI, a file,

@@ -295,6 +295,19 @@ class Context:
                                            C.c_uint32(log_size), out._h))
         return out
 
+    def v1_control_trace(self, steps, final_ctr, log_size, out=None):
+        """nb200_v1_control_trace: v1_alu_trace for a looping program of those 19 opcodes and the branches, JAL, JALR, LUI and AUIPC of
+        add_chain.CONTROL_OPCODES (opcodes 19-28), same arguments and step record; final_ctr holds each program row's execution count.
+        Returns out."""
+        st = np.ascontiguousarray(steps, dtype=np.uint32)
+        ctr = np.ascontiguousarray(final_ctr, dtype=np.uint32)
+        assert st.ndim == 2 and st.shape[0] == 13 and ctr.ndim == 1, "step record shapes"
+        if out is None:
+            out = self.alloc(347, log_size)
+        self._chk(lib().nb200_v1_control_trace(self._h, C.c_size_t(st.shape[1]), st.ctypes.data_as(u32p), C.c_size_t(ctr.size),
+                                               ctr.ctypes.data_as(u32p), C.c_uint32(log_size), out._h))
+        return out
+
     def table_multiplicities(self, air, tree0, tree1, first_row=False):
         """nb200_table_multiplicities: every table fraction's multiplicity column of `tree1` (device batches, finalized order) is overwritten
         with the count of the AIR's lookups into it.  `air` is a loaded AIR (prover.Air).  Returns (n_unmatched, first_unmatched), the latter

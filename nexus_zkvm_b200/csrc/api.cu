@@ -33,6 +33,8 @@ nb200_status v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps
                            nb200_cols* out);
 nb200_status v1_alu_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
                           nb200_cols* out);
+nb200_status v1_control_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                              nb200_cols* out);
 }  // namespace nb
 using namespace nb;
 
@@ -491,6 +493,13 @@ nb200_status nb200_v1_alu_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* 
                                 nb200_cols* out) {
   if (!ctx) return NB200_ERR_ARG;
   return v1_alu_trace(ctx, n_steps, steps, n_prog, final_ctr, log_size, out);
+}
+
+// ---- the same fill for a looping program of those, RV32I's branches, JAL, JALR, LUI and AUIPC (csrc/v1_trace.cu) ----
+nb200_status nb200_v1_control_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr,
+                                    uint32_t log_size, nb200_cols* out) {
+  if (!ctx) return NB200_ERR_ARG;
+  return v1_control_trace(ctx, n_steps, steps, n_prog, final_ctr, log_size, out);
 }
 
 }  // extern "C"

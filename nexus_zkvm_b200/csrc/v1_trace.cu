@@ -1,5 +1,6 @@
 // The v1 main component's main trace filled on the device from a program's step record (nb200_v1_main_trace for ADD / ADDI programs,
-// nb200_v1_alu_trace for the 19 ALU opcodes; one kernel behind two host checks): what add_chain.main_columns builds for the main
+// nb200_v1_alu_trace for the 19 ALU opcodes, nb200_v1_control_trace for those and the 10 control-flow opcodes; one kernel behind three
+// host checks): what add_chain.main_columns builds for the main
 // component on the host, followed by finalize_columns, without the host columns or their upload.  The batch is cleared first (the columns
 // no executed or padding row sets stay zero); then one thread per finalized row position writes its row's other columns (v1_trace.cuh),
 // so consecutive threads write consecutive words of every column.
@@ -20,9 +21,13 @@ __global__ void __launch_bounds__(V1_BLOCK) v1_main_trace_kernel(const u32* __re
   v1::main_row(steps, n_steps, final_ctr, n_prog, log_size, i, out + i, (size_t)1 << log_size);
 }
 
-// The host check of a step record and the fill.  `alu`: the 19 opcodes of nb200_v1_alu_trace, with their operand ranges; otherwise ADD and
-// ADDI only, as nb200_v1_main_trace has always taken them.
-nb200_status v1_fill(nb200_ctx* ctx, const char* who, bool alu, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr,
+// Which opcodes a fill entry takes: ADD and ADDI (nb200_v1_main_trace), the 19 ALU opcodes (nb200_v1_alu_trace) or all 29
+// (nb200_v1_control_trace).
+enum class Opcodes { ADD_ADDI, ALU, CONTROL };
+
+// The host check of a step record and the fill: the opcodes of `ops` with their operand ranges.  The fill does not check that the pcs
+// chain; the main component's next-row Pc constraint does.
+nb200_status v1_fill(nb200_ctx* ctx, const char* who, Opcodes ops, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr,
                      uint32_t log_size, nb200_cols* out) {
   const std::string me = who;
   NB_ARG(ctx, out && (n_steps == 0 || steps) && (n_prog == 0 || final_ctr), me + ": null argument");
@@ -34,11 +39,20 @@ nb200_status v1_fill(nb200_ctx* ctx, const char* who, bool alu, size_t n_steps, 
   auto f = [&](u32 field, size_t t) { return steps[field * n_steps + t]; };
   for (size_t t = 0; t < n_steps; ++t) {
     const u32 op = f(v1::OPCODE, t), op_c = f(v1::OP_C, t);
-    if (alu) {
-      NB_ARG(ctx, op < v1::N_OPCODES, me + ": step " + std::to_string(t) + " has an opcode above 18");
+    if (ops != Opcodes::ADD_ADDI) {
+      if (ops == Opcodes::ALU)
+        NB_ARG(ctx, op < v1::N_OPCODES, me + ": step " + std::to_string(t) + " has an opcode above 18");
+      else
+        NB_ARG(ctx, op < v1::N_ALL_OPCODES, me + ": step " + std::to_string(t) + " has an opcode above 28");
       NB_ARG(ctx, !v1::is_type_i_shift(op) || op_c < 32, me + ": step " + std::to_string(t) + " has a shift amount above 31");
-      NB_ARG(ctx, !v1::is_type_i(op) || op_c + 2048u < 4096u,
+      NB_ARG(ctx, !(v1::is_type_i(op) || op == v1::OP_JALR) || op_c + 2048u < 4096u,
              me + ": step " + std::to_string(t) + " has an immediate that is not a sign-extended 12-bit value");
+      NB_ARG(ctx, !v1::is_type_b(op) || (op_c + 4096u < 8192u && op_c % 2 == 0),
+             me + ": step " + std::to_string(t) + " has a branch offset that is not an even sign-extended 13-bit value");
+      NB_ARG(ctx, op != v1::OP_JAL || (op_c + (1u << 20) < (1u << 21) && op_c % 2 == 0),
+             me + ": step " + std::to_string(t) + " has a JAL offset that is not an even sign-extended 21-bit value");
+      NB_ARG(ctx, (op != v1::OP_LUI && op != v1::OP_AUIPC) || op_c < (1u << 20),
+             me + ": step " + std::to_string(t) + " has a U-type immediate above 20 bits");
     } else {
       NB_ARG(ctx, op == v1::OP_ADD || op == v1::OP_ADDI, me + ": step " + std::to_string(t) + " is not ADD or ADDI");
     }
@@ -68,12 +82,17 @@ nb200_status v1_fill(nb200_ctx* ctx, const char* who, bool alu, size_t n_steps, 
 
 nb200_status v1_main_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
                            nb200_cols* out) {
-  return v1_fill(ctx, "v1_main_trace", false, n_steps, steps, n_prog, final_ctr, log_size, out);
+  return v1_fill(ctx, "v1_main_trace", Opcodes::ADD_ADDI, n_steps, steps, n_prog, final_ctr, log_size, out);
 }
 
 nb200_status v1_alu_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
                           nb200_cols* out) {
-  return v1_fill(ctx, "v1_alu_trace", true, n_steps, steps, n_prog, final_ctr, log_size, out);
+  return v1_fill(ctx, "v1_alu_trace", Opcodes::ALU, n_steps, steps, n_prog, final_ctr, log_size, out);
+}
+
+nb200_status v1_control_trace(nb200_ctx* ctx, size_t n_steps, const uint32_t* steps, size_t n_prog, const uint32_t* final_ctr, uint32_t log_size,
+                              nb200_cols* out) {
+  return v1_fill(ctx, "v1_control_trace", Opcodes::CONTROL, n_steps, steps, n_prog, final_ctr, log_size, out);
 }
 
 }  // namespace nb

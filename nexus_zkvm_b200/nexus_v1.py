@@ -320,15 +320,206 @@ ALU_CHIPS_BEFORE_BIT_OP = [("SltuChip", _record_sltu)]
 ALU_CHIPS_AFTER_BIT_OP = [("SltChip", _record_slt), ("SllChip", _record_sll), ("SrlChip", _record_srl), ("SraChip", _record_sra)]
 
 
-def record_main_component(air, log_size, rel, keccak=False, decoding=False, alu=False):
+def _record_type_b(m, c, col):
+    """DecodingCheck's TypeBChip (type_b.rs:75-233): OpC is the raw 13-bit offset (OpC1_4, OpC5_7, OpC8_10, OpC11, OpC12), ValueC its
+    sign extension; OpA is the instruction's rs1 field, OpB its rs2 field (OpB0_3, OpB4); the instruction word's bytes."""
+    t = sum_of(c, IS_TYPE_B)
+    c14, c57, c810, c11, c12 = c("OpC1_4"), c("OpC5_7"), c("OpC8_10"), c("OpC11"), c("OpC12")
+    a0, a14, b03, b4 = c("OpA0"), c("OpA1_4"), c("OpB0_3"), c("OpB4")
+    vc, iv = col["ValueC"], col["InstrVal"]
+    m.add_constraint(t * (c14 * 2 + c57 * 32 + c810 * 256 + c11 * 2048 + c12 * 4096 - c("OpC")))
+    m.add_constraint(t * (c14 * 2 + c57 * 32 - vc[0]))
+    m.add_constraint(t * (c810 + c11 * 8 + c12 * 15 * 16 - vc[1]))
+    m.add_constraint(t * (c12 * 255 - vc[2]))
+    m.add_constraint(t * (c12 * 255 - vc[3]))
+    m.add_constraint(t * (a0 + a14 * 2 - c("OpA")))
+    m.add_constraint(t * (b03 + b4 * 16 - c("OpB")))
+    m.add_constraint(t * (0b1100011 + c11 * 128 - iv[0]))
+    for flag, f3 in (("IsBeq", 0b000), ("IsBne", 0b001), ("IsBlt", 0b100), ("IsBge", 0b101), ("IsBltu", 0b110), ("IsBgeu", 0b111)):
+        m.add_constraint(c(flag) * (c14 + f3 * 16 + a0 * 128 - iv[1]))
+    m.add_constraint(t * (a14 + b03 * 16 - iv[2]))
+    m.add_constraint(t * (b4 + c57 * 2 + c810 * 16 + c12 * 128 - iv[3]))
+
+
+def _record_type_u(m, c, col):
+    """DecodingCheck's TypeUChip (type_u.rs:53-138): OpC is the 20-bit immediate (OpC12_15, OpC16_23, OpC24_31), ValueC = OpC << 12,
+    OpB = ValueB = 0; the instruction word's bytes."""
+    t = sum_of(c, IS_TYPE_U)
+    c1215, c1623, c2431, a0, a14 = c("OpC12_15"), c("OpC16_23"), c("OpC24_31"), c("OpA0"), c("OpA1_4")
+    vb, vc, iv = col["ValueB"], col["ValueC"], col["InstrVal"]
+    m.add_constraint(t * (c1215 + c1623 * 16 + c2431 * 4096 - c("OpC")))
+    m.add_constraint(t * vc[0])
+    m.add_constraint(t * (c1215 * 16 - vc[1]))
+    m.add_constraint(t * (c1623 - vc[2]))
+    m.add_constraint(t * (c2431 - vc[3]))
+    m.add_constraint(t * (a0 + a14 * 2 - c("OpA")))
+    m.add_constraint(t * c("OpB"))
+    for k in range(4):
+        m.add_constraint(t * vb[k])
+    m.add_constraint(c("IsLui") * (0b0110111 + a0 * 128 - iv[0]))
+    m.add_constraint(c("IsAuipc") * (0b0010111 + a0 * 128 - iv[0]))
+    m.add_constraint(t * (a14 + c1215 * 16 - iv[1]))
+    m.add_constraint(t * (c1623 - iv[2]))
+    m.add_constraint(t * (c2431 - iv[3]))
+
+
+def _record_type_j(m, c, col):
+    """DecodingCheck's TypeJChip (type_j.rs:64-193): OpC is the raw 21-bit offset (OpC1_3, OpC4_7, OpC8_10, OpC11, OpC12_15, OpC16_19,
+    OpC20), ValueC its sign extension, OpB = ValueB = 0; the instruction word's bytes."""
+    t = c("IsJal")
+    c13, c47, c810, c11, c1215, c1619, c20 = (c(n) for n in ("OpC1_3", "OpC4_7", "OpC8_10", "OpC11", "OpC12_15", "OpC16_19", "OpC20"))
+    a0, a14 = c("OpA0"), c("OpA1_4")
+    vb, vc, iv = col["ValueB"], col["ValueC"], col["InstrVal"]
+    m.add_constraint(t * (c13 * 2 + c47 * 16 + c810 * 256 + c11 * 2048 + c1215 * 4096 + c1619 * 65536 + c20 * (1 << 20) - c("OpC")))
+    m.add_constraint(t * (c13 * 2 + c47 * 16 - vc[0]))
+    m.add_constraint(t * (c810 + c11 * 8 + c1215 * 16 - vc[1]))
+    m.add_constraint(t * (c1619 + c20 * 15 * 16 - vc[2]))
+    m.add_constraint(t * (c20 * 255 - vc[3]))
+    m.add_constraint(t * (a0 + a14 * 2 - c("OpA")))
+    m.add_constraint(t * c("OpB"))
+    for k in range(4):
+        m.add_constraint(t * vb[k])
+    m.add_constraint(t * (0b1101111 + a0 * 128 - iv[0]))
+    m.add_constraint(t * (a14 + c1215 * 16 - iv[1]))
+    m.add_constraint(t * (c1619 + c11 * 16 + c13 * 32 - iv[2]))
+    m.add_constraint(t * (c47 + c810 * 16 + c20 * 128 - iv[3]))
+
+
+def _next_pc(m, flag, col, taken):
+    """The two 16-bit halves of PcNext = Pc + (taken ? ValueC : 4) with CarryFlag as the carries (the branch chips' last two constraints)."""
+    vc, pc, pn, cf = col["ValueC"], col["Pc"], col["PcNext"], col["CarryFlag"]
+    m.add_constraint(flag * (taken * (vc[0] + vc[1] * 256) + (1 - taken) * 4 + pc[0] + pc[1] * 256 - cf[0] * 65536 - pn[0] - pn[1] * 256))
+    m.add_constraint(flag * (taken * (vc[2] + vc[3] * 256) + pc[2] + pc[3] * 256 + cf[0] - cf[1] * 65536 - pn[2] - pn[3] * 256))
+
+
+def _record_beq_bne(flag_name, equal_taken):
+    """BeqChip / BneChip (beq.rs:152-260, bne.rs): Neq12 / Neq34 = the 16-bit halves of ValueA and ValueB differ, through the inverses
+    Neq12Aux / Neq34Aux of their differences (any nonzero value with its inverse when they are equal), Neq = either differs, and PcNext."""
+    def record(m, c, col):
+        flag, va, vb = c(flag_name), col["ValueA"], col["ValueB"]
+        neq, n12, n34 = c("Neq"), c("Neq12"), c("Neq34")
+        m.add_constraint(flag * ((va[0] + va[1] * 256 - vb[0] - vb[1] * 256) * c("Neq12Aux") - n12))
+        m.add_constraint(flag * ((va[2] + va[3] * 256 - vb[2] - vb[3] * 256) * c("Neq34Aux") - n34))
+        m.add_constraint(flag * n12 * (1 - n12))
+        m.add_constraint(flag * n34 * (1 - n34))
+        m.add_constraint(flag * (c("Neq12Aux") * c("Neq12AuxInv") - 1))
+        m.add_constraint(flag * (c("Neq34Aux") * c("Neq34AuxInv") - 1))
+        m.add_constraint(flag * ((1 - n12) * (1 - n34) - (1 - neq)))
+        _next_pc(m, flag, col, 1 - neq if equal_taken else neq)
+    return record
+
+
+def _sub_borrows(m, flag, col):
+    """Helper1 = ValueA - ValueB with BorrowFlag as the borrows out of the 16-bit halves (the compare branches' first two constraints)."""
+    va, vb, h1, bf = col["ValueA"], col["ValueB"], col["Helper1"], col["BorrowFlag"]
+    m.add_constraint(flag * (va[0] + va[1] * 256 - vb[0] - vb[1] * 256 - h1[0] - h1[1] * 256 + bf[0] * 65536))
+    m.add_constraint(flag * (va[2] + va[3] * 256 - vb[2] - vb[3] * 256 - h1[2] - h1[3] * 256 + bf[1] * 65536 - bf[0]))
+
+
+def _record_bltu_bgeu(flag_name, less_taken):
+    """BltuChip / BgeuChip (bltu.rs:111-185, bgeu.rs): the unsigned borrow of ValueA - ValueB decides the branch."""
+    def record(m, c, col):
+        flag, ltu = c(flag_name), col["BorrowFlag"][1]
+        _sub_borrows(m, flag, col)
+        _next_pc(m, flag, col, ltu if less_taken else 1 - ltu)
+    return record
+
+
+def _record_blt(m, c, col):
+    """BltChip (blt.rs:138-241): LtFlag = the signed comparison, from the unsigned borrow and the sign bits (ValueA / ValueB's top bytes less
+    Helper2[3] / Helper3[3], over 128)."""
+    flag, va, vb, lt, ltu = c("IsBlt"), col["ValueA"], col["ValueB"], c("LtFlag"), col["BorrowFlag"][1]
+    inv128 = pow(128, P - 2, P)
+    sgn_a, sgn_b = (va[3] - col["Helper2"][3]) * inv128, (vb[3] - col["Helper3"][3]) * inv128
+    _sub_borrows(m, flag, col)
+    m.add_constraint(flag * (sgn_a * (1 - sgn_b) + ltu * (sgn_a * sgn_b + (1 - sgn_a) * (1 - sgn_b)) - lt))
+    _next_pc(m, flag, col, lt)
+    m.add_constraint(flag * (sgn_a * (1 - sgn_a)))
+    m.add_constraint(flag * (sgn_b * (1 - sgn_b)))
+
+
+def _record_bge(m, c, col):
+    """BgeChip (bge.rs:143-268): BLT's comparison with the sign bits in SgnA / SgnB, the branch taken when LtFlag is 0."""
+    flag, va, vb, lt, ltu = c("IsBge"), col["ValueA"], col["ValueB"], c("LtFlag"), col["BorrowFlag"][1]
+    sgn_a, sgn_b = c("SgnA"), c("SgnB")
+    _sub_borrows(m, flag, col)
+    m.add_constraint(flag * (col["Helper2"][3] + sgn_a * 128 - va[3]))
+    m.add_constraint(flag * (col["Helper3"][3] + sgn_b * 128 - vb[3]))
+    m.add_constraint(flag * (sgn_a * (1 - sgn_b) + ltu * (sgn_a * sgn_b + (1 - sgn_a) * (1 - sgn_b)) - lt))
+    _next_pc(m, flag, col, 1 - lt)
+
+
+def _link(m, flag, col):
+    """ValueA = Pc + 4 with CarryFlag as the carries (JalChip's and JalrChip's first two constraints)."""
+    pc, va, cf = col["Pc"], col["ValueA"], col["CarryFlag"]
+    m.add_constraint(flag * (4 + pc[0] + pc[1] * 256 - cf[0] * 65536 - va[0] - va[1] * 256))
+    m.add_constraint(flag * (pc[2] + pc[3] * 256 + cf[0] - cf[1] * 65536 - va[2] - va[3] * 256))
+
+
+def _add_halves(m, flag, x, y, carries, out):
+    """out = x + y over 16-bit halves of bytes, with `carries` the carries out of the low and the high half."""
+    m.add_constraint(flag * (x[0] + x[1] * 256 + y[0] + y[1] * 256 - carries[0] * 65536 - out[0] - out[1] * 256))
+    m.add_constraint(flag * (x[2] + x[3] * 256 + y[2] + y[3] * 256 + carries[0] - carries[1] * 65536 - out[2] - out[3] * 256))
+
+
+def _record_jal(m, c, col):
+    """JalChip (jal.rs:94-160): ValueA = Pc + 4, PcNext = Pc + ValueC with BorrowFlag as its carries."""
+    flag = c("IsJal")
+    _link(m, flag, col)
+    _add_halves(m, flag, col["ValueC"], col["Pc"], col["BorrowFlag"], col["PcNext"])
+
+
+def _record_lui(m, c, col):
+    """LuiChip (lui.rs:59-76): ValueA = ValueC (the immediate << 12)."""
+    for k in range(4):
+        m.add_constraint(c("IsLui") * (col["ValueC"][k] - col["ValueA"][k]))
+
+
+def _record_auipc(m, c, col):
+    """AuipcChip (auipc.rs:66-110): ValueA = Pc + ValueC with CarryFlag as the carries."""
+    _add_halves(m, c("IsAuipc"), col["Pc"], col["ValueC"], col["CarryFlag"], col["ValueA"])
+
+
+def _record_jalr(m, c, col):
+    """JalrChip (jalr.rs:108-213): ValueA = Pc + 4; PcNextAux = ValueB + ValueC with BorrowFlag as its carries; PcNext = PcNextAux with
+    bit 0 (RemAux) cleared, its low byte 2 QtAux."""
+    flag, pn, aux, qt = c("IsJalr"), col["PcNext"], col["PcNextAux"], c("QtAux")
+    _link(m, flag, col)
+    _add_halves(m, flag, col["ValueC"], col["ValueB"], col["BorrowFlag"], aux)
+    m.add_constraint(flag * (aux[0] - qt * 2 - c("RemAux")))
+    m.add_constraint(flag * (qt * 2 - pn[0]))
+    for k in (1, 2, 3):
+        m.add_constraint(flag * (aux[k] - pn[k]))
+
+
+# the decoding types and instruction chips that control=True records, in DecodingCheckChip's and BaseComponent's order (the instruction
+# chips between SltChip and SllChip)
+CONTROL_DECODING = [("TypeBChip", _record_type_b), ("TypeUChip", _record_type_u), ("TypeJChip", _record_type_j)]
+CONTROL_CHIPS = [("BneChip", _record_beq_bne("IsBne", False)), ("BeqChip", _record_beq_bne("IsBeq", True)),
+                 ("BltuChip", _record_bltu_bgeu("IsBltu", True)), ("BltChip", _record_blt), ("BgeuChip", _record_bltu_bgeu("IsBgeu", False)),
+                 ("BgeChip", _record_bge), ("JalChip", _record_jal), ("LuiChip", _record_lui), ("AuipcChip", _record_auipc),
+                 ("JalrChip", _record_jalr)]
+
+
+def sum_of(c, names):
+    """The sum of the named single-limb columns (record_main_component's ssum, for the chips recorded outside it)."""
+    acc = c(names[0])
+    for n in names[1:]:
+        acc = acc + c(n)
+    return acc
+
+
+def record_main_component(air, log_size, rel, keccak=False, decoding=False, alu=False, control=False):
     """Record the main component (`MachineEval<BaseComponent>`, NexusV1Machine's docstring) into `air`: the chips in BaseComponent's order
     against the relations `rel` (name -> air.Relation: BitOp, LoadStore, ProgramCheck, RegisterCheck, Range8/16/32/128/256), then
     `finalize_logup()`.  `keccak`: the keccak extension is enabled, so KeccakChip (CustomInstructionChip, after LoadStoreChip) adds its
     booleanity constraint on IsCustomKeccak (chips/custom.rs:178-196).  `decoding`: DecodingCheckChip's type R and type I constraints
     (_record_decoding_r_i) follow CpuChip's, as DecodingCheckChip follows CpuChip in BaseComponent; its types B, J, S, U and SYS are not
     recorded.  `alu`: the arithmetic of SltuChip, SltChip, SllChip, SrlChip and SraChip (ALU_CHIPS_*) in their places among the chips, so
-    that every RV32I register-register and register-immediate instruction but LUI / AUIPC is constrained.  Returns (component, {column
-    name: its masks})."""
+    that every RV32I register-register and register-immediate instruction but LUI / AUIPC is constrained.  `control` (with `alu`):
+    DecodingCheck's types B, U and J (CONTROL_DECODING) after types R and I, and the arithmetic of the branch, JAL, LUI, AUIPC and JALR
+    chips (CONTROL_CHIPS) between SltChip and SllChip, so that programs may branch, jump and call.  Returns (component, {column name: its
+    masks})."""
     m = air.component(log_size, 2)
     pre, col = {}, {}
     for name, size in PREPROCESSED_COLUMNS + PROGRAM_COLUMNS:           # TraceEval::new: preprocessed ids, then program ids
@@ -398,6 +589,10 @@ def record_main_component(air, log_size, rel, keccak=False, decoding=False, alu=
     # ---------------- DecodingCheckChip, types R and I (chips/decoding/type_r.rs:61-409, type_i.rs:71-442) ----------------
     if decoding:
         _record_decoding_r_i(m, c, col, is_type_r, is_load, alu_imm_no_shift, alu_imm_shift, is_type_i_no_shift)
+    assert not control or (alu and decoding)
+    if control:
+        for _name, record in CONTROL_DECODING:
+            record(m, c, col)
     # ---------------- AddChip / SubChip, and SltuChip (sltu.rs) with `alu` ----------------
     cf = col["CarryFlag"]
     is_add, is_sub = c("IsAdd"), c("IsSub")
@@ -414,10 +609,14 @@ def record_main_component(air, log_size, rel, keccak=False, decoding=False, alu=
         for op_code, flag in ((1, c("IsAnd")), (2, c("IsOr")), (3, c("IsXor"))):
             m.add_to_relation(rel["BitOp"], flag, [m.const(op_code), vb[k] - vb47[k] * 16, vc[k] - vc47[k] * 16, va[k] - va47[k] * 16])
             m.add_to_relation(rel["BitOp"], flag, [m.const(op_code), vb47[k], vc47[k], va47[k]])
-    # ---------------- SltChip, SllChip, SrlChip, SraChip (slt.rs, sll.rs, srl.rs, sra.rs; between them the branch, jump, LUI and AUIPC chips,
-    # not recorded) ----------------
+    # ---------------- SltChip, SllChip, SrlChip, SraChip (slt.rs, sll.rs, srl.rs, sra.rs); between SltChip and SllChip the branch, jump,
+    # LUI and AUIPC chips with `control` ----------------
     if alu:
-        for _name, record in ALU_CHIPS_AFTER_BIT_OP:
+        after = list(ALU_CHIPS_AFTER_BIT_OP)
+        if control:
+            k = [n for n, _r in after].index("SltChip") + 1
+            after = after[:k] + CONTROL_CHIPS + after[k:]
+        for _name, record in after:
             record(m, c, col)
     # ---------------- LoadStoreChip: lookup structure (load_store.rs:650-685,788-903; 4 bytes x {subtract prev, add cur} = 8 fractions) ----------------
     ram1 = ssum(["IsSb", "IsSh", "IsSw", "IsLb", "IsLh", "IsLbu", "IsLhu", "IsLw"])

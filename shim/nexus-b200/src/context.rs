@@ -133,6 +133,16 @@ impl Context {
         self.check(unsafe { nb200_v1_alu_trace(self.raw(), n_steps, steps.as_ptr(), final_ctr.len(), final_ctr.as_ptr(), log_size, h) })?;
         Ok(out)
     }
+    /// `v1_alu_trace` for a looping program of those instructions and RV32I's branches, JAL, JALR, LUI and AUIPC (the opcode table of
+    /// `nb200_v1_control_trace` in include/nb200.h), with the same step record; `final_ctr` holds each program row's execution count.
+    pub fn v1_control_trace(&self, steps: &[u32], n_steps: usize, final_ctr: &[u32], log_size: u32) -> Result<Columns> {
+        assert_eq!(steps.len(), 13 * n_steps);
+        let mut h = ptr::null_mut();
+        self.check(unsafe { nb200_cols_alloc(self.raw(), 347, log_size, &mut h) })?;
+        let out = Columns { ctx: self.clone(), h };
+        self.check(unsafe { nb200_v1_control_trace(self.raw(), n_steps, steps.as_ptr(), final_ctr.len(), final_ctr.as_ptr(), log_size, h) })?;
+        Ok(out)
+    }
     /// NCCL communicator of this context (one process per GPU): rank 0 calls `comm_unique_id()`, ships the bytes to the other ranks, all call `comm_init`.
     pub fn comm_unique_id() -> Result<Vec<u8>> {
         let mut id = vec![0u8; unsafe { nb200_comm_unique_id_bytes() }];

@@ -85,6 +85,9 @@ extern "C" {
     // ---- the same fill for a program of RV32I's ALU instructions, ADD ... SRAI (out: caller's 347-column batch)
     pub fn nb200_v1_alu_trace(ctx: *mut nb200_ctx, n_steps: usize, steps: *const u32, n_prog: usize, final_ctr: *const u32, log_size: u32,
                               out: *mut nb200_cols) -> c_int;
+    // ---- the same fill for a looping program of those, RV32I's branches, JAL, JALR, LUI and AUIPC (out: caller's 347-column batch)
+    pub fn nb200_v1_control_trace(ctx: *mut nb200_ctx, n_steps: usize, steps: *const u32, n_prog: usize, final_ctr: *const u32, log_size: u32,
+                                  out: *mut nb200_cols) -> c_int;
     // ---- one commitment over N GPUs (NCCL inside the library)
     pub fn nb200_comm_unique_id_bytes() -> usize;
     pub fn nb200_comm_get_unique_id(id_out: *mut u8) -> c_int;

@@ -1,8 +1,10 @@
 """Time GPU proofs of the reference's ADD-chain benchmark as an executing v1 trace (nexus_zkvm_b200/add_chain.py), from host columns and from
 device-filled trees, and time the main trace's device fill (nb200_v1_main_trace).  `--program alu` does the same for add_chain.AluMachine, a
-seeded program of RV32I's 19 ALU instructions (filled by nb200_v1_alu_trace), and writes alu_program_prove.json instead.
+seeded program of RV32I's 19 ALU instructions (filled by nb200_v1_alu_trace), and writes alu_program_prove.json instead; `--program
+control` for add_chain.ControlMachine, a seeded looping program that adds the branches, JAL, JALR, LUI and AUIPC (filled by
+nb200_v1_control_trace), and writes control_program_prove.json.
 
-    python tools/add_chain_prove.py [--program {add-chain,alu}] [--log-sizes 16 18 20] [--steps 3] [--warmup 1] [--fill-calls 20] [--out-dir DIR]
+    python tools/add_chain_prove.py [--program {add-chain,alu,control}] [--log-sizes 16 18 20] [--steps 3] [--warmup 1] [--fill-calls 20] [--out-dir DIR]
 
 For each log size n: AddChainMachine(n), 2^n executed steps and no padding rows.  Two arms alternate step by step after the warm-up: `host`
 proves from the host columns (machine.prove with tree 1 built on the host), `device` from AddChainMachine.device_trees (tree 0 and FinalReg
@@ -32,10 +34,10 @@ def one_size(a, log_size, ctx, backend, stream, pool):
     import torch
 
     from nexus_zkvm_b200 import machine as M
-    from nexus_zkvm_b200.add_chain import AddChainMachine, AluMachine
+    from nexus_zkvm_b200.add_chain import AddChainMachine, AluMachine, ControlMachine
 
     t0 = time.perf_counter()
-    m = AluMachine(log_size) if a.program == "alu" else AddChainMachine(log_size)
+    m = {"alu": AluMachine, "control": ControlMachine, "add-chain": AddChainMachine}[a.program](log_size)
     cols = m.fill_main_trace()
     witness_s = time.perf_counter() - t0
     out_batch = ctx.alloc(347, log_size)
@@ -89,7 +91,7 @@ def one_size(a, log_size, ctx, backend, stream, pool):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--program", choices=["add-chain", "alu"], default="add-chain")
+    ap.add_argument("--program", choices=["add-chain", "alu", "control"], default="add-chain")
     ap.add_argument("--log-sizes", type=int, nargs="+", default=[16, 18, 20])
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
@@ -111,7 +113,10 @@ def main():
     workload = {"add-chain": "AddChainMachine: the reference's ADD-chain benchmark (addi x1,x0,1; add x_k,x_j,x_i), 2^n executed steps, v1 "
                              "main component with DecodingCheck R / I + the eight base extensions",
                 "alu": "AluMachine: alu_program(n, seed=0), 2^n executed steps over RV32I's 19 ALU instructions (ADD ... SRAI), v1 main "
-                       "component with DecodingCheck R / I and SltuChip, SltChip, SllChip, SrlChip, SraChip + the eight base extensions"}
+                       "component with DecodingCheck R / I and SltuChip, SltChip, SllChip, SrlChip, SraChip + the eight base extensions",
+                "control": "ControlMachine: control_program(n, seed=0), a looping program over the 19 ALU instructions and RV32I's branches, "
+                           "JAL, JALR, LUI and AUIPC, 2^n executed steps, v1 main component with DecodingCheck R / I / B / U / J, the ALU "
+                           "chips and the ten control-flow chips + the eight base extensions"}
     out = {
         "workload": workload[a.program],
         "config": dict(pow_bits=5, log_blowup=1, log_last=0, n_queries=3),
@@ -123,7 +128,7 @@ def main():
         "card": card(),
     }
     os.makedirs(a.out_dir, exist_ok=True)
-    name = "alu_program_prove.json" if a.program == "alu" else "add_chain_prove.json"
+    name = {"alu": "alu_program_prove.json", "control": "control_program_prove.json", "add-chain": "add_chain_prove.json"}[a.program]
     with open(os.path.join(a.out_dir, name), "w") as f:
         json.dump(out, f, indent=1)
     print(json.dumps(out))
